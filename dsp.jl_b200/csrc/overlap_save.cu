@@ -24,9 +24,11 @@
 #ifndef DSP_OS_PREFETCH
 #define DSP_OS_PREFETCH 0
 #endif
-// threads of the complex 16384-point kernel: 1024 (one butterfly per thread per pass, 64 registers) or 512 (two, 128 registers)
+// threads of the complex 16384-point kernel: 512 (two butterflies per thread per pass, 128 registers) or 1024 (one, 64
+// registers).  On the H100 the 512-thread kernel is the faster one: 2^26 samples, 4097 taps, H100 80 GB HBM3 at a 400 W
+// power limit, measured alternately in one session -- conv 0.695 .. 0.704 against 0.795 .. 0.801 ms.
 #ifndef DSP_OS_C16K_THREADS
-#define DSP_OS_C16K_THREADS 1024
+#define DSP_OS_C16K_THREADS 512
 #endif
 // default kernel of the 16384-point Float32 plans: 0 = 16 x 16 x 16 x 4 (fft_core.cuh), 1 = 32 x 32 x 16 (fft_r32.cuh).
 // On the H100 the 32 x 32 x 16 kernel is the slower one (its complex instance spills 248 bytes at the 128-register cap):
@@ -92,14 +94,19 @@ template <typename T> struct os_elt<T, true> { using type = cx<T>; };
 // global stores (thread t writes y[t + r N/16]: coalesced).  H is in natural order (the forward transform ends in
 // natural order), pre-scaled by 1/N; thread t reads H[t + r N/16]: coalesced, no tiling needed.
 
-// Launch shape of the fused kernel per size, from a "resident threads" sweep on an earlier GPU generation; only the
-// 16384-point Float32 kernel choice (DSP_OS_R32_DEFAULT) has been measured again on the H100.  On sm_90a the 128-register
-// 8192-point instances spill (Float32 real / complex 260 / 280 bytes, Float64 232 / 240 bytes), so their shape is the
-// next one to re-measure there:
+// Launch shape of the fused kernel per size, from a "resident threads" sweep on an earlier GPU generation; the 16384-point
+// Float32 kernels (DSP_OS_R32_DEFAULT, DSP_OS_C16K_THREADS) have been measured again on the H100.  On sm_90a the
+// 128-register 8192-point instances spill (Float32 real / complex 260 / 280 bytes, Float64 232 / 240 bytes), so their
+// shape is the next one to re-measure there:
 //  * N = 512 .. 4096 (and the real N = 256 kernel): 1024 resident threads per SM under a 64-register cap, one radix-16
 //    butterfly in flight per thread -- the extra warps hide the shared-memory latency (faster than 512 threads with two
 //    butterflies in flight under a 128-register cap);
-//  * complex N = 16384 (one CTA per SM: its shared memory holds one block): 1024 threads, 64-register cap;
+//  * complex N = 16384 (one CTA per SM: its shared memory holds one block): 512 threads, 128 registers, two butterflies in
+//    flight.  The earlier GPU generation ran it faster with 1024 threads under a 64-register cap; on the H100 that build
+//    takes 14 % longer and spills 20 / 36 bytes (512 threads: 16 / 16 bytes).  Splitting the block over a two-CTA cluster so
+//    that two 512-thread, 64-register CTAs share each SM does not pay there either: a 512-thread, 64-register 8192-point
+//    kernel at two CTAs per SM costs 0.43 of a 16384-point unit per unit (0.46 with the store count of half a
+//    16384-point block; transform length alone gives 0.46 .. 0.5), which leaves no room for the exchange;
 //  * N = 8192, real N = 16384: 512 resident threads, 128 registers, two butterflies in flight (the 64-register
 //    build spilled there when the shape was chosen).  Double precision: one CTA of up to 256 registers per thread.
 template <typename T, int N, bool CPLX> struct os_threads {
