@@ -17,6 +17,15 @@ __device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
+// expect `bytes` more in the current phase without arriving: a phase fed by several copies issued at different times
+// posts this for all but the last one, then mbar_expect_tx
+__device__ __forceinline__ void mbar_expect_tx_noarrive(uint64_t* bar, uint32_t bytes) {
+    asm volatile("mbarrier.expect_tx.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+
+// order the CTA's earlier generic-proxy accesses of shared memory (made visible to this thread by a barrier) before the
+// async-proxy writes of a bulk copy issued after it: a buffer that was just read can be refilled by TMA
+__device__ __forceinline__ void fence_proxy_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // one elected thread: bytes must be a multiple of 16, src and dst 16-byte aligned
 __device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {

@@ -24,7 +24,8 @@
 #define DSP_FFT_GATE 1
 #endif
 // timing probes (wrong results, never in the shipped library): bit 0 skips the stride-256 passes, bit 1 replaces the
-// first-pass global loads by constants, bit 2 the H loads, bit 3 drops the global stores, bit 4 skips the stride-16 passes
+// first-pass global loads by constants (and turns the overlap-save kernels' TMA staging off: no input is read at all),
+// bit 2 the H loads, bit 3 drops the global stores, bit 4 skips the stride-16 passes
 #ifndef DSP_PROBE
 #define DSP_PROBE 0
 #endif
@@ -419,8 +420,10 @@ __host__ __device__ __forceinline__ void fft_first_pass(const FftCtx<T>& c, int 
     }
 }
 
-// First pass on operands that are already in registers (v[it][r] = sample tid + it NT + r N/16): the overlap-save kernel
-// loads the next unit's samples before the previous unit's last pass, so the L2 -> SM transfer overlaps that pass.
+// First pass on operands that are already in registers (v[it][r] = sample tid + it NT + r N/16).  With SYNC the barrier
+// after the first butterfly orders every thread's reads before any store, so the operands may come from the data buffer
+// itself: the 16384-point overlap-save kernel reads its TMA-staged input (natural order, from a region in front of the data
+// buffer on into the buffer's first bytes) into registers and stores the padded layout over it.
 template <typename T, int N, int NT, bool SYNC, int ITERS, class Scope = FftCtaScope>
 __device__ __forceinline__ void fft_first_pass_regs(const FftCtx<T>& c, int tid, cx<T> (&v)[ITERS][16], Scope sc = Scope()) {
     constexpr int Q = fft_plan_traits<N>::Q;
@@ -505,19 +508,21 @@ __device__ __forceinline__ void fft_middle(const FftCtx<T>& c, int tid, Scope sc
     }
 }
 
-// Last pass of thread unit tp = tid + it * NT < N/16: on return v[r] = X[tp + r N/16].
-template <typename T, int N, int GATE_NT = 0>
-__host__ __device__ __forceinline__ void fft_last_pass(const FftCtx<T>& c, int tp, cx<T> (&v)[16], int tid = 0) {
+// Last pass of thread unit tp = tid + it * NT < N/16 in two halves: fft_last_pass_load reads its 16 operands from the
+// data buffer, fft_last_pass_bfly transforms them (twiddles from the tables only), so that a caller can hand the data
+// buffer on between the two.  fft_last_pass does both: on return v[r] = X[tp + r N/16].
+template <typename T, int N>
+__host__ __device__ __forceinline__ void fft_last_pass_load(const FftCtx<T>& c, int tp, cx<T> (&v)[16]) {
+    constexpr int Q = fft_plan_traits<N>::Q;
+    // padaddr(tp + r Q) = padaddr(tp) + padaddr(r Q): tp < Q never carries into the bits of r Q (compile-time offsets)
+    const cx<T>* p = c.sm + padaddr<T, N>(tp);
+#pragma unroll
+    for (int r = 0; r < 16; ++r) v[r] = p[padaddr<T, N>(r * Q)];
+}
+template <typename T, int N>
+__host__ __device__ __forceinline__ void fft_last_pass_bfly(const FftCtx<T>& c, int tp, cx<T> (&v)[16]) {
     using P = fft_plan_traits<N>;
     constexpr int Q = P::Q, RL = P::RL;
-    if constexpr (GATE_NT > 256) fft_gate_wait<GATE_NT>(tid);
-    {
-        // padaddr(tp + r Q) = padaddr(tp) + padaddr(r Q): tp < Q never carries into the bits of r Q (compile-time offsets)
-        const cx<T>* p = c.sm + padaddr<T, N>(tp);
-#pragma unroll
-        for (int r = 0; r < 16; ++r) v[r] = p[padaddr<T, N>(r * Q)];
-    }
-    if constexpr (GATE_NT > 256) fft_gate_open<GATE_NT>(tid);
     if constexpr (RL == 16) {
         cx<T> w[8];
         load_tw8<T, Q, fft_tw_row(N)>(Q == 16 ? c.t16 : c.t256, tp, w);
@@ -546,10 +551,17 @@ __host__ __device__ __forceinline__ void fft_last_pass(const FftCtx<T>& c, int t
         }
     }
 }
+template <typename T, int N, int GATE_NT = 0>
+__host__ __device__ __forceinline__ void fft_last_pass(const FftCtx<T>& c, int tp, cx<T> (&v)[16], int tid = 0) {
+    if constexpr (GATE_NT > 256) fft_gate_wait<GATE_NT>(tid);
+    fft_last_pass_load<T, N>(c, tp, v);
+    if constexpr (GATE_NT > 256) fft_gate_open<GATE_NT>(tid);
+    fft_last_pass_bfly<T, N>(c, tp, v);
+}
 
 // The last pass in chunks of one butterfly (a radix below 16 gives a thread 16/RL butterflies): chunk a leaves
 // u[j] = X[tp + (a + (16/RL) j) N/16], j < RL.  Lets a consumer that streams its outputs away (global stores) keep only RL
-// values live at a time -- the overlap-save kernel holds the next unit's 16 prefetched samples in registers meanwhile.
+// values live at a time.
 template <int N> struct fft_last_chunks {
     static constexpr int RL = fft_plan_traits<N>::RL;
     static constexpr int COUNT = 16 / RL;                 // 1 when the last pass is a radix-16 pass
