@@ -128,10 +128,9 @@ static inline int64_t cdiv(int64_t a, int64_t b) { return (a + b - 1) / b; }
 // overlap-save) are launched with programmatic stream serialisation: a kernel's CTAs may become resident as soon as the
 // previous kernel's CTAs leave an SM, stage their twiddle tables / window (constants since plan creation) and then block
 // in `pdl_wait()` until the previous grid has completed and its memory is visible -- the launch gap and the table prologue
-// (68 KB per CTA for the 16384-point kernel) overlap the previous kernel's tail instead of following it.  EVERY thread
-// executes pdl_wait() before its first access to anything a preceding kernel could have written or still be reading, so
-// the chain is transitive.  Without the launch attribute both instructions are no-ops.  DSPB200_PDL=0 turns it off.
-bool pdl_enabled();
+// (49 KB per CTA for the 16384-point Float32 kernel) overlap the previous kernel's tail instead of following it.  EVERY
+// thread executes pdl_wait() before its first access to anything a preceding kernel could have written or still be
+// reading, so the chain is transitive.  Kernels launched without the attribute execute both instructions as no-ops.
 #ifdef __CUDACC__
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -144,7 +143,7 @@ static inline cudaError_t launch_pdl(void (*kern)(KA...), unsigned grid, unsigne
     cfg.stream = st;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at;
     cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kern, KA(args)...);

@@ -19,19 +19,11 @@
 #include "common.cuh"
 #include <math.h>
 
-// wave-gated shared-memory loads after CTA-wide barriers (see fft_gate_wait); 0 switches it off for A/B timing
-#ifndef DSP_FFT_GATE
-#define DSP_FFT_GATE 1
-#endif
 // timing probes (wrong results, never in the shipped library): bit 0 skips the stride-256 passes, bit 1 replaces the
 // first-pass global loads by constants (and turns the overlap-save kernels' TMA staging off: no input is read at all),
 // bit 2 the H loads, bit 3 drops the global stores, bit 4 skips the stride-16 passes
 #ifndef DSP_PROBE
 #define DSP_PROBE 0
-#endif
-// last-pass twiddle table of the 512- / 1024- / 2048-point Float32 transforms in shared memory (1) or global memory via L1 (0)
-#ifndef DSP_TL_SMEM_SMALL
-#define DSP_TL_SMEM_SMALL 1
 #endif
 
 namespace dspb200 {
@@ -239,7 +231,7 @@ template <typename T> struct FftCtx {
 
 template <typename T, int N> __host__ __device__ constexpr bool fft_tl_in_smem() {
     // 16384: W_N^t alone, 32 KB; 512 / 1024 / 2048: the whole last-pass table, 2 / 4 / 8 KB (several CTAs per SM still fit)
-    return sizeof(T) == 4 && (N == 16384 || DSP_TL_SMEM_SMALL && (N == 512 || N == 1024 || N == 2048));
+    return sizeof(T) == 4 && (N == 16384 || N == 512 || N == 1024 || N == 2048);
 }
 template <int N> __host__ __device__ constexpr int fft_tl_len() { return (N / fft_plan_traits<N>::RL) * fft_plan_traits<N>::TLK; }
 template <int N> __host__ __device__ constexpr bool fft_uses_t16() { return N >= 256; }
@@ -496,7 +488,7 @@ __device__ __forceinline__ void fft_middle(const FftCtx<T>& c, int tid, Scope sc
     static_assert(NMID < 2 || std::is_same<Scope, FftCtaScope>::value, "thread groups run transforms of at most 4096 points");
     if constexpr (NMID >= 1) {
 #if !(DSP_PROBE & 16)
-        fft_pass16<T, N, NT, 16, DSP_FFT_GATE != 0>(c, tid);
+        fft_pass16<T, N, NT, 16, true>(c, tid);
 #endif
         if constexpr (NMID == 2) {
             fft_group256_sync<NT>(tid);

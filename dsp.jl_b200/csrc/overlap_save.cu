@@ -10,41 +10,12 @@
 // Each sample is read once and written once from/to HBM; the nv-1 halo re-read comes from L2.  Real signals ride two blocks per complex FFT (z = a + i b; h real => y = a*h + i b*h).
 // H carries the 1/nfft of the unnormalised inverse (src/dspbase.jl:516, src/Filters/filt.jl:498).
 #include "fft_core.cuh"
-#include "fft_r32.cuh"
 #include "async_copy.cuh"
 #include <cufft.h>
 #include <math.h>
 #include <stdlib.h>
 #include <new>
 #include <vector>
-
-// threads of the complex 16384-point kernel: 512 (two butterflies per thread per pass, 128 registers) or 1024 (one, 64
-// registers).  On the H100 the 512-thread kernel is the faster one: 2^26 samples, 4097 taps, H100 80 GB HBM3 at a 400 W
-// power limit, measured alternately in one session -- conv 0.695 .. 0.704 against 0.795 .. 0.801 ms.
-#ifndef DSP_OS_C16K_THREADS
-#define DSP_OS_C16K_THREADS 512
-#endif
-// default kernel of the 16384-point Float32 plans: 0 = 16 x 16 x 16 x 4 (fft_core.cuh), 1 = 32 x 32 x 16 (fft_r32.cuh).
-// On the H100 the 32 x 32 x 16 kernel is the slower one (its complex instance spills 248 bytes at the 128-register cap):
-// 2^26 samples, 4097 taps, H100 SXM 80 GB -- ComplexF32 0.85 against 0.78 ms at a 700 W power limit, real Float32 0.435
-// against 0.387 ms at 400 W.
-#ifndef DSP_OS_R32_DEFAULT
-#define DSP_OS_R32_DEFAULT 0
-#endif
-// load gating of the 32 x 32 x 16 kernel: bits 0-1 middle passes, bits 2-3 the fused bracket, bits 4-5 the final last pass
-// (off: two waves of 8 warps do not need it)
-#ifndef DSP_R32_GATE
-#define DSP_R32_GATE 0
-#endif
-// samples (of 32) of the next unit's first-pass butterfly loaded into registers before the current unit's last pass
-// (8 / 16 / 24 all spill at 128 registers per thread: the prefetched values end up in local memory; off)
-// request the filter spectrum before the last-pass butterflies of the fused bracket (1) or after them (0)
-#ifndef DSP_R32_HEARLY
-#define DSP_R32_HEARLY 0
-#endif
-#ifndef DSP_R32_PREFETCH
-#define DSP_R32_PREFETCH 0
-#endif
 
 namespace dspb200 {
 
@@ -59,8 +30,6 @@ struct OsPlanImpl {
     void* d_t256 = nullptr;
     int sm_count = 0;               // device_sm_count() at plan creation
     int fused_per_sm = 0;   // resident CTAs per SM of this plan's fused kernel (occupancy calculator, asked once)
-    void* d_t32 = nullptr;  // 16384-point Float32 plans: tables of the 32 x 32 x 16 kernel (fft_r32.cuh)
-    void* d_t1024 = nullptr;
     void* d_H = nullptr;    // natural order; fused: cx<T>[nfft] pre-scaled by 1/nfft; generic: nfft or nfft/2+1 bins
     // generic
     cufftHandle fwd = 0, inv = 0;
@@ -95,16 +64,16 @@ template <typename T> struct os_elt<T, true> { using type = cx<T>; };
 // stores 0.543 .. 0.546.
 
 // Launch shape of the fused kernel per size, from a "resident threads" sweep on an earlier GPU generation; the 16384-point
-// Float32 kernels (DSP_OS_R32_DEFAULT, DSP_OS_C16K_THREADS) have been measured again on the H100.  On sm_90a the
-// 128-register 8192-point instances spill (Float32 real / complex 260 / 280 bytes, Float64 232 / 240 bytes), so their
-// shape is the next one to re-measure there:
+// Float32 kernels have been measured again on the H100.  On sm_90a the 128-register 8192-point instances spill (Float32
+// real / complex 260 / 280 bytes, Float64 232 / 240 bytes), so their shape is the next one to re-measure there:
 //  * N = 512 .. 4096 (and the real N = 256 kernel): 1024 resident threads per SM under a 64-register cap, one radix-16
 //    butterfly in flight per thread -- the extra warps hide the shared-memory latency (faster than 512 threads with two
 //    butterflies in flight under a 128-register cap);
 //  * complex N = 16384 (one CTA per SM: its shared memory holds one block): 512 threads, 128 registers, two butterflies in
-//    flight.  The earlier GPU generation ran it faster with 1024 threads under a 64-register cap; on the H100 that build
-//    takes 14 % longer and spills 20 / 36 bytes (512 threads: 16 / 16 bytes).  Splitting the block over a two-CTA cluster so
-//    that two 512-thread, 64-register CTAs share each SM does not pay there either: a 512-thread, 64-register 8192-point
+//    flight: on the H100 it is faster than 1024 threads with one butterfly each under a 64-register cap, the earlier
+//    generation's choice (2^26 samples, 4097 taps, H100 80 GB HBM3 at 400 W, alternating: conv 0.695 .. 0.704 against
+//    0.795 .. 0.801 ms).  Splitting the block over a two-CTA cluster so that two 512-thread, 64-register CTAs share each
+//    SM does not pay there either: a 512-thread, 64-register 8192-point
 //    kernel at two CTAs per SM costs 0.43 of a 16384-point unit per unit (0.46 with the store count of half a
 //    16384-point block; transform length alone gives 0.46 .. 0.5), which leaves no room for the exchange.  Its next unit's
 //    input is staged by TMA (OsStage), and the last pass reads both butterflies' operands before any math (the copy may
@@ -113,12 +82,12 @@ template <typename T> struct os_elt<T, true> { using type = cx<T>; };
 //    build spilled there when the shape was chosen).  Double precision: one CTA of up to 256 registers per thread.
 template <typename T, int N, bool CPLX> struct os_threads {
     static constexpr bool f32 = sizeof(T) == 4;
-    static constexpr int value = (f32 && N == 16384 && CPLX) ? DSP_OS_C16K_THREADS : fft_threads<N>::value;
+    static constexpr int value = fft_threads<N>::value;
     static constexpr bool wide = f32 && ((N >= 512 && N <= 4096) || (N == 256 && !CPLX));     // 1024 resident threads
-    static constexpr int minblocks = value == 1024 ? 1 : (wide ? 1024 / value : fft_minblocks<T, N>::value);
+    static constexpr int minblocks = wide ? 1024 / value : fft_minblocks<T, N>::value;
     // the 16384-point Float32 kernels at 512 threads (two butterflies per thread in every pass): the next unit's input is
     // staged in shared memory by TMA while the current one runs (OsStage)
-    static constexpr bool staged = f32 && N == 16384 && N / 16 == 2 * value;
+    static constexpr bool staged = f32 && N == 16384;
 };
 // Staged kernels: the first OS_STAGE_HEAD bytes of a unit's span land in a region of their own right in front of the data
 // buffer (32 KB of the 33 KB the 16384-point block leaves free), the rest at the data buffer's head -- contiguous, so the
@@ -243,7 +212,7 @@ __device__ __forceinline__ void os_unit(const FftCtx<T>& ctx, int tid, const OsU
     for (int it = 0; it < ITERS; ++it) {
         const int tp = tid + it * NT;
         if (Q % NT == 0 || tp < Q) {
-            fft_last_pass<T, N, (DSP_FFT_GATE && ITERS == 1 && Q % NT == 0) ? NT : 0>(ctx, tp, v[it], tid);
+            fft_last_pass<T, N, (ITERS == 1 && Q % NT == 0) ? NT : 0>(ctx, tp, v[it], tid);
 #pragma unroll
 #if DSP_PROBE & 4
             for (int r = 0; r < 16; ++r) v[it][r] = cswap(cmul(v[it][r], mkc<T>(T(0.5), T(r))));
@@ -284,9 +253,8 @@ __device__ __forceinline__ void os_unit(const FftCtx<T>& ctx, int tid, const OsU
     };
     // Last pass.  Staged kernels: every thread reads the operands of both of its butterflies, then -- one barrier later,
     // when nobody reads the data buffer any more -- one thread issues the copy of the rest of the next unit's span into it,
-    // and the butterflies and the global stores run while the copy is in flight.  The 1024-thread kernel (one butterfly per thread, 64 registers)
-    // loads all 16 inputs behind the load gate and stores 16 outputs; the other kernels stream it one radix-RL butterfly at
-    // a time -- RL live values instead of 16
+    // and the butterflies and the global stores run while the copy is in flight.  The other kernels stream it one radix-RL
+    // butterfly at a time -- RL live values instead of 16
     if constexpr (STAGED) {
         cx<T> w[ITERS][16];
 #pragma unroll
@@ -307,10 +275,6 @@ __device__ __forceinline__ void os_unit(const FftCtx<T>& ctx, int tid, const OsU
 #pragma unroll
             for (int r = 0; r < 16; ++r) put(tp + r * Q, w[it][r]);
         }
-    } else if constexpr (ITERS == 1 && Q % NT == 0 && NT >= 1024) {
-        fft_last_pass<T, N, DSP_FFT_GATE ? NT : 0>(ctx, tid, v[0], tid);
-#pragma unroll
-        for (int r = 0; r < 16; ++r) put(tid + r * Q, v[0][r]);
     } else {
         auto chunk = [&](auto a_, int tp) {
             constexpr int A = decltype(a_)::value;
@@ -432,165 +396,6 @@ os_fused_kernel(const void* __restrict__ u_, int64_t u_begin, int64_t nu_local, 
         if (interior) os_unit<T, N, CPLX, NT, true, ITERS>(ctx, tid, g, H, st, staged, next_u);
         else os_unit<T, N, CPLX, NT, false, ITERS>(ctx, tid, g, H, st, staged, next_u);
         staged = next_u != nullptr;
-    }
-}
-
-// ---------------------------------------------------------------------------------------------- 32 x 32 x 16 kernel
-// The 16384-point Float32 block as 32 x 32 x 16 (fft_r32.cuh): 512 threads, one radix-32 butterfly per thread in the first
-// and the middle pass, two radix-16 butterflies in the last one.  Same unit geometry, same H, same results up to rounding.
-// `pre` / `have_pre`: the first DSP_R32_PREFETCH samples of this thread's first-pass butterfly, loaded by the PREVIOUS unit
-// right before its last pass (next_u: slot 0 of the next unit when that unit is interior, else null) so that part of the
-// L2 -> SM transfer overlaps that pass.
-template <typename T, bool CPLX, bool INTERIOR>
-__device__ __forceinline__ void os_unit32(const r32::Ctx<T>& ctx, int tid, const OsUnit<typename os_elt<T, CPLX>::type>& g,
-                                          const cx<T>* __restrict__ H, cx<T> (&pre)[DSP_R32_PREFETCH > 0 ? DSP_R32_PREFETCH : 1],
-                                          bool have_pre, const typename os_elt<T, CPLX>::type* __restrict__ next_u) {
-    constexpr int PF = DSP_R32_PREFETCH;
-    cx<T> v[32];
-    if (PF > 0 && have_pre) {
-#pragma unroll
-        for (int r = 0; r < 32; ++r) v[r] = r < PF ? pre[r < PF ? r : 0] : os_sample<T, CPLX, INTERIOR>(g, tid + r * r32::Q32);
-    } else {
-#pragma unroll
-        for (int r = 0; r < 32; ++r) v[r] = os_sample<T, CPLX, INTERIOR>(g, tid + r * r32::Q32);
-    }
-    fft_bfly<T, 32, true>(v, nullptr);
-    __syncthreads();                                   // the previous unit's last pass has read the buffer
-    r32::store_block<T>(ctx.sm, tid, v);
-    __syncthreads();
-    r32::middle_pass<T, DSP_R32_GATE & 3>(ctx, tid);
-    __syncthreads();
-    {
-        // last forward pass of the butterflies tid and tid + 512, x H, swap: together they hold Y[tid + 512 m], m < 32,
-        // the inputs of the plain first-pass butterfly of residue class tid of the second transform
-        cx<T> a[16], b[16];
-#if DSP_R32_HEARLY
-        // H of the first butterfly is requested before its shared-memory loads, H of the second before the second's: the L2
-        // latency of the 32 filter-spectrum loads hides behind the two butterflies instead of following them
-        cx<T> h[16];
-#pragma unroll
-        for (int r = 0; r < 16; ++r) h[r] = ldg_cx<T>(H + tid + r * r32::Q16);
-        r32::last_pass<T>(ctx, tid, a, tid);
-#pragma unroll
-        for (int r = 0; r < 16; ++r) v[2 * r] = cswap(cmul(a[r], h[r]));
-#pragma unroll
-        for (int r = 0; r < 16; ++r) h[r] = ldg_cx<T>(H + tid + r32::Q32 + r * r32::Q16);
-        r32::last_pass<T>(ctx, tid + r32::Q32, b, tid);
-#pragma unroll
-        for (int r = 0; r < 16; ++r) v[2 * r + 1] = cswap(cmul(b[r], h[r]));
-#else
-        r32::last_pass<T, (DSP_R32_GATE >> 2) & 1>(ctx, tid, a, tid);
-        r32::last_pass<T, (DSP_R32_GATE >> 2) & 2>(ctx, tid + r32::Q32, b, tid);
-#pragma unroll
-        for (int r = 0; r < 16; ++r) {
-            v[2 * r] = cswap(cmul(a[r], ldg_cx<T>(H + tid + r * r32::Q16)));
-            v[2 * r + 1] = cswap(cmul(b[r], ldg_cx<T>(H + tid + r32::Q32 + r * r32::Q16)));
-        }
-#endif
-    }
-    fft_bfly<T, 32, true>(v, nullptr);
-    __syncthreads();                                   // every thread has read its last-pass inputs
-    r32::store_block<T>(ctx.sm, tid, v);
-    __syncthreads();
-    r32::middle_pass<T, DSP_R32_GATE & 3>(ctx, tid);
-    __syncthreads();
-    if (PF > 0 && next_u != nullptr) {
-        OsUnit<typename os_elt<T, CPLX>::type> gn;
-        gn.u = next_u;
-        gn.L = g.L;
-#pragma unroll
-        for (int r = 0; r < PF; ++r) pre[r] = os_sample<T, CPLX, true>(gn, tid + r * r32::Q32);
-    }
-#pragma unroll
-    for (int it = 0; it < 2; ++it) {
-        const int tp = tid + it * r32::Q32;
-        cx<T> y[16];
-        if (it == 0) r32::last_pass<T, (DSP_R32_GATE >> 4) & 3>(ctx, tp, y, tid);
-        else r32::last_pass<T>(ctx, tp, y);
-#pragma unroll
-        for (int r = 0; r < 16; ++r) {
-            const int j = tp + r * r32::Q16;
-            if (j < g.nvm1) continue;
-            if constexpr (CPLX) {                      // swapped domain: result = (y.y, y.x)
-                if constexpr (INTERIOR) g.out[j] = mkc<T>(y[r].y, y[r].x);
-                else if (j < g.jend) g.out[j] = (j < g.jzero) ? mkc<T>(y[r].y, y[r].x) : mkc<T>(T(0), T(0));
-            } else {
-                const int jb = j + g.L;
-                if constexpr (INTERIOR) {
-                    g.out[j] = y[r].y;
-                    g.out[jb] = y[r].x;
-                } else {
-                    if (j < g.jend) g.out[j] = (j < g.jzero) ? y[r].y : T(0);
-                    if (jb < g.jend) g.out[jb] = (jb < g.jzero) ? y[r].x : T(0);
-                }
-            }
-        }
-    }
-}
-
-template <typename T, bool CPLX>
-__global__ void __launch_bounds__(r32::NT, 1)
-os_fused32_kernel(const void* __restrict__ u_, int64_t u_begin, int64_t nu_local, int64_t u_col_stride,
-                  void* __restrict__ out_, int64_t out_begin, int64_t out_count, int64_t out_col_stride,
-                  int64_t zero_from, int nv, int64_t units_per_col, int64_t total_units, const cx<T>* __restrict__ g32,
-                  const cx<T>* __restrict__ g1024, const cx<T>* __restrict__ H) {
-    constexpr int N = r32::N;
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    using E = typename os_elt<T, CPLX>::type;
-    const int tid = threadIdx.x;
-    pdl_launch_dependents();
-    const r32::Ctx<T> ctx = r32::make_ctx<T>(reinterpret_cast<cx<T>*>(smem_raw), g32, g1024, tid);
-    pdl_wait();                                        // tables staged; from here on data of preceding kernels is touched
-    __syncthreads();
-    const int L = N - nv + 1;
-    const int span = CPLX ? N : N + L;
-    const bool onecol = units_per_col >= total_units;
-    cx<T> pre[DSP_R32_PREFETCH > 0 ? DSP_R32_PREFETCH : 1];
-    bool have_pre = false;
-    for (int64_t gu = blockIdx.x; gu < total_units; gu += gridDim.x) {
-        const int64_t col = onecol ? 0 : gu / units_per_col;
-        const int64_t unit = gu - col * units_per_col;
-        const int64_t q = CPLX ? unit : 2 * unit;
-        const int64_t s0 = out_begin + q * L - (nv - 1);
-        const int64_t i0 = s0 - u_begin;
-        OsUnit<E> g;
-        g.u = reinterpret_cast<const E*>(u_) + col * u_col_stride + i0;
-        g.out = reinterpret_cast<E*>(out_) + col * out_col_stride + (s0 - out_begin);
-        g.jlo = os_clamp(-i0);
-        g.jhi = os_clamp(nu_local - i0);
-        g.jend = os_clamp(out_begin + out_count - s0);
-        g.jzero = os_clamp_diff(zero_from, s0);
-        g.nvm1 = nv - 1;
-        g.L = L;
-        const bool interior = g.jlo <= 0 && g.jhi >= span && g.jend >= span && g.jzero >= span;
-        // pull the input range of this CTA's next unit into L2 while this one computes
-        if (tid == 0 && gu + gridDim.x < total_units) {
-            const int64_t gn = gu + gridDim.x;
-            const int64_t coln = onecol ? 0 : gn / units_per_col;
-            const int64_t qn = (CPLX ? 1 : 2) * (gn - coln * units_per_col);
-            int64_t lo = out_begin + qn * L - (nv - 1) - u_begin;
-            int64_t hi = lo + span;
-            if (lo < 0) lo = 0;
-            if (hi > nu_local) hi = nu_local;
-            const uintptr_t a0 = ((uintptr_t)(reinterpret_cast<const E*>(u_) + coln * u_col_stride + lo) + 15) & ~(uintptr_t)15;
-            const uintptr_t a1 = (uintptr_t)(reinterpret_cast<const E*>(u_) + coln * u_col_stride + hi) & ~(uintptr_t)15;
-            if (hi > lo && a1 > a0) tma_prefetch_l2(reinterpret_cast<const void*>(a0), (uint32_t)(a1 - a0));
-        }
-        // the next unit's samples are prefetched by this one iff that unit is interior (same column: slot 0 is L (2L) further)
-        const E* next_u = nullptr;
-        if (DSP_R32_PREFETCH > 0 && gu + gridDim.x < total_units) {
-            const int64_t gn = gu + gridDim.x;
-            const int64_t coln = onecol ? 0 : gn / units_per_col;
-            const int64_t qn = (CPLX ? 1 : 2) * (gn - coln * units_per_col);
-            const int64_t s0n = out_begin + qn * L - (nv - 1);
-            const int64_t i0n = s0n - u_begin;
-            const bool inn = i0n >= 0 && i0n + span <= nu_local && out_begin + out_count - s0n >= span &&
-                             os_clamp_diff(zero_from, s0n) >= span;
-            if (inn) next_u = reinterpret_cast<const E*>(u_) + coln * u_col_stride + i0n;
-        }
-        if (interior) os_unit32<T, CPLX, true>(ctx, tid, g, H, pre, have_pre, next_u);
-        else os_unit32<T, CPLX, false>(ctx, tid, g, H, pre, have_pre, next_u);
-        have_pre = next_u != nullptr;
     }
 }
 
@@ -811,9 +616,7 @@ __global__ void conv_direct_kernel(const void* __restrict__ large_, int64_t nl, 
 }
 
 // ---------------------------------------------------------------------------------------------- dispatch
-#ifndef DSP_OS_SIZES   // (override on the command line to build a single size while tuning)
 #define DSP_OS_SIZES(X) X(32) X(64) X(128) X(256) X(512) X(1024) X(2048) X(4096) X(8192) X(16384)
-#endif
 
 static bool os_fused_ok(int64_t nfft, int64_t nv, bool f64) {
     if (nfft < 32 || (nfft & (nfft - 1))) return false;
@@ -859,37 +662,7 @@ static int launch_os_fused(OsPlanImpl* p, const OsRange& a, cudaStream_t st) {
     return DSPB200_OK;
 }
 
-// which kernel runs a 16384-point Float32 plan: DSPB200_OS_R32 = 0 / 1 forces the 16x16x16x4 / 32x32x16 kernel
-static bool os_use_r32(bool cplx) {
-    if (const char* e = getenv("DSPB200_OS_R32")) return e[0] == '1';
-    (void)cplx;
-    return DSP_OS_R32_DEFAULT != 0;
-}
-
-template <bool CPLX>
-static int launch_os_fused32(OsPlanImpl* p, const OsRange& a, cudaStream_t st) {
-    const size_t smem = (size_t)r32::smem_elems<float>() * sizeof(cx<float>);
-    auto kern = os_fused32_kernel<float, CPLX>;
-    const int64_t nblk = cdiv(a.out_count, p->L);
-    const int64_t upc = CPLX ? nblk : (nblk + 1) / 2;
-    const int64_t units = upc * a.ncols;
-    if (units < 1) return DSPB200_OK;
-    DSP_TRY(set_smem(kern, smem));
-    const int64_t cap = p->sm_count;                               // one CTA per SM (213 KB of shared memory)
-    const int64_t blocks = units < cap ? units : cap;
-    DSP_CUDA(launch_pdl(kern, (unsigned)blocks, r32::NT, smem, st, a.u, a.u_begin, a.nu_local, a.u_col_stride, a.out,
-                        a.out_begin, a.out_count, a.out_col_stride, a.zero_from, (int)p->nv, upc, units,
-                        reinterpret_cast<const cx<float>*>(p->d_t32), reinterpret_cast<const cx<float>*>(p->d_t1024),
-                        reinterpret_cast<const cx<float>*>(p->d_H)));
-    DSP_LAUNCH_OK();
-    return DSPB200_OK;
-}
-
 template <typename T> static int os_fused_dispatch(OsPlanImpl* p, const OsRange& a, cudaStream_t st) {
-    if constexpr (sizeof(T) == 4) {
-        if (p->nfft == 16384 && p->d_t32 != nullptr && os_use_r32(p->cplx))
-            return p->cplx ? launch_os_fused32<true>(p, a, st) : launch_os_fused32<false>(p, a, st);
-    }
     switch (p->nfft) {
 #define X(NN)                                                                                   \
     case NN:                                                                                    \
@@ -1255,14 +1028,6 @@ int dspb200_os_plan_create(dspb200_os_plan** plan, int dtype, const void* v_host
             if (e == cudaSuccess) e = cudaMalloc(&p->d_t256, t256.size());
             if (e == cudaSuccess) e = cudaMemcpy(p->d_t256, t256.data(), t256.size(), cudaMemcpyHostToDevice);
             if (e == cudaSuccess) e = cudaMalloc(&p->d_H, (size_t)p->nfft * csz);
-            if (e == cudaSuccess && !p->f64 && p->nfft == 16384) {             // tables of the 32 x 32 x 16 kernel
-                std::vector<cx<float>> a32(r32::T32_LEN), a1024(r32::T1024_LEN);
-                r32::fill_tables<float>(a32.data(), a1024.data());
-                e = cudaMalloc(&p->d_t32, a32.size() * sizeof(cx<float>));
-                if (e == cudaSuccess) e = cudaMemcpy(p->d_t32, a32.data(), a32.size() * sizeof(cx<float>), cudaMemcpyHostToDevice);
-                if (e == cudaSuccess) e = cudaMalloc(&p->d_t1024, a1024.size() * sizeof(cx<float>));
-                if (e == cudaSuccess) e = cudaMemcpy(p->d_t1024, a1024.data(), a1024.size() * sizeof(cx<float>), cudaMemcpyHostToDevice);
-            }
             if (e != cudaSuccess) { rc = cuda_fail(e, "twiddle upload", __FILE__, __LINE__); break; }
             rc = p->f64 ? os_filter_dispatch<double>(p, d_v) : os_filter_dispatch<float>(p, d_v);
         } else {
@@ -1404,8 +1169,6 @@ int dspb200_os_plan_destroy(dspb200_os_plan* plan) {
     if (p->d_tw) cudaFree(p->d_tw);
     if (p->d_t16) cudaFree(p->d_t16);
     if (p->d_t256) cudaFree(p->d_t256);
-    if (p->d_t32) cudaFree(p->d_t32);
-    if (p->d_t1024) cudaFree(p->d_t1024);
     if (p->d_H) cudaFree(p->d_H);
     if (p->fft_ok) { cufftDestroy(p->fwd); cufftDestroy(p->inv); }
     p->td.release(); p->fd.release();

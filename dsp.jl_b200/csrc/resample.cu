@@ -16,11 +16,6 @@
 #include <new>
 #include <vector>
 
-// outputs per phase per thread of the multi-phase kernel, Float32 arithmetic (register tile)
-#ifndef DSP_RS_G32
-#define DSP_RS_G32 4
-#endif
-
 namespace dspb200 {
 
 constexpr int RS_NT = 256;
@@ -266,27 +261,20 @@ resample_mp_kernel(const EX* __restrict__ x, int64_t x_begin, int64_t nx_local, 
 //     shared-memory stores (long-scoreboard, 20 % of the samples) is off the critical path;
 //   * two CTA-wide barriers per tile instead of three, no per-tile tap staging.
 // Edge tiles (samples outside the stored range are zero) are filled synchronously with the bounds test.
-#ifndef DSP_RS_HQ
-#define DSP_RS_HQ 1
-#endif
-// DSP_RS_V3 (default): what the profile of the version above (far fewer FFMA among the executed instructions than in a
-// chunk) showed outside the chunks --
-//   * the tap rows are staged ONCE per persistent CTA in shared memory and read with 128-bit broadcast loads (6 per chunk
-//     for 3 phases instead of 24 uniform constant loads), which also lets the chunk loop stay ROLLED: two copies of the chunk
-//     body (unchecked, and the checked one for the last chunk's padding taps) instead of eight with a uniform branch per tap
-//     (97 KB of code);
-//   * interior tiles are copied out without the 64-bit bounds tests; single-column launches skip the 64-bit division per tile.
-// Same products in the same order: bit-identical to DSP_RS_V3 = 0 (build target rsv0 for the A/B).
-#ifndef DSP_RS_V3
-#define DSP_RS_V3 1
-#endif
+// Interior tiles are copied out without the 64-bit bounds tests; single-column launches skip the 64-bit division per tile.
+// V3 instances (rs_v3) also stage the tap rows ONCE per persistent CTA in shared memory, where the profile of the
+// constant-bank version showed far fewer FFMA among the executed instructions than in a chunk: the rows are read with
+// 128-bit broadcast loads (6 per chunk for 3 phases instead of 24 uniform constant loads), which also lets the chunk loop
+// stay ROLLED -- two copies of the chunk body (unchecked, and the checked one for the last chunk's padding taps) instead of
+// eight with a uniform branch per tap (97 KB of code).  Same products in the same order with either tap source:
+// bit-identical results.
 // V3's tap registers are worth it where the thread's live state (sample window + accumulators + one column group of taps)
 // still fits the 80-register budget of three resident CTAs and the window addresses are compile-time offsets (8 % GD == 0);
 // the other instances keep the constant-bank taps (they spill with V3).
 template <typename EO, typename TR, int I, int D, int G> struct rs_v3 {
     using M = rs_mp<I, D, G>;
     static constexpr int est = (M::OFFMAX + 8 + M::NO) * (int)(sizeof(EO) / 4) + I * 4;
-    static constexpr bool value = DSP_RS_V3 != 0 && est <= 80 && (8 % M::GD == 0);
+    static constexpr bool value = est <= 80 && (8 % M::GD == 0);
 };
 template <typename TR, int I> struct alignas(16) RsTaps { TR h[I][64]; };
 
@@ -394,19 +382,12 @@ resample_mp2_kernel(const EX* __restrict__ x, int64_t x_begin, int64_t nx_local,
 #pragma unroll
                     for (int q = 0; q < M::OFFMAX + 8; ++q) xv[q] = rs_cvt<EO, EX>::get(xs[M::xpos(tid * M::GD + r0 + q)]);
                 }
-                TR hq[I][8];                                  // the chunk's taps
-#if DSP_RS_HQ                                                 // 128-bit uniform loads from the parameter bank (A/B: DSP_RS_HQ=0)
+                TR hq[I][8];                                  // the chunk's taps: 128-bit uniform loads from the parameter bank
 #pragma unroll
                 for (int ph = 0; ph < I; ++ph)
 #pragma unroll
                     for (int v = 0; v < 8; v += 16 / (int)sizeof(TR))
                         *reinterpret_cast<uint4*>(&hq[ph][v]) = *reinterpret_cast<const uint4*>(&taps.h[ph][c * 8 + v]);
-#else                                                         // constant-bank operands of the multiply-adds themselves
-#pragma unroll
-                for (int ph = 0; ph < I; ++ph)
-#pragma unroll
-                    for (int v = 0; v < 8; ++v) hq[ph][v] = taps.h[ph][c * 8 + v];
-#endif
 #pragma unroll
                 for (int q = 0; q < 8; ++q) {
                     if (r0 + q < tpp) {                       // the zero padding taps never touch a sample
@@ -583,16 +564,11 @@ static int rs_launch_mp(RsPlanImpl* p, const RsArgs& a, cudaStream_t st, bool* d
     return DSPB200_OK;
 }
 
-static bool rs_mp2_enabled() {
-    static const bool on = [] { const char* e = getenv("DSPB200_RS_MP2"); return !(e && e[0] == '0'); }();
-    return on;
-}
-
 template <typename EX, typename TR, typename EO, int I, int D, int G>
 static int rs_launch_mp2(RsPlanImpl* p, const RsArgs& a, cudaStream_t st, bool* done) {
     using M = rs_mp<I, D, G>;
     *done = false;
-    if (!rs_mp2_enabled() || p->tpp8 > 64) return DSPB200_OK;
+    if (p->tpp8 > 64) return DSPB200_OK;
     const std::vector<TR>& h8 = [&]() -> const std::vector<TR>& {
         if constexpr (sizeof(TR) == 4) return p->h8_32; else return p->h8_64;
     }();
@@ -638,7 +614,7 @@ static int rs_launch(RsPlanImpl* p, const RsArgs& a, cudaStream_t st) {
     if (p->interp >= 2 && p->interp <= 4 && p->decim <= 4 && p->d_pfb8 && a.phi0 >= 0) {
         // multi-phase kernel: G = outputs per phase per thread (Float32 arithmetic: 4; Float64: 2 -- register budget)
         bool done = false;
-        constexpr int GM = sizeof(TR) == 4 ? DSP_RS_G32 : 2;
+        constexpr int GM = sizeof(TR) == 4 ? 4 : 2;
         const int key = (int)p->interp * 10 + (int)p->decim;
         switch (key) {                                    // pipelined kernel first (taps as kernel parameters, <= 64 per phase)
             case 21: DSP_TRY((rs_launch_mp2<EX, TR, EO, 2, 1, GM>(p, a, st, &done))); break;

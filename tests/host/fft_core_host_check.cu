@@ -8,7 +8,6 @@
 static inline void __syncthreads() {}
 #endif
 #include "../../dsp.jl_b200/csrc/fft_core.cuh"
-#include "../../dsp.jl_b200/csrc/fft_r32.cuh"
 #include <complex>
 #include <vector>
 #include <cstdio>
@@ -157,95 +156,6 @@ template <typename T, int N> static int check(double tol) {
     return ok ? 0 : 1;
 }
 
-// the 32 x 32 x 16 plan of the 16384-point transform (fft_r32.cuh): forward transform and the overlap-save bracket,
-// every "thread" in turn as os_unit32 sequences them
-static int check_r32(double tol) {
-    using T = float;
-    constexpr int N = r32::N;
-    std::vector<cx<T>> sm(r32::padded_len()), t32(r32::T32_LEN), t1024(r32::T1024_LEN);
-    r32::fill_tables<T>(t32.data(), t1024.data());
-    r32::Ctx<T> ctx{sm.data(), t32.data(), t1024.data()};
-    std::vector<cx<T>> x(N), h(N), H(N), X(N), y(N);
-    std::vector<cd> xr(N), hr(N);
-    srand(4321);
-    for (int j = 0; j < N; ++j) {
-        double a = rand() / (double)RAND_MAX - 0.5, b = rand() / (double)RAND_MAX - 0.5;
-        x[j] = mkc<T>((T)a, (T)b); xr[j] = cd((double)x[j].x, (double)x[j].y);
-        a = rand() / (double)RAND_MAX - 0.5; b = rand() / (double)RAND_MAX - 0.5;
-        h[j] = (j < N / 4 + 1) ? mkc<T>((T)a, (T)b) : mkc<T>(T(0), T(0)); hr[j] = cd((double)h[j].x, (double)h[j].y);
-    }
-    auto forward = [&](const std::vector<cx<T>>& in, std::vector<cx<T>>& out) {
-        for (int c = 0; c < r32::Q32; ++c) {
-            cx<T> v[32];
-            for (int r = 0; r < 32; ++r) v[r] = in[c + r * r32::Q32];
-            fft_bfly<T, 32, true>(v, nullptr);
-            r32::store_block<T>(ctx.sm, c, v);
-        }
-        for (int tid = 0; tid < r32::NT; ++tid) r32::middle_pass<T>(ctx, tid);
-        for (int tp = 0; tp < r32::Q16; ++tp) {
-            cx<T> v[16];
-            r32::last_pass<T>(ctx, tp, v);
-            for (int r = 0; r < 16; ++r) out[tp + r * r32::Q16] = v[r];
-        }
-    };
-    forward(x, X);
-    std::vector<cd> Xr = xr;
-    ref_fft(Xr, false);
-    double num = 0, den = 0;
-    for (int k = 0; k < N; ++k) { num += std::norm(cd((double)X[k].x, (double)X[k].y) - Xr[k]); den += std::norm(Xr[k]); }
-    const double ef = std::sqrt(num / den);
-    forward(h, H);
-    for (int k = 0; k < N; ++k) H[k] = cscale(H[k], T(1) / T(N));
-    // conv: first | middle | [last x2, x H, swap, plain 32] | middle | last
-    for (int c = 0; c < r32::Q32; ++c) {
-        cx<T> v[32];
-        for (int r = 0; r < 32; ++r) v[r] = x[c + r * r32::Q32];
-        fft_bfly<T, 32, true>(v, nullptr);
-        r32::store_block<T>(ctx.sm, c, v);
-    }
-    for (int tid = 0; tid < r32::NT; ++tid) r32::middle_pass<T>(ctx, tid);
-    std::vector<cx<T>> regs((size_t)r32::Q32 * 32);
-    for (int tid = 0; tid < r32::NT; ++tid) {
-        cx<T> a[16], b[16], v[32];
-        r32::last_pass<T>(ctx, tid, a);
-        r32::last_pass<T>(ctx, tid + r32::Q32, b);
-        for (int r = 0; r < 16; ++r) {
-            v[2 * r] = cswap(cmul(a[r], H[tid + r * r32::Q16]));
-            v[2 * r + 1] = cswap(cmul(b[r], H[tid + r32::Q32 + r * r32::Q16]));
-        }
-        fft_bfly<T, 32, true>(v, nullptr);
-        for (int r = 0; r < 32; ++r) regs[(size_t)tid * 32 + r] = v[r];
-    }
-    for (int tid = 0; tid < r32::NT; ++tid) {
-        cx<T> v[32];
-        for (int r = 0; r < 32; ++r) v[r] = regs[(size_t)tid * 32 + r];
-        r32::store_block<T>(ctx.sm, tid, v);
-    }
-    for (int tid = 0; tid < r32::NT; ++tid) r32::middle_pass<T>(ctx, tid);
-    for (int tp = 0; tp < r32::Q16; ++tp) {
-        cx<T> v[16];
-        r32::last_pass<T>(ctx, tp, v);
-        for (int r = 0; r < 16; ++r) y[tp + r * r32::Q16] = cswap(v[r]);
-    }
-    std::vector<cd> Hr = hr, Yr(N);
-    ref_fft(Hr, false);
-    for (int k = 0; k < N; ++k) Yr[k] = Xr[k] * Hr[k];
-    ref_fft(Yr, true);
-    num = den = 0;
-    for (int j = 0; j < N; ++j) { num += std::norm(cd((double)y[j].x, (double)y[j].y) - Yr[j] / (double)N); den += std::norm(Yr[j] / (double)N); }
-    const double ec = std::sqrt(num / den);
-    // scattered first-pass stores: lanes c .. c+7 write 16-byte chunks of their 32-slot runs
-    int worst = 1;
-    for (int c0 = 0; c0 + 8 <= r32::Q32; c0 += 8) {
-        int cnt[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-        for (int l = 0; l < 8; ++l) cnt[((long long)r32::pad(32 * r32::block_of(c0 + l)) * 8 / 16) % 8]++;
-        for (int g = 0; g < 8; ++g) if (cnt[g] > worst) worst = cnt[g];
-    }
-    const bool ok = ef < tol && ec < 2 * tol && worst == 1;
-    printf("N=16384 f32 32x32x16  forward relerr %.3e  conv relerr %.3e  scatter-store wavefronts/quarter-warp %d  %s\n", ef, ec, worst, ok ? "ok" : "FAIL");
-    return ok ? 0 : 1;
-}
-
 int main() {
     int bad = 0;
     bad += check<float, 32>(5e-7);
@@ -258,7 +168,6 @@ int main() {
     bad += check<float, 4096>(5e-7);
     bad += check<float, 8192>(5e-7);
     bad += check<float, 16384>(5e-7);
-    bad += check_r32(5e-7);
     bad += check<double, 256>(1e-15);
     bad += check<double, 1024>(1e-15);
     bad += check<double, 2048>(1e-15);

@@ -196,21 +196,6 @@ def test_conv_config2_scaled(dt):
     assert relerr(y, truth) <= max(2 * relerr(ref32, truth), tol(dt))
 
 
-@pytest.mark.parametrize("dt", [np.complex64, np.float32])
-def test_conv_os_r32_kernel_opt_in(dt, monkeypatch):
-    # DSPB200_OS_R32=1 selects the 32 x 32 x 16 kernel for 16384-point Float32 plans instead of the default
-    # 16 x 16 x 16 x 4 kernel: same parity bar, and different roundings show that the other kernel ran
-    nv, nu = 4097, 1 << 20
-    u, v = randn(nu, dt), randn(nv, dt)
-    truth = od.conv_exact(u, v)
-    default = dsp.conv(u, v, algorithm="fft_overlapsave", nfft=16384)
-    monkeypatch.setenv("DSPB200_OS_R32", "1")
-    r32 = dsp.conv(u, v, algorithm="fft_overlapsave", nfft=16384)
-    assert r32.dtype == default.dtype == np.dtype(dt)
-    assert relerr(default, truth) < TOL32 and relerr(r32, truth) < TOL32
-    assert not np.array_equal(r32, default)
-
-
 def test_conv_config2_full_size_probes():
     # BASELINE config 2 at full size (2^26 ComplexF32, 4097 taps): direct double-precision evaluation of the
     # convolution sum at 2000 probe outputs (incl. both edges and block boundaries), plus linearity.
