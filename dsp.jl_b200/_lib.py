@@ -73,6 +73,8 @@ SIGNATURES = {
     "dspb200_spec_nsegments": (_i64, [_vp, _i64]),
     "dspb200_welch_exec": (_int, [_vp, _vp, _i64, _dbl, _vp]),
     "dspb200_welch_exec_dev": (_int, [_vp, _vp, _i64, _dbl, _vp, _vp]),
+    "dspb200_welch_batch_exec": (_int, [_vp, _vp, _i64, _i64, _dbl, _vp]),
+    "dspb200_welch_batch_exec_dev": (_int, [_vp, _vp, _i64, _i64, _dbl, _vp, _vp]),
     "dspb200_welch_exec_range_dev": (_int, [_vp, _vp, _i64, _i64, _i64, _i64, _dbl, _vp, _vp]),
     "dspb200_welch_begin_dev": (_int, [_vp, _vp]),
     "dspb200_welch_accumulate_dev": (_int, [_vp, _vp, _i64, _i64, _i64, _i64, _vp]),
@@ -232,6 +234,13 @@ class SpecPlan(_Plan):
 
     def welch_dev(self, s_ptr, length, r, out_ptr, stream=0):
         check(lib.dspb200_welch_exec_dev(self.handle, s_ptr, length, float(r), out_ptr, stream))
+
+    def welch_batch(self, s, length, nchan, r, out):
+        """s: Fortran-ordered length x nchan array; out: Fortran-ordered nout x nchan array."""
+        check(lib.dspb200_welch_batch_exec(self.handle, ptr(s), int(length), int(nchan), float(r), ptr(out)))
+
+    def welch_batch_dev(self, s_ptr, length, nchan, r, out_ptr, stream=0):
+        check(lib.dspb200_welch_batch_exec_dev(self.handle, s_ptr, int(length), int(nchan), float(r), out_ptr, stream))
 
     def welch_begin_dev(self, stream=0):
         check(lib.dspb200_welch_begin_dev(self.handle, stream))

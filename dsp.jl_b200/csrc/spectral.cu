@@ -45,6 +45,11 @@ struct SpecPlanImpl {
     int nparts = 0;               // CTAs of the Welch kernel == rows of `partial`
     int rows_used = 0;            // rows of `partial` written since welch_begin (host bookkeeping, stream order = call order)
     DevBuf partial;               // fused Welch: [nparts][nfft] real T
+    // batched Welch (dspb200_welch_batch_exec_dev): its own kernel configuration cache and scratch, so that a streaming
+    // accumulation open on the plan (partial / rows_used, acc) is left as it was
+    WelchCfg welch_batch_cfg[2];
+    DevBuf bpartial;              // fused: one row of nfft real T per (channel, slice), at most WELCH_BATCH_SCRATCH bytes
+    DevBuf bacc;                  // generic: double[nbins_fft], one channel at a time
     // generic path
     cufftHandle fft = 0;
     bool fft_ok = false;
@@ -281,6 +286,192 @@ __global__ void __launch_bounds__(1024) welch_finalize_kernel(const T* __restric
             if (onesided && !(k == 0 || k == N / 2)) m = m2;
         }
         out[k] = (T)(sum * m);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------- batched fused Welch
+// Many channels (the columns of a len x nchan matrix, `chan_stride` samples apart), one launch.  A work item is a
+// (channel, slice) pair: slice j of a channel owns its units [j per, min((j+1) per, upc)), so units never cross a channel and
+// a real unit's two segments always belong to one channel (the finalize pass un-mixes bins k and N-k of one row).  Virtual
+// CTA v takes the contiguous item range [v ipv, (v+1) ipv); it accumulates |Z|^2 in registers over an item's units and writes
+// ONE partial row per item (row = item index).  Same front end, FFT and shared-memory layout as welch_fused_kernel; the TMA
+// prefetch of the next unit runs across item and channel boundaries.  No atomics: the result is deterministic.
+template <typename T, int N, bool CPLX, int MODE, int G>
+__global__ void __launch_bounds__((welch_bounds<T, N, G>::NTG * G), (welch_bounds<T, N, G>::minblocks))
+welch_batch_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t nseg, int64_t upc, int64_t per, int slices,
+                   int64_t nitems, int64_t hop, int n, const typename win_t<T>::type* __restrict__ win,
+                   const cx<T>* __restrict__ tw, const cx<T>* __restrict__ g16, const cx<T>* __restrict__ g256,
+                   T* __restrict__ partial) {
+    constexpr int NT = fft_threads<N>::value;
+    constexpr int NB16 = N / 16;
+    constexpr int ITL = (NB16 + NT - 1) / NT;
+    using L = welch_layout<T, N, CPLX, MODE>;
+    using Scope = typename std::conditional<G == 1, FftCtaScope, FftGroupScope<NT>>::type;
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    using In = typename in_type<T, CPLX>::type;
+    const In* s = reinterpret_cast<const In*>(s_);
+    const int gid = G == 1 ? 0 : threadIdx.x / NT;
+    const int tid = G == 1 ? threadIdx.x : threadIdx.x - gid * NT;
+    constexpr bool TMA = MODE >= 1;
+    constexpr bool WSM = MODE == 2;
+    constexpr bool WREG = MODE == 3;
+    using W = typename win_t<T>::type;
+    cx<T>* tabs = reinterpret_cast<cx<T>*>(smem_raw);
+    W* wsm = reinterpret_cast<W*>(smem_raw + L::table_bytes());
+    unsigned char* gbase = smem_raw + L::table_bytes() + L::window_bytes(n) + (size_t)gid * L::group_bytes(n, hop);
+    cx<T>* sm = reinterpret_cast<cx<T>*>(gbase);
+    In* stage = reinterpret_cast<In*>(sm + padded_len<T>(N));
+    uint64_t* bar = reinterpret_cast<uint64_t*>(gbase + L::group_bytes(n, hop) - 16);
+    pdl_launch_dependents();
+    const FftCtx<T> ctx = fft_make_ctx_at<T, N, NT * G>(sm, tabs, g16, g256, tw, threadIdx.x);
+    if constexpr (WSM) {
+        for (int i = threadIdx.x; i < n; i += NT * G) wsm[i] = win[i];
+    }
+    Scope scope;
+    if constexpr (G > 1) scope.id = 8 + gid;
+    W wreg[WREG ? ITL : 1][WREG ? 16 : 1];
+    if constexpr (WREG) {
+#pragma unroll
+        for (int it = 0; it < ITL; ++it)
+#pragma unroll
+            for (int r = 0; r < 16; ++r) {
+                const int j = tid + it * NT + r * NB16;
+                wreg[it][r] = (j < n && tid + it * NT < NB16) ? win[j] : W{};
+            }
+    }
+    T acc[ITL][16];
+#pragma unroll
+    for (int i = 0; i < ITL; ++i)
+#pragma unroll
+        for (int r = 0; r < 16; ++r) acc[i][r] = T(0);
+
+    const int64_t vcta = (int64_t)blockIdx.x * G + gid, nvcta = (int64_t)gridDim.x * G;
+    const int64_t ipv = (nitems + nvcta - 1) / nvcta;
+    const int64_t i0 = vcta * ipv < nitems ? vcta * ipv : nitems;
+    const int64_t i1 = i0 + ipv < nitems ? i0 + ipv : nitems;
+    // item -> (channel, first unit, end unit)
+    auto item_range = [&](int64_t i, int64_t& c, int64_t& ua, int64_t& ub) {
+        c = i / slices;
+        ua = (i - c * slices) * per;
+        ub = ua + per < upc ? ua + per : upc;
+    };
+    auto unit_src = [&](int64_t c, int64_t u) -> const In* { return s + c * chan_stride + (CPLX ? u : 2 * u) * hop; };
+    auto unit_bytes = [&](int64_t u) -> uint32_t {
+        const bool hasB = !CPLX && (2 * u + 1 < nseg);
+        return (uint32_t)((hasB ? hop + n : n) * sizeof(In));
+    };
+    if constexpr (TMA) {
+        if (tid == 0) {
+            mbar_init(bar, 1);
+            mbar_fence_init();
+        }
+    }
+    pdl_wait();
+    __syncthreads();
+    int64_t c = 0, ua = 0, ub = 0;
+    if (i0 < i1) item_range(i0, c, ua, ub);
+    if constexpr (TMA) {
+        if (tid == 0 && i0 < i1) {
+            mbar_expect_tx(bar, unit_bytes(ua));
+            tma_load_1d(stage, unit_src(c, ua), unit_bytes(ua), bar);
+        }
+    }
+    uint32_t parity = 0;
+
+    for (int64_t item = i0; item < i1; ++item) {
+        for (int64_t u = ua; u < ub; ++u) {
+            const bool hasB = !CPLX && (2 * u + 1 < nseg);
+            const In* pa = TMA ? stage : unit_src(c, u);
+            const In* pb = pa + hop;
+            if constexpr (TMA) {
+                mbar_wait(bar, parity);
+                parity ^= 1;
+            }
+            auto ld0 = [&](int j, int it, int r) -> cx<T> {
+                if (j >= n) return mkc<T>(T(0), T(0));
+                if constexpr (CPLX) {
+                    cx<T> v = pa[j];
+                    if (WREG || WSM || win) { const W w = WREG ? wreg[WREG ? it : 0][WREG ? r : 0] : (WSM ? wsm[j] : win[j]); v = mkc<T>(win_mul(v.x, w), win_mul(v.y, w)); }
+                    return v;
+                } else {
+                    T a = pa[j];
+                    T b = hasB ? pb[j] : T(0);
+                    if (WREG || WSM || win) { const W w = WREG ? wreg[WREG ? it : 0][WREG ? r : 0] : (WSM ? wsm[j] : win[j]); a = win_mul(a, w); b = win_mul(b, w); }
+                    return mkc<T>(a, b);
+                }
+            };
+            fft_first_pass<T, N, NT, true>(ctx, tid, ld0, scope);
+            if constexpr (TMA) {
+                // the next unit: the following one of this item, else the first one of the next item
+                if (tid == 0) {
+                    int64_t nc = c, nu = u + 1, nub = ub;
+                    if (nu == ub && item + 1 < i1) item_range(item + 1, nc, nu, nub);
+                    if (nu < nub) {
+                        mbar_expect_tx(bar, unit_bytes(nu));
+                        tma_load_1d(stage, unit_src(nc, nu), unit_bytes(nu), bar);
+                    }
+                }
+            }
+            scope.sync();
+            fft_middle<T, N, NT>(ctx, tid, scope);
+#pragma unroll
+            for (int it = 0; it < ITL; ++it) {
+                const int tp = tid + it * NT;
+                if (NB16 % NT != 0 && tp >= NB16) break;
+                cx<T> v[16];
+                fft_last_pass<T, N>(ctx, tp, v);
+#pragma unroll
+                for (int r = 0; r < 16; ++r) acc[it][r] += cabs2(v[r]);
+            }
+        }
+        T* dst = partial + item * N;
+#pragma unroll
+        for (int it = 0; it < ITL; ++it) {
+            const int tp = tid + it * NT;
+            if (tp < NB16) {
+#pragma unroll
+                for (int r = 0; r < 16; ++r) {
+                    dst[tp + r * NB16] = acc[it][r];
+                    acc[it][r] = T(0);
+                }
+            }
+        }
+        if (item + 1 < i1) item_range(item + 1, c, ua, ub);
+    }
+}
+
+// Channel c of the batch: rows c*slices .. c*slices + slices - 1 of `partial`, reduced in Float64 in a fixed order (warp sl
+// sums rows sl, sl + nw, ...; then the nw warp sums in order), un-mixed and scaled as in welch_finalize_kernel, written to
+// column c of the nout x nchan result.  blockIdx.y = channel; blockDim.x = 32 nw with nw = min(32, slices).
+template <typename T, int N>
+__global__ void __launch_bounds__(1024) welch_batch_finalize_kernel(const T* __restrict__ partial, int slices, T* __restrict__ out,
+                                                                    int nout, int real_in, int onesided, double m1, double m2) {
+    __shared__ double red[32][33];
+    pdl_launch_dependents();
+    pdl_wait();
+    const int b = threadIdx.x & 31, sl = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    const int k = blockIdx.x * 32 + b;
+    const T* rows = partial + (int64_t)blockIdx.y * slices * N;
+    double sum = 0.0;
+    if (k < nout) {
+        const T* c0 = rows + k;
+        const T* c1 = rows + ((N - k) & (N - 1));
+        if (real_in) {
+            for (int c = sl; c < slices; c += nw) sum += (double)c0[(int64_t)c * N] + (double)c1[(int64_t)c * N];
+        } else {
+            for (int c = sl; c < slices; c += nw) sum += (double)c0[(int64_t)c * N];
+        }
+    }
+    red[sl][b] = sum;
+    __syncthreads();
+    if (sl == 0 && k < nout) {
+        for (int i = 1; i < nw; ++i) sum += red[i][b];
+        double m = m1;
+        if (real_in) {
+            sum *= 0.5;
+            if (onesided && !(k == 0 || k == N / 2)) m = m2;
+        }
+        out[(int64_t)blockIdx.y * nout + k] = (T)(sum * m);
     }
 }
 
@@ -946,6 +1137,110 @@ static int launch_welch_finalize(SpecPlanImpl* p, double r, void* out, cudaStrea
     return DSPB200_OK;
 }
 
+// Partial rows of the batched Welch path: at most this many bytes per plan, in a buffer of its own (a streaming accumulation
+// open on the plan keeps its rows).  A batch whose channels need more rows runs in channel groups.
+static constexpr size_t WELCH_BATCH_SCRATCH = (size_t)32 << 20;
+
+// Slices per channel for `gc` channels of `upc` units on `nv` virtual CTAs: the split whose busiest virtual CTA runs the fewest
+// units (items per virtual CTA x units per item), the fewest slices on ties, at most `max_slices`.  Every slice is non-empty.
+static int64_t welch_batch_slices(int64_t gc, int64_t upc, int64_t nv, int64_t max_slices) {
+    int64_t lim = upc < max_slices ? upc : max_slices;
+    if (lim > 2 * nv) lim = 2 * nv;
+    int64_t best = 1, best_cost = cdiv(gc, nv) * upc;
+    for (int64_t sl = 2; sl <= lim; ++sl) {
+        const int64_t per = cdiv(upc, sl);
+        if (cdiv(upc, per) != sl) continue;                  // same split as a smaller slice count
+        const int64_t cost = cdiv(gc * sl, nv) * per;
+        if (cost < best_cost) { best = sl; best_cost = cost; }
+    }
+    return best;
+}
+
+// Batched Welch over the nchan columns of a len x nchan matrix (k segments each).  The kernel configuration (MODE x G) is
+// chosen by the same preference list as launch_welch_fused, cached separately.
+template <typename T, int N, bool CPLX>
+static int launch_welch_batch(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan, int64_t k, double r, void* out,
+                              cudaStream_t st) {
+    constexpr int NT = fft_threads<N>::value;
+    using In = typename in_type<T, CPLX>::type;
+    using W = typename win_t<T>::type;
+    using Kern = void (*)(const void*, int64_t, int64_t, int64_t, int64_t, int, int64_t, int64_t, int, const W*, const cx<T>*,
+                          const cx<T>*, const cx<T>*, T*);
+    constexpr bool MULTI = sizeof(T) == 4 && N >= 1024 && N <= 4096;
+    // TMA staging needs every unit start 16-byte aligned: the base, the channel stride (launch_stft_fused's rule), hop and n
+    const bool aligned = ((uintptr_t)s % 16 == 0) && ((len * sizeof(In)) % 16 == 0 || nchan == 1) &&
+                         ((p->hop * sizeof(In)) % 16 == 0) && ((p->n * sizeof(In)) % 16 == 0);
+    const W* win = reinterpret_cast<const W*>(p->d_window);
+    SpecPlanImpl::WelchCfg& cfg = p->welch_batch_cfg[aligned ? 1 : 0];
+    if (cfg.kern == nullptr) {
+        struct Cand { Kern k; size_t smem; int g, warps, per_sm; };
+        Cand best{nullptr, 0, 0, -1, 0};
+        auto consider = [&](Kern kn, size_t smem, int g) -> int {
+            if (best.warps >= 12) return DSPB200_OK;
+            if (smem > p->smem_optin) return DSPB200_OK;
+            DSP_TRY(set_smem(kn, smem));
+            int per_sm = 0;
+            DSP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kn, NT * g, smem));
+            if (per_sm < 1) return DSPB200_OK;
+            const int warps = per_sm * g * NT / 32;
+            if (warps > best.warps) best = Cand{kn, smem, g, warps, per_sm};
+            return DSPB200_OK;
+        };
+#define DSP_WELCH_CAND(MODE_, G_) \
+    DSP_TRY(consider(welch_batch_kernel<T, N, CPLX, MODE_, G_>, welch_layout<T, N, CPLX, MODE_>::total(p->n, p->hop, G_), G_))
+        constexpr bool WREGOK = sizeof(T) == 4 && N <= 4096;
+        if (aligned) {
+            if (win) {
+                if constexpr (CPLX) {
+                    if constexpr (WREGOK) DSP_WELCH_CAND(3, 1);
+                    DSP_WELCH_CAND(2, 1);
+                    if constexpr (MULTI) { DSP_WELCH_CAND(3, 2); DSP_WELCH_CAND(2, 2); }
+                } else {
+                    if constexpr (MULTI) { DSP_WELCH_CAND(2, 3); DSP_WELCH_CAND(2, 2); }
+                    DSP_WELCH_CAND(2, 1);
+                    if constexpr (WREGOK) DSP_WELCH_CAND(3, 1);
+                }
+            }
+            if constexpr (MULTI && !CPLX) DSP_WELCH_CAND(1, 3);
+            DSP_WELCH_CAND(1, 1);
+            if constexpr (MULTI) DSP_WELCH_CAND(1, 2);
+        }
+        if (best.k == nullptr) DSP_WELCH_CAND(0, 1);
+#undef DSP_WELCH_CAND
+        DSP_REQUIRE(best.k != nullptr, "no batched Welch kernel configuration fits (nfft=%lld)", (long long)p->nfft);
+        DSP_TRY(set_smem(best.k, best.smem));
+        cfg.kern = reinterpret_cast<void*>(best.k); cfg.smem = best.smem; cfg.g = best.g; cfg.per_sm = best.per_sm;
+        cfg.threads = NT * best.g;
+    }
+    const int64_t upc = CPLX ? k : (k + 1) / 2;
+    const int64_t cap = (int64_t)p->sm_count * cfg.per_sm;           // resident CTAs: one wave
+    const int64_t nv = cap * cfg.g;                                   // resident virtual CTAs
+    const int64_t rows_cap = (int64_t)(WELCH_BATCH_SCRATCH / ((size_t)N * sizeof(T)));
+    const int64_t gc_max = nchan < rows_cap ? nchan : rows_cap;
+    const auto* tw = reinterpret_cast<const cx<T>*>(p->d_tw);
+    const auto* g16 = reinterpret_cast<const cx<T>*>(p->d_t16);
+    const auto* g256 = reinterpret_cast<const cx<T>*>(p->d_t256);
+    for (int64_t c0 = 0; c0 < nchan; c0 += gc_max) {
+        const int64_t gc = nchan - c0 < gc_max ? nchan - c0 : gc_max;
+        const int64_t slices = welch_batch_slices(gc, upc, nv, rows_cap / gc);
+        const int64_t per = cdiv(upc, slices);
+        const int64_t nitems = gc * slices;
+        DSP_TRY(p->bpartial.reserve((size_t)nitems * N * sizeof(T)));
+        const int64_t want = cdiv(nitems, cfg.g);
+        const int grid = (int)(want < cap ? want : cap);
+        DSP_CUDA(launch_pdl(reinterpret_cast<Kern>(cfg.kern), (unsigned)grid, (unsigned)cfg.threads, cfg.smem, st,
+                            (const void*)((const In*)s + c0 * len), len, k, upc, per, (int)slices, nitems, p->hop, (int)p->n,
+                            win, tw, g16, g256, reinterpret_cast<T*>(p->bpartial.p)));
+        DSP_LAUNCH_OK();
+        const int nw = slices < 32 ? (int)slices : 32;
+        welch_batch_finalize_kernel<T, N><<<dim3((unsigned)cdiv(p->nout, 32), (unsigned)gc), 32 * nw, 0, st>>>(
+            reinterpret_cast<const T*>(p->bpartial.p), (int)slices, reinterpret_cast<T*>(out) + c0 * p->nout, (int)p->nout,
+            CPLX ? 0 : 1, (int)p->onesided, 1.0 / r, 2.0 / r);
+        DSP_LAUNCH_OK();
+    }
+    return DSPB200_OK;
+}
+
 template <typename T, int N, bool CPLX>
 static int launch_stft_fused(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan, int64_t k, double r,
                              int psd_only, void* out, cudaStream_t st) {
@@ -1032,6 +1327,20 @@ template <typename T> static int welch_finalize_dispatch(SpecPlanImpl* p, double
         DSP_FUSED_SIZES(X)
 #undef X
     }
+    return DSPB200_EUNSUPPORTED;
+}
+template <typename T> static int welch_batch_dispatch(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan, int64_t k,
+                                                       double r, void* out, cudaStream_t st) {
+    switch (p->nfft) {
+#define X(NN)                                                                                               \
+    case NN:                                                                                                \
+        if constexpr (sizeof(T) == 8 && NN > 8192) break;                                                   \
+        else return p->cplx ? launch_welch_batch<T, NN, true>(p, s, len, nchan, k, r, out, st)              \
+                            : launch_welch_batch<T, NN, false>(p, s, len, nchan, k, r, out, st);
+        DSP_FUSED_SIZES(X)
+#undef X
+    }
+    set_error("no fused Welch kernel for nfft=%lld", (long long)p->nfft);
     return DSPB200_EUNSUPPORTED;
 }
 template <typename T> static int stft_fused_dispatch(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan,
@@ -1132,6 +1441,30 @@ template <typename T> static int stft_generic(SpecPlanImpl* p, const void* s, in
                                                            (T)(2.0 / r), out, c * k + b0);
             DSP_LAUNCH_OK();
         }
+    }
+    return DSPB200_OK;
+}
+
+// cuFFT sizes of the batched Welch: one channel after another through the generic segment / FFT / power kernels, into the
+// batch's own Float64 accumulator
+template <typename T> static int welch_batch_generic(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan, int64_t k,
+                                                      double r, void* out, cudaStream_t st) {
+    DSP_TRY(p->bacc.reserve((size_t)p->nbins_fft * sizeof(double)));
+    double* acc = reinterpret_cast<double*>(p->bacc.p);
+    for (int64_t c = 0; c < nchan; ++c) {
+        DSP_CUDA(cudaMemsetAsync(acc, 0, (size_t)p->nbins_fft * sizeof(double), st));
+        for (int64_t b0 = 0; b0 < k; b0 += p->batch) {
+            const int64_t nseg = k - b0 < p->batch ? k - b0 : p->batch;
+            DSP_TRY(generic_segments<T>(p, s, c * len + b0 * p->hop, nseg, st));
+            const int threads = 128;
+            pow_acc_kernel<T><<<(int)cdiv(p->nbins_fft, threads), threads, 0, st>>>(
+                reinterpret_cast<const cx<T>*>(p->specbuf.p), p->nbins_fft, nseg, acc);
+            DSP_LAUNCH_OK();
+        }
+        const int threads = 128;
+        pow_finalize_kernel<T><<<(int)cdiv(p->nout, threads), threads, 0, st>>>(acc, p->nbins_fft, p->nfft, p->nout, p->onesided,
+                                                                                1.0 / r, 2.0 / r, reinterpret_cast<T*>(out) + c * p->nout);
+        DSP_LAUNCH_OK();
     }
     return DSPB200_OK;
 }
@@ -1463,6 +1796,57 @@ int dspb200_welch_exec_dev(dspb200_spec_plan* plan, const void* s, int64_t len, 
     return dspb200_welch_exec_range_dev(plan, s, len, 0, 0, k, r, out, stream);
 }
 
+// Batched welch_pgram: the nchan columns of the column-major len x nchan matrix `s` are independent signals, each Welch-averaged
+// with the plan's configuration; out is nout x nchan.  Fused sizes: one launch over (channel, slice) work items plus one
+// finalize launch per channel group (welch_batch_kernel); cuFFT sizes: channel by channel.
+int dspb200_welch_batch_exec_dev(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, double r, void* out,
+                                 void* stream) {
+    DSP_RANGE("dspb200_welch_batch_exec_dev");
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    DSP_REQUIRE(nchan >= 0 && len >= 0, "negative size");
+    SpecPlanImpl* p = &plan->impl;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (nchan == 0) return DSPB200_OK;
+    DSP_REQUIRE(out != nullptr, "out is NULL");
+    const int64_t k = nsegments(p, len);
+    if (k == 0) {                                        // fill!(out, 0), src/periodograms.jl:747
+        DSP_CUDA(cudaMemsetAsync(out, 0, (size_t)(p->nout * nchan) * (p->f64 ? 8 : 4), st));
+        return DSPB200_OK;
+    }
+    DSP_REQUIRE(s != nullptr, "s is NULL");
+    DSP_REQUIRE(r != 0.0, "r must be nonzero");
+    if (p->fused)
+        return p->f64 ? welch_batch_dispatch<double>(p, s, len, nchan, k, r, out, st)
+                      : welch_batch_dispatch<float>(p, s, len, nchan, k, r, out, st);
+    DSP_TRY(generic_prepare(p));
+    return p->f64 ? welch_batch_generic<double>(p, s, len, nchan, k, r, out, st)
+                  : welch_batch_generic<float>(p, s, len, nchan, k, r, out, st);
+}
+
+int dspb200_welch_batch_exec(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, double r, void* out) {
+    DSP_RANGE("dspb200_welch_batch_exec");
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    DSP_REQUIRE(nchan >= 0 && len >= 0, "negative size");
+    SpecPlanImpl* p = &plan->impl;
+    if (nchan == 0) return DSPB200_OK;
+    DSP_REQUIRE(out != nullptr, "out is NULL");
+    DSP_CUDA(cudaSetDevice(p->device));
+    DSP_TRY(ensure_streams(p));
+    const size_t esz = dtype_size(p->dtype);
+    const size_t out_bytes = (size_t)(p->nout * nchan) * (p->f64 ? 8 : 4);
+    const bool any = nsegments(p, len) > 0;
+    if (any) {
+        DSP_REQUIRE(s != nullptr, "s is NULL");
+        DSP_TRY(p->in[0].reserve((size_t)(len * nchan) * esz));
+    }
+    DSP_TRY(p->out.reserve(out_bytes));
+    if (any) DSP_CUDA(cudaMemcpyAsync(p->in[0].p, s, (size_t)(len * nchan) * esz, cudaMemcpyHostToDevice, p->s_exec));
+    DSP_TRY(dspb200_welch_batch_exec_dev(plan, any ? p->in[0].p : nullptr, len, nchan, r, p->out.p, p->s_exec));
+    DSP_CUDA(cudaMemcpyAsync(out, p->out.p, out_bytes, cudaMemcpyDeviceToHost, p->s_exec));
+    DSP_CUDA(cudaStreamSynchronize(p->s_exec));
+    return DSPB200_OK;
+}
+
 // Host-pointer Welch: the signal is streamed through two device buffers in segment-aligned chunks so the
 // H2D copy of chunk c+1 overlaps the kernel of chunk c (effective when `s` is pinned).
 int dspb200_welch_exec(dspb200_spec_plan* plan, const void* s, int64_t len, double r, void* out) {
@@ -1736,7 +2120,7 @@ int dspb200_spec_plan_destroy(dspb200_spec_plan* plan) {
     if (p->d_t16) cudaFree(p->d_t16);
     if (p->d_t32) cudaFree(p->d_t32);
     if (p->d_t256) cudaFree(p->d_t256);
-    p->partial.release(); p->segbuf.release(); p->specbuf.release(); p->acc.release();
+    p->partial.release(); p->bpartial.release(); p->bacc.release(); p->segbuf.release(); p->specbuf.release(); p->acc.release();
     p->in[0].release(); p->in[1].release(); p->out.release(); p->tmp.release();
     if (p->fft_ok) cufftDestroy(p->fft);
     for (int i = 0; i < 2; ++i) {

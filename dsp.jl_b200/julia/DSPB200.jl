@@ -216,6 +216,34 @@ end
 welch_pgram(s::Vector{T}, config::GPUWelchConfig{T}) where {T<:GPUNumber} =
     welch_pgram!(Vector{abs2type(T)}(undef, length(config.freq)), s, config)
 
+# Batched Welch: the columns of `s` are independent channels, each Welch-averaged with the same configuration in one launch
+# (dspb200_welch_batch_exec).  The reference has no matrix method, so these are not added to the DSP.* overlay below.
+function welch_pgram!(out::Matrix, s::Matrix{T}, config::GPUWelchConfig{T}) where {T<:GPUNumber}
+    len, nchan = size(s)
+    size(out) == (length(config.freq), nchan) ||
+        throw(DimensionMismatch("Expected `output` to be of size (length(config.freq), size(s, 2)) = $((length(config.freq), nchan)); got $(size(out))"))
+    eltype(out) == abs2type(T) ||
+        throw(ArgumentError("Eltype of output ($(eltype(out))) doesn't match the expected type: $(abs2type(T))."))
+    k = len >= config.nsamples ? div(len - config.nsamples, config.nsamples - config.noverlap) + 1 : 0
+    if k == 0 || nchan == 0
+        fill!(out, 0)
+    else
+        GC.@preserve s out check(ccall((:dspb200_welch_batch_exec, libdspb200), Cint,
+            (Ptr{Cvoid}, Ptr{Cvoid}, Int64, Int64, Cdouble, Ptr{Cvoid}), config.plan.ptr, s, len, nchan, k * config.r, out))
+    end
+    return Periodograms.Periodogram(out, config.freq)
+end
+welch_pgram(s::Matrix{T}, config::GPUWelchConfig{T}) where {T<:GPUNumber} =
+    welch_pgram!(Matrix{abs2type(T)}(undef, length(config.freq), size(s, 2)), s, config)
+function welch_pgram(s::Matrix{T}, n::Int=size(s, 1) >> 3, noverlap::Int=n >> 1; onesided::Bool=T <: Real,
+                     nfft::Int=DSP.nextfastfft(n), fs::Real=1,
+                     window::Union{Function,AbstractVector,Nothing}=nothing) where {T<:GPUNumber}
+    config = WelchConfig(size(s, 1), T; n, noverlap, onesided, nfft, fs, window)
+    p = welch_pgram(s, config)
+    close!(config.plan)
+    return p
+end
+
 # welch_pgram(filt(b, x), config) as one pipelined call (dspb200_filt_welch_exec): x is uploaded in chunks that overlap the
 # kernels, the filter output never leaves the GPU.  Same values as `welch_pgram(DSP.filt(b, x), config)`.
 function filt_welch(b::Vector{T}, x::Vector{T}, config::GPUWelchConfig{T}) where {T<:GPUNumber}

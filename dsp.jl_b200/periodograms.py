@@ -128,16 +128,22 @@ def _signal(s):
     return np.ascontiguousarray(s, dtype=fftintype(s.dtype))           # buffer eltype, :55
 
 
+def _signal_matrix(s):
+    """A len x nchan matrix of independent channels, column-major (one contiguous column per channel)."""
+    return np.asfortranarray(s, dtype=fftintype(s.dtype))
+
+
 # --------------------------------------------------------------------------------------------- WelchConfig
 
 class WelchConfig:
     """WelchConfig(data_or_nsamples, eltype; n, noverlap, onesided, nfft, fs, window), src/periodograms.jl:516-587.
-    Owns the device plan (segmenter + FFT + window), reusable across calls like the reference's plan/buffers."""
+    Owns the device plan (segmenter + FFT + window), reusable across calls like the reference's plan/buffers.
+    `data` may be a len x nchan matrix of channels: nsamples is then its number of rows."""
 
     def __init__(self, data, eltype=None, n=None, noverlap=None, onesided=None, nfft=None, fs=1, window=_UNSET):
         if eltype is None:
             data = np.asarray(data)
-            nsamples, eltype = data.shape[-1], data.dtype
+            nsamples, eltype = data.shape[0], data.dtype
         else:
             nsamples = int(data)
         eltype = np.dtype(eltype)
@@ -166,21 +172,27 @@ class WelchConfig:
 
 
 def welch_pgram(s, n=None, noverlap=None, onesided=None, nfft=None, fs=1, window=_UNSET):
-    """welch_pgram(s, n, noverlap; kw...) (src/periodograms.jl:647-649) or welch_pgram(s, config) (:702-705)."""
+    """welch_pgram(s, n, noverlap; kw...) (src/periodograms.jl:647-649) or welch_pgram(s, config) (:702-705).
+    A 2-D `s` (len x nchan) is the batched extension: every column is an independent signal, Welch-averaged with the same
+    configuration in one launch; power is nout x nchan and the defaults come from len = size(s, 1)."""
     if isinstance(n, WelchConfig):
         config = n
     else:
         if isinstance(s, DeviceArray):
-            nn = s.shape[-1] >> 3 if n is None else int(n)
-            config = WelchConfig(s.shape[-1], s.dtype, n=nn, noverlap=(nn >> 1 if noverlap is None else noverlap),
+            nn = s.shape[0] >> 3 if n is None else int(n)
+            config = WelchConfig(s.shape[0], s.dtype, n=nn, noverlap=(nn >> 1 if noverlap is None else noverlap),
                                  onesided=onesided, nfft=nfft, fs=fs, window=window)
         else:
             s = np.asarray(s)
-            nn = s.shape[-1] >> 3 if n is None else int(n)
+            nn = s.shape[0] >> 3 if n is None else int(n)
             config = WelchConfig(s, n=nn, noverlap=(nn >> 1 if noverlap is None else noverlap), onesided=onesided,
                                  nfft=nfft, fs=fs, window=window)
     if isinstance(s, DeviceArray):
         return _welch_device(s, config)
+    if np.ndim(s) == 2:
+        sig = _signal_matrix(np.asarray(s))
+        out = np.empty((config.freq.size, sig.shape[1]), dtype=fftabs2type(sig.dtype), order="F")
+        return _welch_batch(out, sig, config)
     sig = _signal(s)
     out = np.empty(config.nfft // 2 + 1 if config.onesided else config.nfft, dtype=fftabs2type(sig.dtype))
     return _welch_helper(out, sig, config)
@@ -219,21 +231,29 @@ def filt_welch(x, n_or_b, b_or_config=None, config=None, nfft=None):
 
 
 def welch_pgram_(out, s, n=None, noverlap=None, onesided=None, nfft=None, fs=1, window=None):
-    """welch_pgram!(out, s, config) (src/periodograms.jl:734-744) / welch_pgram!(out, s, n, noverlap; kw...) (:683-686)."""
+    """welch_pgram!(out, s, config) (src/periodograms.jl:734-744) / welch_pgram!(out, s, n, noverlap; kw...) (:683-686).
+    A 2-D `s` (len x nchan) needs an nout x nchan `out` (the batched extension of welch_pgram)."""
     if isinstance(n, WelchConfig):
         config = n
     else:
         s0 = np.asarray(s)
-        nn = s0.shape[-1] >> 3 if n is None else int(n)
+        nn = s0.shape[0] >> 3 if n is None else int(n)
         config = WelchConfig(s0, n=nn, noverlap=(nn >> 1 if noverlap is None else noverlap), onesided=onesided,
                              nfft=nfft, fs=fs, window=window)
-    sdt = np.asarray(s).dtype
-    if out.size != config.freq.size:
+    s = np.asarray(s)
+    sdt = s.dtype
+    if s.ndim == 2:
+        if out.shape != (config.freq.size, s.shape[1]):
+            raise DimensionMismatch(f"Expected `output` to be of size (length(config.freq), size(s, 2)) = "
+                                    f"{(config.freq.size, s.shape[1])}; got {out.shape}")
+    elif out.size != config.freq.size:
         raise DimensionMismatch(f"Expected `output` to be of length `length(config.freq)`; got {out.size} and {config.freq.size}")
     if out.dtype != fftabs2type(sdt):
         raise ArgumentError(f"Eltype of output ({out.dtype}) doesn't match the expected type: {fftabs2type(sdt)}.")
     if fftintype(sdt) != config.intype:
         raise ArgumentError(f"float(eltype(s)) = {sdt} doesn't match the eltype of the input buffer: {config.intype}.")
+    if s.ndim == 2:
+        return _welch_batch(out, _signal_matrix(s), config)
     return _welch_helper(out, _signal(s), config)
 
 
@@ -253,12 +273,38 @@ def _welch_helper(out, sig, config):
     return Periodogram(out, config.freq)
 
 
+def _welch_batch(out, sig, config):
+    """welch_pgram_helper! on every column of a len x nchan matrix in one batched call; out is nout x nchan."""
+    if sig.dtype != config.intype:
+        raise ArgumentError(f"float(eltype(s)) = {sig.dtype} doesn't match the eltype of the input buffer: {config.intype}.")
+    length, nchan = sig.shape
+    k = arraysplit_count(length, config.nsamples, config.noverlap)
+    if k == 0 or nchan == 0:
+        out[...] = 0
+        return Periodogram(out, config.freq)
+    res = out if out.flags.f_contiguous else np.empty(out.shape, dtype=out.dtype, order="F")
+    config.plan.welch_batch(sig, length, nchan, k * config.r, res)
+    if res is not out:
+        out[...] = res
+    return Periodogram(out, config.freq)
+
+
 def _welch_device(s, config):
-    """welch_pgram on a device-resident vector: only the nout-sample power vector crosses PCIe."""
-    if s.ndim != 1:
-        raise ArgumentError("expected a vector")
+    """welch_pgram on a device-resident vector or len x nchan matrix: only the power (nout, or nout x nchan) crosses PCIe."""
+    if s.ndim not in (1, 2):
+        raise ArgumentError("expected a vector or a len x nchan matrix")
     if s.dtype != config.intype:
         raise ArgumentError(f"float(eltype(s)) = {s.dtype} doesn't match the eltype of the input buffer: {config.intype}.")
+    if s.ndim == 2:
+        length, nchan = s.shape
+        out = np.zeros((config.freq.size, nchan), dtype=fftabs2type(s.dtype), order="F")
+        k = arraysplit_count(length, config.nsamples, config.noverlap)
+        if k == 0 or nchan == 0:
+            return Periodogram(out, config.freq)
+        dout = DeviceArray(out.shape, out.dtype)
+        config.plan.welch_batch_dev(s.ptr, length, nchan, k * config.r, dout.ptr, 0)
+        dout.to_host(out)
+        return Periodogram(out, config.freq)
     out = np.zeros(config.nfft // 2 + 1 if config.onesided else config.nfft, dtype=fftabs2type(s.dtype))
     k = arraysplit_count(s.shape[0], config.nsamples, config.noverlap)
     if k == 0:

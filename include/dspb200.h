@@ -155,6 +155,18 @@ DSPB200_API int64_t dspb200_spec_nsegments(const dspb200_spec_plan* plan, int64_
  * periodogram (:393-417) is the k = 1 case (n = length(s)). */
 DSPB200_API int dspb200_welch_exec(dspb200_spec_plan* plan, const void* s, int64_t len, double r, void* out);
 DSPB200_API int dspb200_welch_exec_dev(dspb200_spec_plan* plan, const void* s, int64_t len, double r, void* out, void* stream);
+/* Batched welch_pgram (an extension: the reference's welch_pgram takes a vector): `s` is a column-major len x nchan matrix
+ * whose columns are independent signals, each Welch-averaged with the plan's configuration; out is nout x nchan (real
+ * eltype of dtype, column c = channel c).  r = k*fs*norm2 is the same for every column.  k == 0 writes zeros; nchan == 0
+ * returns at once; negative sizes give DSPB200_EINVALID.  Power-of-two fused sizes run every channel in one launch over
+ * (channel, slice) work items, with partial rows in scratch of the plan's own, at most 32 MiB (more channels run in groups);
+ * cuFFT sizes run channel by channel.  The batch does not touch the accumulator of dspb200_welch_begin_dev /
+ * dspb200_welch_accumulate_dev, so a streaming accumulation open on the plan may continue after it (in stream order).
+ * The _dev form takes device pointers and a cudaStream_t and returns without synchronising; the host form copies `s` in
+ * and `out` back and returns when done. */
+DSPB200_API int dspb200_welch_batch_exec(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, double r, void* out);
+DSPB200_API int dspb200_welch_batch_exec_dev(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, double r,
+                                             void* out, void* stream);
 /* Segment-range form for multi-GPU sharding: accumulates only segments [seg_begin, seg_end) of the signal
  * whose sample `sample_offset` is s[0]; the caller sums the partial spectra (NCCL all-reduce, SURVEY.md 8e). */
 DSPB200_API int dspb200_welch_exec_range_dev(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t sample_offset,
