@@ -103,6 +103,8 @@ SIGNATURES = {
     "dspb200_resample_arb_plan_create": (_int, [_pp, _int, _int, _vp, _i64, _i64]),
     "dspb200_resample_arb_exec": (_int, [_vp, _vp, _i64, _i64, _dbl, _dbl, _vp, _i64]),
     "dspb200_resample_arb_exec_dev": (_int, [_vp, _vp, _i64, _i64, _dbl, _dbl, _vp, _i64, _vp]),
+    "dspb200_resample_arb_batch_exec": (_int, [_vp, _vp, _i64, _i64, _i64, _i64, _dbl, _dbl, _vp, _i64]),
+    "dspb200_resample_arb_batch_exec_dev": (_int, [_vp, _vp, _i64, _i64, _i64, _i64, _dbl, _dbl, _vp, _i64, _vp]),
     "dspb200_resample_plan_destroy": (_int, [_vp]),
 }
 for _name, (_res, _args) in SIGNATURES.items():
@@ -348,6 +350,15 @@ class ResampleArbPlan(_Plan):
 
     def exec_dev(self, x_ptr, nx, n0, acc0, delta, out_ptr, nout, stream=0):
         check(lib.dspb200_resample_arb_exec_dev(self.handle, x_ptr, nx, n0, float(acc0), float(delta), out_ptr, nout, stream))
+
+    def exec_batch(self, x, nx, ldx, ncols, n0, acc0, delta, out, nout):
+        """x: Fortran-ordered ldx x ncols array (the first nx samples of each column are used); out: nout x ncols."""
+        check(lib.dspb200_resample_arb_batch_exec(self.handle, ptr(x), int(nx), int(ldx), int(ncols), int(n0), float(acc0),
+                                                  float(delta), ptr(out), int(nout)))
+
+    def exec_batch_dev(self, x_ptr, nx, ldx, ncols, n0, acc0, delta, out_ptr, nout, stream=0):
+        check(lib.dspb200_resample_arb_batch_exec_dev(self.handle, x_ptr, int(nx), int(ldx), int(ncols), int(n0), float(acc0),
+                                                      float(delta), out_ptr, int(nout), stream))
 
 
 def conv_fft(u, v, nfft, out):

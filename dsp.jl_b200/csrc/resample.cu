@@ -436,52 +436,127 @@ template <typename TR> __device__ __forceinline__ cx<TR> arb_mix(cx<TR> yu, cx<T
     return mkc<TR>((TR)fma((double)yu.x, alpha, (double)yl.x), (TR)fma((double)yu.y, alpha, (double)yl.y));
 }
 
-template <typename EX, typename TR, typename EO>
-__global__ void __launch_bounds__(RS_NT)
-resample_arb_kernel(const EX* __restrict__ x, int64_t nx, const TR* __restrict__ pfb, const TR* __restrict__ dpfb, int tpp,
-                    int nphases, int64_t n0, double acc0, double delta, EO* __restrict__ out, int64_t nout, int in_smem) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    TR* ps = reinterpret_cast<TR*>(smem_raw);
-    TR* ds = ps + (size_t)nphases * tpp;
-    if (in_smem) {
-        const int tot = nphases * tpp;
-        for (int i = threadIdx.x; i < tot; i += RS_NT) { ps[i] = pfb[i]; ds[i] = dpfb[i]; }
-        __syncthreads();
-    }
-    const int64_t j = (int64_t)blockIdx.x * RS_NT + threadIdx.x;
-    if (j >= nout) return;
-    const double N = (double)nphases, jd = (double)j;
+// P_j = acc0 + j*delta split into q = floor(P_j / Nphi) and r = P_j - q*Nphi in [0, Nphi).
+__device__ __forceinline__ void arb_phase(int64_t j, double N, double acc0, double delta, double* q_out, double* r_out) {
+    const double jd = (double)j;
     const double hi = jd * delta, lo = fma(jd, delta, -hi);          // j*delta = hi + lo exactly
     double q = floor((hi + acc0) / N);
     double r = fma(-q, N, hi);                                       // exact: q*N is an integer, |hi - q*N| small
     r = (r + lo) + acc0;
     while (r < 0.0) { r += N; q -= 1.0; }
     while (r >= N) { r -= N; q += 1.0; }
+    *q_out = q;
+    *r_out = r;
+}
+
+// Output j of one column xc (nx stored samples, zero elsewhere).  Its window is read from the staged span xs, which holds
+// samples [xs_begin, xs_begin + xs_len) of the column, when it lies inside it, else from xc with the bounds test.  A zero
+// sample multiplied in leaves the sums bit-identical to skipping it (an accumulator that starts at +0 never becomes -0),
+// so both sources give the same output.
+template <typename EX, typename TR, typename EO>
+__device__ __forceinline__ EO arb_output(int64_t j, const EX* __restrict__ xc, int64_t nx, const EX* xs, int64_t xs_begin,
+                                         int xs_len, const TR* bank, const TR* dbank, int tpp, int nphases, int64_t n0,
+                                         double acc0, double delta) {
+    double q, r;
+    arb_phase(j, (double)nphases, acc0, delta, &q, &r);
     const double fl = floor(r);
     const int phi = (int)fl;
     const double alpha = r - fl;
     const int64_t first = n0 + (int64_t)q - (tpp - 1);               // oldest sample of the window
-    const TR* hrow = (in_smem ? ps : pfb) + (size_t)phi * tpp;
-    const TR* drow = (in_smem ? ds : dpfb) + (size_t)phi * tpp;
+    const TR* hrow = bank + (size_t)phi * tpp;
+    const TR* drow = dbank + (size_t)phi * tpp;
     EO yl = rs_zero((EO*)nullptr), yu = rs_zero((EO*)nullptr);
-    if (first >= 0 && first + tpp <= nx) {
-        const EX* xp = x + first;
+    const int64_t ls = first - xs_begin;
+    if (ls >= 0 && ls + tpp <= xs_len) {
+        const EX* xp = xs + ls;
         for (int t = 0; t < tpp; ++t) {
             const EO xv = rs_cvt<EO, EX>::get(xp[t]);
             yl = rs_fma(hrow[t], xv, yl);
             yu = rs_fma(drow[t], xv, yu);
         }
     } else {
+#pragma unroll 1
         for (int t = 0; t < tpp; ++t) {
             const int64_t i = first + t;
             if (i >= 0 && i < nx) {
-                const EO xv = rs_cvt<EO, EX>::get(x[i]);
+                const EO xv = rs_cvt<EO, EX>::get(xc[i]);
                 yl = rs_fma(hrow[t], xv, yl);
                 yu = rs_fma(drow[t], xv, yu);
             }
         }
     }
-    out[j] = arb_mix(yu, yl, alpha);
+    return arb_mix(yu, yl, alpha);
+}
+
+// Many columns in one launch.  A work item is (column, tile of `tile` consecutive outputs); persistent CTAs walk the work
+// list, so the column count has no grid-dimension limit.  Per item the input span the tile's windows cover (oldest sample
+// of its first output .. newest sample of its last) is staged in shared memory once -- neighbouring outputs share all but
+// about delta/Nphi of their tpp samples, so the dot loops read shared memory instead of going through L1 per tap.  The span
+// start is rounded down to a 16-byte boundary of the column; when the column base is 16-byte aligned (vec16) the interior
+// is copied with 16-byte cp.async.  Both tap banks are staged once per CTA when they fit (banks_in_smem), else read through
+// L1.  xs_len = 0 stages nothing: every window is then read from global memory.
+constexpr int RS_ARB_NT = 256;
+template <typename EX, typename TR, typename EO>
+__global__ void __launch_bounds__(RS_ARB_NT)
+resample_arb_batch_kernel(const EX* __restrict__ x, int64_t nx, int64_t ldx, const TR* __restrict__ pfb,
+                          const TR* __restrict__ dpfb, int tpp, int nphases, int banks_in_smem, int64_t n0, double acc0,
+                          double delta, EO* __restrict__ out, int64_t nout, int tile, int xs_len, int vec16,
+                          int64_t tiles_per_col, int64_t total_work) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    constexpr int V = 16 / (int)sizeof(EX);                          // samples per 16 bytes
+    EX* xs = reinterpret_cast<EX*>(smem_raw);                        // xs_len samples, a multiple of 16 bytes
+    TR* hs = reinterpret_cast<TR*>(xs + xs_len);
+    TR* ds = hs + (size_t)nphases * tpp;
+    const int tid = threadIdx.x, nth = blockDim.x;
+    if (banks_in_smem) {
+        const int tot = nphases * tpp;
+#pragma unroll 1
+        for (int i = tid; i < tot; i += nth) { hs[i] = pfb[i]; ds[i] = dpfb[i]; }
+        __syncthreads();
+    }
+    const TR* bank = banks_in_smem ? hs : pfb;
+    const TR* dbank = banks_in_smem ? ds : dpfb;
+    for (int64_t w = blockIdx.x; w < total_work; w += gridDim.x) {
+        const int64_t col = w / tiles_per_col;
+        const int64_t j0 = (w - col * tiles_per_col) * tile;
+        const EX* xc = x + col * ldx;
+        int64_t xs_begin = 0;
+        if (xs_len > 0) {
+            double q0, r0;
+            arb_phase(j0, (double)nphases, acc0, delta, &q0, &r0);
+            const int64_t gb = n0 + (int64_t)q0 - (tpp - 1);
+            xs_begin = gb - ((gb % V) + V) % V;
+            __syncthreads();                                         // the previous item's windows have been read
+            if (vec16) {
+#pragma unroll 1
+                for (int v = tid; v < xs_len / V; v += nth) {
+                    const int64_t i = xs_begin + (int64_t)v * V;
+                    if (i >= 0 && i + V <= nx) {
+                        __pipeline_memcpy_async(&xs[v * V], &xc[i], 16);
+                    } else {
+#pragma unroll
+                        for (int k = 0; k < V; ++k) {
+                            if (i + k >= 0 && i + k < nx) xs[v * V + k] = xc[i + k];
+                            else xs[v * V + k] = rs_zero((EX*)nullptr);
+                        }
+                    }
+                }
+                __pipeline_commit();
+                __pipeline_wait_prior(0);
+            } else {
+#pragma unroll 1
+                for (int k = tid; k < xs_len; k += nth) {
+                    const int64_t i = xs_begin + k;
+                    if (i >= 0 && i < nx) xs[k] = xc[i];
+                    else xs[k] = rs_zero((EX*)nullptr);
+                }
+            }
+            __syncthreads();
+        }
+        EO* oc = out + col * nout;
+        for (int jl = tid; jl < tile && j0 + jl < nout; jl += nth)
+            oc[j0 + jl] = arb_output<EX, TR, EO>(j0 + jl, xc, nx, xs, xs_begin, xs_len, bank, dbank, tpp, nphases, n0, acc0, delta);
+    }
 }
 
 struct RsPlanImpl {
@@ -494,6 +569,8 @@ struct RsPlanImpl {
     std::vector<float> h8_32;    // host copies of d_pfb8 (kernel-parameter taps of resample_mp2_kernel)
     std::vector<double> h8_64;
     bool arbitrary = false;
+    size_t arb_occ_smem = 0;     // resident resample_arb_batch_kernel CTAs per SM for the last (smem, threads) launched
+    int arb_occ_threads = 0, arb_per_sm = 0;
     int64_t tpp8 = 0;
     size_t smem_optin = 0;
     DevBuf in, out;
@@ -682,34 +759,76 @@ static int rs_run(RsPlanImpl* p, const RsArgs& a, cudaStream_t st) {
 
 using namespace dspb200;
 
+// Tile of resample_arb_batch_kernel: the largest power of two T in [32, 1024] whose staged span -- at most
+// ceil((T-1)*delta/Nphi) + tpp + 1 samples (the window of output j0 + T-1 starts at most ceil((T-1)*delta/Nphi) samples
+// after that of j0, +1 for the rounding of the phase), plus up to 16 bytes of alignment in front, rounded up to 16 bytes --
+// takes at most RS_ARB_SPAN_MAX bytes.  Both tap banks are staged when together they take at most RS_ARB_BANKS_MAX bytes, so
+// a CTA never asks for more than 192 KB.  Without a fitting T nothing is staged (T = 256).
+constexpr size_t RS_ARB_SPAN_MAX = 96 * 1024, RS_ARB_BANKS_MAX = 96 * 1024;
+struct RsArbTiling { int tile, threads, xs_len, banks_in_smem; size_t smem; };
+
+static RsArbTiling rs_arb_tiling(int64_t tpp, int64_t nphases, double delta, size_t x_bytes, size_t tap_bytes) {
+    RsArbTiling t{256, 256, 0, 0, 0};
+    const size_t bank_bytes = 2 * (size_t)(nphases * tpp) * tap_bytes;
+    t.banks_in_smem = bank_bytes <= RS_ARB_BANKS_MAX;
+    const int64_t V = 16 / (int64_t)x_bytes;
+    for (int T = 1024; T >= 32; T /= 2) {
+        const double steps = ceil((double)(T - 1) * delta / (double)nphases);
+        if (steps * (double)x_bytes > (double)RS_ARB_SPAN_MAX) continue;
+        const int64_t span = (int64_t)steps + tpp + 1;
+        const int64_t xs_len = (span + V - 1 + V - 1) / V * V;
+        if ((size_t)xs_len * x_bytes > RS_ARB_SPAN_MAX) continue;
+        t.tile = T;
+        t.xs_len = (int)xs_len;
+        break;
+    }
+    t.threads = t.tile < RS_ARB_NT ? t.tile : RS_ARB_NT;
+    t.smem = (size_t)t.xs_len * x_bytes + (t.banks_in_smem ? bank_bytes : 0);
+    return t;
+}
+
 template <typename EX, typename TR, typename EO>
-static int rs_arb_launch(RsPlanImpl* p, const void* x, int64_t nx, int64_t n0, double acc0, double delta, void* out, int64_t nout,
-                         cudaStream_t st) {
-    const size_t bank_bytes = (size_t)(p->interp * p->tpp) * sizeof(TR) * 2;
-    const int in_smem = bank_bytes <= 96 * 1024;
-    const size_t smem = in_smem ? bank_bytes : 0;
-    auto kern = resample_arb_kernel<EX, TR, EO>;
-    if (smem > 48 * 1024) DSP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int64_t blocks = cdiv(nout, RS_NT);
-    DSP_REQUIRE(blocks < (int64_t)0x7fffffff, "too many outputs for one launch");
-    kern<<<(unsigned)blocks, RS_NT, smem, st>>>((const EX*)x, nx, (const TR*)p->d_pfb, (const TR*)p->d_dpfb, (int)p->tpp,
-                                                (int)p->interp, n0, acc0, delta, (EO*)out, nout, in_smem);
+static int rs_arb_launch(RsPlanImpl* p, const void* x, int64_t nx, int64_t ldx, int64_t ncols, int64_t n0, double acc0,
+                         double delta, void* out, int64_t nout, cudaStream_t st) {
+    if (nout == 0 || ncols == 0) return DSPB200_OK;
+    const RsArbTiling t = rs_arb_tiling(p->tpp, p->interp, delta, sizeof(EX), sizeof(TR));
+    DSP_REQUIRE(t.smem <= p->smem_optin, "arbitrary-rate tile needs %zu bytes of shared memory", t.smem);
+    auto kern = resample_arb_batch_kernel<EX, TR, EO>;
+    static bool attr_set = false;                                    // per instantiation
+    if (!attr_set) {
+        DSP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_optin));
+        attr_set = true;
+    }
+    if (p->arb_occ_smem != t.smem || p->arb_occ_threads != t.threads) {
+        int n = 0;
+        DSP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, t.threads, t.smem));
+        p->arb_per_sm = n < 1 ? 1 : n;
+        p->arb_occ_smem = t.smem;
+        p->arb_occ_threads = t.threads;
+    }
+    const int64_t tiles_per_col = cdiv(nout, t.tile), total = tiles_per_col * ncols;
+    int64_t grid = (int64_t)device_sm_count() * p->arb_per_sm;
+    if (grid > total) grid = total;
+    const int vec16 = ((uintptr_t)x % 16 == 0) && ((size_t)ldx * sizeof(EX)) % 16 == 0;
+    kern<<<(unsigned)grid, t.threads, t.smem, st>>>((const EX*)x, nx, ldx, (const TR*)p->d_pfb, (const TR*)p->d_dpfb,
+                                                    (int)p->tpp, (int)p->interp, t.banks_in_smem, n0, acc0, delta, (EO*)out,
+                                                    nout, t.tile, t.xs_len, vec16, tiles_per_col, total);
     DSP_LAUNCH_OK();
     return DSPB200_OK;
 }
 
-static int rs_arb_run(RsPlanImpl* p, const void* x, int64_t nx, int64_t n0, double acc0, double delta, void* out, int64_t nout,
-                      cudaStream_t st) {
+static int rs_arb_run(RsPlanImpl* p, const void* x, int64_t nx, int64_t ldx, int64_t ncols, int64_t n0, double acc0,
+                      double delta, void* out, int64_t nout, cudaStream_t st) {
     const bool o64 = p->dtype_out == DSPB200_F64 || p->dtype_out == DSPB200_C64;
     switch (p->dtype_x) {
         case DSPB200_F32:
-            return o64 ? rs_arb_launch<float, double, double>(p, x, nx, n0, acc0, delta, out, nout, st)
-                       : rs_arb_launch<float, float, float>(p, x, nx, n0, acc0, delta, out, nout, st);
-        case DSPB200_F64: return rs_arb_launch<double, double, double>(p, x, nx, n0, acc0, delta, out, nout, st);
+            return o64 ? rs_arb_launch<float, double, double>(p, x, nx, ldx, ncols, n0, acc0, delta, out, nout, st)
+                       : rs_arb_launch<float, float, float>(p, x, nx, ldx, ncols, n0, acc0, delta, out, nout, st);
+        case DSPB200_F64: return rs_arb_launch<double, double, double>(p, x, nx, ldx, ncols, n0, acc0, delta, out, nout, st);
         case DSPB200_C32:
-            return o64 ? rs_arb_launch<cx<float>, double, cx<double>>(p, x, nx, n0, acc0, delta, out, nout, st)
-                       : rs_arb_launch<cx<float>, float, cx<float>>(p, x, nx, n0, acc0, delta, out, nout, st);
-        default: return rs_arb_launch<cx<double>, double, cx<double>>(p, x, nx, n0, acc0, delta, out, nout, st);
+            return o64 ? rs_arb_launch<cx<float>, double, cx<double>>(p, x, nx, ldx, ncols, n0, acc0, delta, out, nout, st)
+                       : rs_arb_launch<cx<float>, float, cx<float>>(p, x, nx, ldx, ncols, n0, acc0, delta, out, nout, st);
+        default: return rs_arb_launch<cx<double>, double, cx<double>>(p, x, nx, ldx, ncols, n0, acc0, delta, out, nout, st);
     }
 }
 
@@ -857,37 +976,50 @@ int dspb200_resample_arb_plan_create(dspb200_resample_plan** plan, int dtype_x, 
     return DSPB200_OK;
 }
 
-int dspb200_resample_arb_exec_dev(dspb200_resample_plan* plan, const void* x, int64_t nx, int64_t n0, double acc0, double delta,
-                                  void* out, int64_t nout, void* stream) {
-    DSP_RANGE("dspb200_resample_arb_exec_dev");
+int dspb200_resample_arb_batch_exec_dev(dspb200_resample_plan* plan, const void* x, int64_t nx, int64_t ldx, int64_t ncols,
+                                        int64_t n0, double acc0, double delta, void* out, int64_t nout, void* stream) {
+    DSP_RANGE("dspb200_resample_arb_batch_exec_dev");
     DSP_REQUIRE(plan != nullptr, "plan is NULL");
     RsPlanImpl* p = &plan->impl;
     DSP_REQUIRE(p->arbitrary, "not an arbitrary-rate plan");
-    DSP_REQUIRE(nx >= 0 && nout >= 0, "negative size");
+    DSP_REQUIRE(nx >= 0 && nout >= 0 && ncols >= 0, "negative size");
+    DSP_REQUIRE(ldx >= nx, "column stride ldx < nx");
     DSP_REQUIRE(delta > 0.0 && acc0 >= 0.0 && acc0 < (double)p->interp, "bad phase state");
-    if (nout == 0) return DSPB200_OK;
+    if (nout == 0 || ncols == 0) return DSPB200_OK;
     DSP_REQUIRE(out != nullptr && (x != nullptr || nx == 0), "NULL argument");
-    return rs_arb_run(p, x, nx, n0, acc0, delta, out, nout, (cudaStream_t)stream);
+    return rs_arb_run(p, x, nx, ldx, ncols, n0, acc0, delta, out, nout, (cudaStream_t)stream);
+}
+
+int dspb200_resample_arb_exec_dev(dspb200_resample_plan* plan, const void* x, int64_t nx, int64_t n0, double acc0, double delta,
+                                  void* out, int64_t nout, void* stream) {
+    return dspb200_resample_arb_batch_exec_dev(plan, x, nx, nx, 1, n0, acc0, delta, out, nout, stream);
+}
+
+int dspb200_resample_arb_batch_exec(dspb200_resample_plan* plan, const void* x, int64_t nx, int64_t ldx, int64_t ncols,
+                                    int64_t n0, double acc0, double delta, void* out, int64_t nout) {
+    DSP_RANGE("dspb200_resample_arb_batch_exec");
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    DSP_REQUIRE(nx >= 0 && nout >= 0 && ncols >= 0, "negative size");
+    DSP_REQUIRE(ldx >= nx, "column stride ldx < nx");
+    if (nout == 0 || ncols == 0) return DSPB200_OK;
+    DSP_REQUIRE(out != nullptr && (x != nullptr || ldx == 0), "NULL argument");
+    RsPlanImpl* p = &plan->impl;
+    DSP_CUDA(cudaSetDevice(p->device));
+    if (!p->stream) DSP_CUDA(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
+    const size_t in_bytes = (size_t)(ldx * ncols) * dtype_size(p->dtype_x);
+    const size_t out_bytes = (size_t)(nout * ncols) * dtype_size(p->dtype_out);
+    DSP_TRY(p->in.reserve(in_bytes ? in_bytes : 16));
+    DSP_TRY(p->out.reserve(out_bytes));
+    if (in_bytes) DSP_CUDA(cudaMemcpyAsync(p->in.p, x, in_bytes, cudaMemcpyHostToDevice, p->stream));
+    DSP_TRY(dspb200_resample_arb_batch_exec_dev(plan, p->in.p, nx, ldx, ncols, n0, acc0, delta, p->out.p, nout, p->stream));
+    DSP_CUDA(cudaMemcpyAsync(out, p->out.p, out_bytes, cudaMemcpyDeviceToHost, p->stream));
+    DSP_CUDA(cudaStreamSynchronize(p->stream));
+    return DSPB200_OK;
 }
 
 int dspb200_resample_arb_exec(dspb200_resample_plan* plan, const void* x, int64_t nx, int64_t n0, double acc0, double delta,
                               void* out, int64_t nout) {
-    DSP_RANGE("dspb200_resample_arb_exec");
-    DSP_REQUIRE(plan != nullptr, "plan is NULL");
-    DSP_REQUIRE(nx >= 0 && nout >= 0, "negative size");
-    if (nout == 0) return DSPB200_OK;
-    DSP_REQUIRE(out != nullptr && (x != nullptr || nx == 0), "NULL argument");
-    RsPlanImpl* p = &plan->impl;
-    DSP_CUDA(cudaSetDevice(p->device));
-    if (!p->stream) DSP_CUDA(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
-    const size_t in_bytes = (size_t)nx * dtype_size(p->dtype_x), out_bytes = (size_t)nout * dtype_size(p->dtype_out);
-    DSP_TRY(p->in.reserve(in_bytes ? in_bytes : 16));
-    DSP_TRY(p->out.reserve(out_bytes));
-    if (in_bytes) DSP_CUDA(cudaMemcpyAsync(p->in.p, x, in_bytes, cudaMemcpyHostToDevice, p->stream));
-    DSP_TRY(dspb200_resample_arb_exec_dev(plan, p->in.p, nx, n0, acc0, delta, p->out.p, nout, p->stream));
-    DSP_CUDA(cudaMemcpyAsync(out, p->out.p, out_bytes, cudaMemcpyDeviceToHost, p->stream));
-    DSP_CUDA(cudaStreamSynchronize(p->stream));
-    return DSPB200_OK;
+    return dspb200_resample_arb_batch_exec(plan, x, nx, nx, 1, n0, acc0, delta, out, nout);
 }
 
 int dspb200_resample_plan_destroy(dspb200_resample_plan* plan) {

@@ -387,15 +387,49 @@ def filt_multirate(h, x, ratio, nphases=32):
     return FIRFilter(h, ratio, nphases).filt(x)
 
 
+def _arb_resample_call(sf, nx):
+    """The filt! call that resample(x, rate::AbstractFloat) makes on each column (src/Filters/stream_filt.jl:696-725), as
+    arguments of the arbitrary-rate kernel on the column itself.  sf is a fresh FIRArbitrary filter; undelay! (:706-714)
+    is applied here.  The reference zero-pads the column to one sample more than inputlength(outLen, RoundUp) (:699) and
+    filters [history; padded column]: the kernel sees the same samples when it reads min(nx, npad) samples of the column,
+    zero elsewhere, with the newest sample of output 0 at index inputDeficit - 1.  The extra padding sample only
+    guarantees that the exact count of outputs reaches outLen; the retained outputs never see it.
+    Returns (outLen, samples read per column, n0, outputs the padded call would produce)."""
+    outlen = math.ceil(nx * sf.rate)                                                          # :698
+    sf.setphase(sf.timedelay())                                                               # undelay!
+    npad = max(sf.inputlength(outlen, round_up=True), 0) + 1
+    avail = 0
+    if npad >= sf.input_deficit:                                                              # :590-594
+        avail = _arb_advance(sf.phi_accumulator, sf.input_deficit, sf.delta, sf.nphases, npad)[0]
+    return outlen, min(nx, npad), sf.input_deficit - 1, avail
+
+
 def _resample_arbitrary(x, rate, h, nphases, dims):
     """resample(x, rate::AbstractFloat[, h, Nphi]; dims), src/Filters/stream_filt.jl:692-704, 751-775: a fresh FIRArbitrary
-    filter per column, undelay!, zero-padding to inputlength(outLen, RoundUp), first ceil(length * rate) outputs."""
-    if isinstance(x, DeviceArray):
-        raise NotImplementedError("arbitrary-rate resampling of a DeviceArray: copy to the host first")
-    x = np.asarray(x)
+    filter per column, undelay!, zero-padding to inputlength(outLen, RoundUp), first ceil(length * rate) outputs.  Every
+    column has the same phase state, so all columns go to the device in one launch.  A DeviceArray (a vector or a
+    column-major len x nchan matrix resampled along dims=0) stays in device memory."""
+    dev = isinstance(x, DeviceArray)
+    if not dev:
+        x = np.asarray(x)
     if not rate > 0.0:
         raise DomainError("rate must be greater than 0")
     sf = FIRFilter(h, rate, nphases)
+    if dev:
+        if x.ndim > 2 or (x.ndim == 2 and dims not in (None, 0)):
+            raise ArgumentError("a DeviceArray is resampled as a vector or a len x nchan matrix along dims=0")
+        nx = x.shape[0]
+        ncols = x.shape[1] if x.ndim == 2 else 1
+        outlen, m, n0, avail = _arb_resample_call(sf, nx)
+        if ncols and avail < outlen:
+            raise AssertionError("Resample output shorter than expected.")                   # :722
+        plan = _lib.ResampleArbPlan(x.dtype, sf.h, sf.nphases)
+        out = DeviceArray((outlen, ncols) if x.ndim == 2 else (outlen,), plan.out_dtype)
+        plan.exec_batch_dev(x.ptr, m, nx, ncols, n0, sf.phi_accumulator, sf.delta, out.ptr, outlen, 0)
+        from .device import sync
+        sync()
+        plan.close()
+        return out
     if x.ndim > 1:
         if dims is None:
             raise ArgumentError("resample of an array needs `dims`")
@@ -404,25 +438,21 @@ def _resample_arbitrary(x, rate, h, nphases, dims):
         xm = x
     nx = xm.shape[0]
     cols = xm.reshape(nx, -1)
-    outlen = math.ceil(nx * rate)                                                             # :698
-    res = None
-    for c in range(cols.shape[1]):
-        sf.reset()
-        sf.setphase(sf.timedelay())                                                           # undelay!, :706-714
-        # one sample more than inputlength(outLen, RoundUp) (:699): the extra zero only guarantees that the exact count
-        # of outputs reaches outLen; the retained outputs never see it
-        npad = max(sf.inputlength(outlen, round_up=True), 0) + 1
-        xp = np.zeros(npad, dtype=cols.dtype)
-        m = min(nx, npad)
-        xp[:m] = cols[:m, c]
-        y = sf.filt(xp)
-        if y.size < outlen:
-            raise AssertionError("Resample output shorter than expected.")                   # :722
-        if res is None:
-            res = np.empty((outlen, cols.shape[1]), dtype=y.dtype, order="F")
-        res[:, c] = y[:outlen]
-    if res is None:
+    ncols = cols.shape[1]
+    outlen, m, n0, avail = _arb_resample_call(sf, nx)
+    if ncols == 0:
         res = np.empty((outlen, 0), dtype=np.float64)
+    else:
+        if avail < outlen:
+            raise AssertionError("Resample output shorter than expected.")                   # :722
+        xdt = _gpu_dtype(_promote(cols))
+        plan = _lib.ResampleArbPlan(xdt, sf.h, sf.nphases)
+        res = np.empty((outlen, ncols), dtype=plan.out_dtype, order="F")
+        if x.ndim > 1:
+            plan.exec_batch(np.asfortranarray(cols, dtype=xdt), m, nx, ncols, n0, sf.phi_accumulator, sf.delta, res, outlen)
+        else:
+            plan.exec(np.ascontiguousarray(cols[:m, 0], dtype=xdt), m, n0, sf.phi_accumulator, sf.delta, res[:, 0], outlen)
+        plan.close()
     if x.ndim > 1:
         return np.moveaxis(res.reshape((outlen,) + xm.shape[1:]), 0, dims)
     return res.reshape(outlen)
@@ -448,14 +478,15 @@ def resample(x, rate, h=None, nphases=32, dims=None):
     if np.iscomplexobj(h):
         raise NotImplementedError("complex resampling taps are outside the GPU hot-path scope")
     hT = np.ascontiguousarray(h, dtype=np.float32 if h.dtype == np.float32 else np.float64)
-    if dev:                                              # device pipeline form (vector)
-        if x.ndim != 1:
-            raise ArgumentError("device resample takes a vector")
+    if dev:                                              # device pipeline form: a vector or a len x nchan matrix along dims=0
+        if x.ndim > 2 or (x.ndim == 2 and dims not in (None, 0)):
+            raise ArgumentError("a DeviceArray is resampled as a vector or a len x nchan matrix along dims=0")
         nout = math.ceil(x.shape[0] * rate)
+        ncols = x.shape[1] if x.ndim == 2 else 1
         n0, phi0 = resample_phase(hT.size, rate)
         plan = _lib.ResamplePlan(x.dtype, hT, rate.numerator, rate.denominator)
-        out = DeviceArray((nout,), plan.out_dtype)
-        plan.exec_dev(x.ptr, x.shape[0], 1, n0, phi0, out.ptr, nout, 0)
+        out = DeviceArray((nout, ncols) if x.ndim == 2 else (nout,), plan.out_dtype)
+        plan.exec_dev(x.ptr, x.shape[0], ncols, n0, phi0, out.ptr, nout, 0)
         from .device import sync
         sync()
         plan.close()

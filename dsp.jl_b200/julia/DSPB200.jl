@@ -435,6 +435,31 @@ function resample(x::Vector{Tx}, rate::AbstractFloat, h::Vector{Th}=Filters.resa
     return resize!(y, outlen)
 end
 
+# DSP.resample(X, rate::AbstractFloat, h, Nϕ; dims) of a matrix, src/Filters/stream_filt.jl:751-775.  Every column gets a
+# fresh filter after undelay!, so all columns share (n0, acc0, delta) and run in one launch.  The kernel reads
+# min(size(X, dims), npad) samples of each column (npad: the padded length of the vector method), zero elsewhere.
+function resample(X::Matrix{Tx}, rate::AbstractFloat, h::Vector{Th}=Filters.resample_filter(rate), Nϕ::Integer=32;
+                  dims::Integer) where {Tx<:GPUNumber,Th<:GPUReal}
+    Xc = dims == 1 ? X : dims == 2 ? permutedims(X) : throw(ArgumentError("dims must be 1 or 2"))
+    nx, ncols = size(Xc)
+    sf = Filters.FIRFilter(h, rate, Nϕ)
+    Filters.setphase!(sf, Filters.timedelay(sf))                 # undelay!, :706-714
+    kern = sf.kernel
+    outlen = ceil(Int, nx * rate)
+    npad = max(Filters.inputlength(sf, outlen, RoundUp), 0) + 1
+    if ncols > 0
+        avail = npad < kern.inputDeficit ? 0 : arb_advance(kern.ϕAccumulator, kern.inputDeficit, kern.Δ, kern.Nϕ, npad)[1]
+        avail >= outlen || throw(AssertionError("Resample output shorter than expected."))  # :722
+    end
+    out = Matrix{promote_type(Th, Tx)}(undef, outlen, ncols)
+    plan = arb_plan(Tx, h, Nϕ)
+    GC.@preserve Xc out check(ccall((:dspb200_resample_arb_batch_exec, libdspb200), Cint,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Int64, Int64, Int64, Int64, Cdouble, Cdouble, Ptr{Cvoid}, Int64),
+        plan.ptr, Xc, min(nx, npad), nx, ncols, kern.inputDeficit - 1, kern.ϕAccumulator, kern.Δ, out, outlen))
+    close!(plan)
+    return dims == 1 ? out : permutedims(out)
+end
+
 # ---- conv(u, v) for matrices / rank-3 arrays (src/dspbase.jl:611-660) and periodogram(s::Matrix) (src/periodograms.jl:473-509)
 function conv_nd!(out::Array{T,N}, u::Array{T,N}, v::Array{T,N}; algorithm::Symbol=:auto) where {T<:GPUNumber,N}
     # algorithm resolution of conv!, src/dspbase.jl:720-751

@@ -262,6 +262,14 @@ DSPB200_API int dspb200_resample_arb_exec(dspb200_resample_plan* plan, const voi
                                           double delta, void* out, int64_t nout);
 DSPB200_API int dspb200_resample_arb_exec_dev(dspb200_resample_plan* plan, const void* x, int64_t nx, int64_t n0, double acc0,
                                               double delta, void* out, int64_t nout, void* stream);
+/* Column c holds samples x[c*ldx + i], i in [0, nx), zero elsewhere (ldx >= nx); output column c is out[c*nout + j].
+ * Every column uses the same (n0, acc0, delta) -- a fresh filter after undelay!, as resample(X, rate; dims) does.
+ * One kernel launch for all columns; ncols == 0 launches nothing. */
+DSPB200_API int dspb200_resample_arb_batch_exec(dspb200_resample_plan* plan, const void* x, int64_t nx, int64_t ldx,
+                                                int64_t ncols, int64_t n0, double acc0, double delta, void* out, int64_t nout);
+DSPB200_API int dspb200_resample_arb_batch_exec_dev(dspb200_resample_plan* plan, const void* x, int64_t nx, int64_t ldx,
+                                                    int64_t ncols, int64_t n0, double acc0, double delta, void* out,
+                                                    int64_t nout, void* stream);
 DSPB200_API int dspb200_resample_plan_destroy(dspb200_resample_plan* plan);
 
 #ifdef __cplusplus
