@@ -4,6 +4,7 @@ Host-side mirror of the reference's call signatures for that path (the Julia glu
 the same thin layer over the same C ABI, include/dspb200.h):
 
     filt, filt_, conv, conv_, optimalfftfiltlength                    (src/dspbase.jl)
+    PolynomialRatio, coefb, coefa, DF2TFilter (FIR)                    (src/Filters/coefficients.jl, src/Filters/filt.jl)
     fftfilt, fftfilt_, tdfilt, tdfilt_, resample, resample_filter      (src/Filters)
     periodogram, welch_pgram, welch_pgram_, WelchConfig, spectrogram, stft, power, freq, time
                                                                        (src/periodograms.jl)
@@ -16,10 +17,11 @@ name `dspb200` by the shim `dspb200.py` at the repository root.
 from . import _lib
 from ._lib import DSPB200Error, device_count, launch_count
 from .device import DeviceArray, sync, to_device, to_host
-from .errors import ArgumentError, DimensionMismatch, DomainError
+from .errors import ArgumentError, DimensionMismatch, DomainError, InexactError
 from .util import fftabs2type, fftintype, fftouttype, nextfastfft, rfftfreq, fftfreq
 from .windows import bartlett, hamming, hann, hanning, kaiser, rect
 from .dspbase import SMALL_FILT_CUTOFF, conv, conv_, filt, filt_, optimalfftfiltlength, os_fft_complexity
+from .df2t import DF2TFilter, PolynomialRatio, coefa, coefb
 from .filters import (FIRFilter, fftfilt, fftfilt_, filt_multirate, inputlength, kaiserord, outputlength, resample,
                       resample_filter, resample_phase, tdfilt, tdfilt_)
 from .filters import filt_ as filt_hx_

@@ -52,6 +52,8 @@ SIGNATURES = {
     "dspb200_fir_plan_create": (_int, [_pp, _int, _vp, _i64]),
     "dspb200_fir_exec": (_int, [_vp, _vp, _i64, _i64, _vp]),
     "dspb200_fir_exec_dev": (_int, [_vp, _vp, _i64, _i64, _vp, _vp]),
+    "dspb200_fir_exec_state": (_int, [_vp, _vp, _i64, _i64, _vp, _vp, _vp]),
+    "dspb200_fir_exec_state_dev": (_int, [_vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp]),
     "dspb200_fir_plan_destroy": (_int, [_vp]),
     "dspb200_os_plan_create": (_int, [_pp, _int, _vp, _i64, _i64]),
     "dspb200_os_plan_nfft": (_int, [_vp, C.POINTER(_i64), C.POINTER(_int)]),
@@ -183,6 +185,14 @@ class FirPlan(_Plan):
 
     def exec_dev(self, x_ptr, nx, ncols, out_ptr, stream=0):
         check(lib.dspb200_fir_exec_dev(self.handle, x_ptr, nx, ncols, out_ptr, stream))
+
+    def exec_state(self, x, nx, ncols, si_in, si_out, out):
+        """Host arrays, Fortran-ordered: x / out nx x ncols, si_in / si_out (nb-1) x ncols (None: zero / discarded)."""
+        check(lib.dspb200_fir_exec_state(self.handle, ptr(x), nx, ncols, None if si_in is None else ptr(si_in),
+                                         None if si_out is None else ptr(si_out), ptr(out)))
+
+    def exec_state_dev(self, x_ptr, nx, ncols, si_in_ptr, si_out_ptr, out_ptr, stream=0):
+        check(lib.dspb200_fir_exec_state_dev(self.handle, x_ptr, nx, ncols, si_in_ptr, si_out_ptr, out_ptr, stream))
 
 
 class OsPlan(_Plan):

@@ -7,8 +7,14 @@
 // chunk, 128-bit loads) evaluates exactly that chain per output, so Float32/Float64 results match the reference bit for bit
 // on FMA hardware.  It stages the x tile (+ tap-chunk halo) and the tap chunk in shared memory, padded so that the
 // sliding-window reads are bank-conflict free.
+//
+// The stateful form (DF2TFilter / filt(b, 1, x, si), src/Filters/filt.jl:157-181, src/deprecated.jl:80-101) is the same
+// kernel with STATE = true: in transposed direct form the FIR state is the partial chain of the next nb - 1 outputs, so
+// the call evaluates outputs 0 .. nx + nb - 2 of the column, seeds outputs i < nb - 1 with si_in[i] and stores outputs
+// nx + j as si_out[j].  Filtering in chunks is therefore bit-identical to filtering in one call.
 #include "common.cuh"
 #include "fir_tile.cuh"
+#include <cstring>
 #include <new>
 
 namespace dspb200 {
@@ -18,10 +24,15 @@ template <typename T> struct fir_elt<T, true> { using type = cx<T>; };
 
 // ---------------------------------------------------------------------------------------------- register-tiled kernel
 // fir_tile.cuh: a thread owns G consecutive outputs, 8 taps per chunk, two 8-sample register runs that swap roles.
-template <typename E, int NT>
-__global__ void __launch_bounds__(NT)
+// STATE (DF2TFilter, filt(b, a, x, si)): a column has nx + nb - 1 outputs; outputs i < nb - 1 start their chain from
+// si_in[i], outputs i >= nx are the final state si_out[i - nx] (fir_tile.cuh, fir_state_init / fir_state_store).
+// si_in / si_out hold nb - 1 elements per column and may be NULL (zero state / state not wanted).  The STATE instances ask
+// for one resident CTA per SM at least: without that bound ptxas keeps the ComplexF32 256-thread instance at 64 registers
+// and spills the state pointers.
+template <typename E, int NT, bool STATE>
+__global__ void __launch_bounds__(NT, STATE ? 1 : 0)
 fir_tile_kernel(const E* __restrict__ x, int64_t nx, int64_t tiles_per_col, const E* __restrict__ b, int nb,
-                E* __restrict__ out) {
+                E* __restrict__ out, const E* __restrict__ si_in, E* __restrict__ si_out) {
     using Gm = fir_geom<E, NT>;
     constexpr int G = Gm::G;
     __shared__ __align__(16) E xs[Gm::XS];
@@ -33,8 +44,12 @@ fir_tile_kernel(const E* __restrict__ x, int64_t nx, int64_t tiles_per_col, cons
     const E* xc = x + col * nx;
     E* oc = out + col * nx;
     E acc[G];
+    if constexpr (STATE) {
+        fir_state_init<E, G>(acc, i0 + (int64_t)G * tid, si_in ? si_in + col * (nb - 1) : nullptr, nb);
+    } else {
 #pragma unroll
-    for (int o = 0; o < G; ++o) acc[o] = fir_zero((E*)nullptr);
+        for (int o = 0; o < G; ++o) acc[o] = fir_zero((E*)nullptr);
+    }
     const int nb8 = (nb + 7) & ~7;                                      // taps nb .. nb8-1 are padding (skipped)
     for (int k_hi = nb8 - 1; k_hi >= 0; k_hi -= Gm::KC) {
         const int kc = k_hi + 1 < Gm::KC ? k_hi + 1 : Gm::KC;           // padded taps k_hi, k_hi-1, .., k_hi-kc+1 (a multiple of 8)
@@ -47,6 +62,8 @@ fir_tile_kernel(const E* __restrict__ x, int64_t nx, int64_t tiles_per_col, cons
     if (i + G <= nx && (reinterpret_cast<uintptr_t>(oc + i) & 15) == 0) {
 #pragma unroll
         for (int v = 0; v < G; v += Gm::VEC) *reinterpret_cast<uint4*>(oc + i + v) = *reinterpret_cast<const uint4*>(&acc[v]);
+    } else if constexpr (STATE) {
+        fir_state_store<E, G>(acc, i, nx, nb, oc, si_out ? si_out + col * (nb - 1) : nullptr);
     } else {
 #pragma unroll
         for (int o = 0; o < G; ++o)
@@ -54,12 +71,39 @@ fir_tile_kernel(const E* __restrict__ x, int64_t nx, int64_t tiles_per_col, cons
     }
 }
 
+// 128-thread tiles when the 256-thread grid would not cover every SM eight times over, so short inputs still spread
+// over the whole GPU.  nout = outputs per column (nx, or nx + nb - 1 with STATE).
+template <typename E, bool STATE>
+static int fir_launch(const E* x, int64_t nx, int64_t nout, int64_t ncols, const E* b, int nb, E* out, const E* si_in, E* si_out,
+                      cudaStream_t st) {
+    const bool small = cdiv(nout, fir_geom<E, 256>::TILE) * ncols < (int64_t)8 * device_sm_count();
+    const int64_t tiles = cdiv(nout, small ? fir_geom<E, 128>::TILE : fir_geom<E, 256>::TILE), blocks = tiles * ncols;
+    DSP_REQUIRE(blocks < (int64_t)0x7fffffff, "too many tiles for one launch");
+    if (small) fir_tile_kernel<E, 128, STATE><<<(unsigned)blocks, 128, 0, st>>>(x, nx, tiles, b, nb, out, si_in, si_out);
+    else fir_tile_kernel<E, 256, STATE><<<(unsigned)blocks, 256, 0, st>>>(x, nx, tiles, b, nb, out, si_in, si_out);
+    DSP_LAUNCH_OK();
+    return DSPB200_OK;
+}
+
+template <bool STATE>
+static int fir_dispatch(int dtype, const void* x, int64_t nx, int64_t nout, int64_t ncols, const void* b, int nb, void* out,
+                        const void* si_in, void* si_out, cudaStream_t st) {
+#define FIR_CALL(E_) fir_launch<E_, STATE>((const E_*)x, nx, nout, ncols, (const E_*)b, nb, (E_*)out, (const E_*)si_in, (E_*)si_out, st)
+    switch (dtype) {
+        case DSPB200_F32: return FIR_CALL(float);
+        case DSPB200_F64: return FIR_CALL(double);
+        case DSPB200_C32: return FIR_CALL(cx<float>);
+        default: return FIR_CALL(cx<double>);
+    }
+#undef FIR_CALL
+}
+
 struct FirPlanImpl {
     int dtype = 0;
     int64_t nb = 0;
     int device = 0;
     void* d_b = nullptr;
-    DevBuf in, out;
+    DevBuf in, out, state;
     cudaStream_t stream = nullptr;
 };
 
@@ -99,23 +143,73 @@ int dspb200_fir_exec_dev(dspb200_fir_plan* plan, const void* x, int64_t nx, int6
     if (nx == 0 || ncols == 0) return DSPB200_OK;
     DSP_REQUIRE(x && out, "NULL argument");
     FirPlanImpl* p = &plan->impl;
+    return fir_dispatch<false>(p->dtype, x, nx, nx, ncols, p->d_b, (int)p->nb, out, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+int dspb200_fir_exec_state_dev(dspb200_fir_plan* plan, const void* x, int64_t nx, int64_t ncols, const void* si_in, void* si_out,
+                               void* out, void* stream) {
+    DSP_RANGE("dspb200_fir_exec_state_dev");
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    DSP_REQUIRE(nx >= 0 && ncols >= 0, "negative size");
+    FirPlanImpl* p = &plan->impl;
+    const int64_t ns = p->nb - 1;
+    const size_t sbytes = (size_t)(ns * ncols) * dtype_size(p->dtype);
+    const size_t xbytes = (size_t)(nx * ncols) * dtype_size(p->dtype);
+    // Every CTA reads its samples and the tap halo of the tile before it, and the state, while other CTAs write: a buffer
+    // that is written must not overlap one that is read (or the other written one).
+    auto overlap = [](const void* a, size_t na, const void* b, size_t nb_) {
+        return a && b && na && nb_ && (const char*)a < (const char*)b + nb_ && (const char*)b < (const char*)a + na;
+    };
+    DSP_REQUIRE(!overlap(si_in, sbytes, si_out, sbytes), "si_in and si_out overlap");
+    DSP_REQUIRE(!overlap(x, xbytes, out, xbytes), "x and out overlap (filtering in place needs the host form)");
+    DSP_REQUIRE(!overlap(x, xbytes, si_out, sbytes) && !overlap(si_in, sbytes, out, xbytes) && !overlap(out, xbytes, si_out, sbytes),
+                "a state buffer overlaps x or out");
+    if (ncols == 0) return DSPB200_OK;
     cudaStream_t st = (cudaStream_t)stream;
-#define FIR_TILED(E_) do {                                                                                   \
-        /* short inputs: 128-thread tiles, so that the tiles spread evenly over the SMs */                   \
-        const bool small = cdiv(nx, fir_geom<E_, 256>::TILE) * ncols < (int64_t)8 * device_sm_count();       \
-        const int64_t tiles = cdiv(nx, small ? fir_geom<E_, 128>::TILE : fir_geom<E_, 256>::TILE), blocks = tiles * ncols; \
-        DSP_REQUIRE(blocks < (int64_t)0x7fffffff, "too many tiles for one launch");                          \
-        if (small) fir_tile_kernel<E_, 128><<<(unsigned)blocks, 128, 0, st>>>((const E_*)x, nx, tiles, (const E_*)p->d_b, (int)p->nb, (E_*)out); \
-        else fir_tile_kernel<E_, 256><<<(unsigned)blocks, 256, 0, st>>>((const E_*)x, nx, tiles, (const E_*)p->d_b, (int)p->nb, (E_*)out); \
-    } while (0)
-    switch (p->dtype) {
-        case DSPB200_F32: FIR_TILED(float); break;
-        case DSPB200_F64: FIR_TILED(double); break;
-        case DSPB200_C32: FIR_TILED(cx<float>); break;
-        default: FIR_TILED(cx<double>); break;
+    if (nx == 0) {                                                       // the state passes through unchanged
+        if (si_out && sbytes) {
+            if (si_in) DSP_CUDA(cudaMemcpyAsync(si_out, si_in, sbytes, cudaMemcpyDeviceToDevice, st));
+            else DSP_CUDA(cudaMemsetAsync(si_out, 0, sbytes, st));
+        }
+        return DSPB200_OK;
     }
-#undef FIR_TILED
-    DSP_LAUNCH_OK();
+    DSP_REQUIRE(x && out, "NULL argument");
+    if (ns == 0)                                                         // nb == 1: no state, out = x * b[1] (src/Filters/filt.jl:161-162)
+        return fir_dispatch<false>(p->dtype, x, nx, nx, ncols, p->d_b, 1, out, nullptr, nullptr, st);
+    return fir_dispatch<true>(p->dtype, x, nx, nx + ns, ncols, p->d_b, (int)p->nb, out, si_in, si_out, st);
+}
+
+int dspb200_fir_exec_state(dspb200_fir_plan* plan, const void* x, int64_t nx, int64_t ncols, const void* si_in, void* si_out,
+                           void* out) {
+    DSP_RANGE("dspb200_fir_exec_state");
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    DSP_REQUIRE(nx >= 0 && ncols >= 0, "negative size");
+    if (ncols == 0) return DSPB200_OK;
+    DSP_REQUIRE(nx == 0 || (x && out), "NULL argument");
+    FirPlanImpl* p = &plan->impl;
+    const size_t es = dtype_size(p->dtype);
+    const size_t bytes = (size_t)(nx * ncols) * es, sbytes = (size_t)((p->nb - 1) * ncols) * es;
+    if (nx == 0) {                                                       // the state passes through unchanged
+        if (si_out && sbytes && si_out != si_in) {
+            if (si_in) memmove(si_out, si_in, sbytes);
+            else memset(si_out, 0, sbytes);
+        }
+        return DSPB200_OK;
+    }
+    DSP_CUDA(cudaSetDevice(p->device));
+    if (!p->stream) DSP_CUDA(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
+    DSP_TRY(p->in.reserve(bytes));
+    DSP_TRY(p->out.reserve(bytes));
+    DSP_TRY(p->state.reserve(2 * sbytes + 16));                          // [si_in | si_out]: staged apart, so the host pointers may alias
+    char* d_si_in = (char*)p->state.p;
+    char* d_si_out = d_si_in + sbytes;
+    DSP_CUDA(cudaMemcpyAsync(p->in.p, x, bytes, cudaMemcpyHostToDevice, p->stream));
+    if (si_in && sbytes) DSP_CUDA(cudaMemcpyAsync(d_si_in, si_in, sbytes, cudaMemcpyHostToDevice, p->stream));
+    DSP_TRY(dspb200_fir_exec_state_dev(plan, p->in.p, nx, ncols, si_in ? d_si_in : nullptr, si_out ? d_si_out : nullptr, p->out.p,
+                                       p->stream));
+    DSP_CUDA(cudaMemcpyAsync(out, p->out.p, bytes, cudaMemcpyDeviceToHost, p->stream));
+    if (si_out && sbytes) DSP_CUDA(cudaMemcpyAsync(si_out, d_si_out, sbytes, cudaMemcpyDeviceToHost, p->stream));
+    DSP_CUDA(cudaStreamSynchronize(p->stream));
     return DSPB200_OK;
 }
 
@@ -142,7 +236,7 @@ int dspb200_fir_plan_destroy(dspb200_fir_plan* plan) {
     if (!plan) return DSPB200_OK;
     FirPlanImpl* p = &plan->impl;
     if (p->d_b) cudaFree(p->d_b);
-    p->in.release(); p->out.release();
+    p->in.release(); p->out.release(); p->state.release();
     if (p->stream) cudaStreamDestroy(p->stream);
     delete plan;
     return DSPB200_OK;

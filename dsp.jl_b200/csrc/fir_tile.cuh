@@ -124,4 +124,27 @@ __host__ __device__ __forceinline__ void fir_round(int tid, E (&acc)[fir_geom<E,
     }
 }
 
+// Stateful calls (STATE instances of fir_tile_kernel).  The reference's state after i samples is si[j] = the chain of
+// output i + j with the samples from i on left out (src/dspbase.jl:95-105), so a call that starts from si_in evaluates
+// output i < nb - 1 as the usual chain seeded with si_in[i] (the taps that reach before sample 0 multiply zeros and leave
+// the accumulator as it is), and its final state si_out[j] is the chain of the virtual output nx + j over zero samples
+// from nx on.  The thread's outputs are i .. i + G - 1; si_in / si_out are the column's nb - 1 state values, or NULL.
+template <typename E, int G>
+__host__ __device__ __forceinline__ void fir_state_init(E (&acc)[G], int64_t i, const E* __restrict__ si_in, int nb) {
+#pragma unroll
+    for (int o = 0; o < G; ++o) acc[o] = (si_in && i + o < nb - 1) ? si_in[i + o] : fir_zero((E*)nullptr);
+}
+
+// outputs i < nx go to the column's output, outputs nx <= i < nx + nb - 1 to the final state
+template <typename E, int G>
+__host__ __device__ __forceinline__ void fir_state_store(const E (&acc)[G], int64_t i, int64_t nx, int nb, E* __restrict__ oc,
+                                                         E* __restrict__ si_out) {
+#pragma unroll
+    for (int o = 0; o < G; ++o) {
+        const int64_t k = i + o;
+        if (k < nx) oc[k] = acc[o];
+        else if (si_out && k < nx + nb - 1) si_out[k - nx] = acc[o];
+    }
+}
+
 }  // namespace dspb200

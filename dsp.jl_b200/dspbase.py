@@ -53,11 +53,28 @@ def _cols(x, dt):
 
 # --------------------------------------------------------------------------------------------- filt(b, a, x)
 
-def filt(b, a, x=None):
-    """filt(b, a, x) (src/dspbase.jl:14-15) and, with two arguments, Filters.filt(h, x) (src/Filters/filt.jl:445-446)."""
+def filt(b, a, x=None, si=None):
+    """filt(b, a, x) (src/dspbase.jl:14-15) and, with two arguments, Filters.filt(h, x) (src/Filters/filt.jl:445-446),
+    filt(f::DF2TFilter, x) and filt(f::PolynomialRatio, x) (src/Filters/filt.jl:30, 215-224).  The deprecated
+    filt(b, a, x, si) and filt(f::PolynomialRatio, x, si) (src/deprecated.jl) filter from the initial state si (copied)."""
+    from . import df2t
+    if isinstance(b, df2t.DF2TFilter):
+        if x is not None:
+            raise ArgumentError("filt(f::DF2TFilter, x) takes one signal")
+        return b.filt(a)
+    if isinstance(b, df2t.PolynomialRatio):
+        if si is not None:
+            raise ArgumentError("filt(f::PolynomialRatio, x, si) takes three arguments")
+        if x is not None:
+            return df2t.filt_deprecated(b, None, a, x)
+        return filt(b.coefb, b.coefa, a)
+    if si is not None:
+        return df2t.filt_deprecated(b, a, x, si)
     if x is None:
         from .filters import filt as _filt_hx
         return _filt_hx(b, a)
+    if isinstance(x, DeviceArray):
+        return _filt_device(b, a, x)
     from fractions import Fraction
     if isinstance(x, (int, np.integer, Fraction)) and not isinstance(x, bool) and np.ndim(a) == 1 and np.ndim(b) == 1:
         from .filters import filt_multirate                     # filt(h, x, ratio), src/Filters/stream_filt.jl:663-666
@@ -71,8 +88,52 @@ def filt(b, a, x=None):
     return out      # integer inputs are computed and returned as Float64 (no integer GPU kernels)
 
 
-def filt_(out, b, a, x):
-    """filt!(out, b, a, x), src/dspbase.jl:26-66.  FIR only (length(a) == 1); IIR is outside the hot path."""
+def _filt_device(b, a, x):
+    """filt(b, a, x::DeviceArray) with length(a) == 1: the same kernel as the host call, on the device-resident columns of
+    x (its eltype must be promote_type(b, a, x)); returns a DeviceArray."""
+    b = np.atleast_1d(np.asarray(b))
+    a = np.atleast_1d(np.asarray(a))
+    if b.size == 0:
+        raise ArgumentError("filter vector b must be non-empty")
+    if a.size == 0:
+        raise ArgumentError("filter vector a must be non-empty")
+    if a[0] == 0:
+        raise ArgumentError("filter vector a[1] must be nonzero")
+    if a.size != 1:
+        raise NotImplementedError("IIR filtering (length(a) > 1) is outside the GPU hot-path scope (SURVEY.md 8a)")
+    T = _promote(b, a, x)
+    if T != x.dtype:
+        raise ArgumentError(f"filt of a DeviceArray computes in its eltype {x.dtype}, but promote_type(b, a, x) is {T}")
+    if a[0] != 1:                                   # :43-47 coefficient normalisation
+        b = b / a[0]
+    out = DeviceArray(x.shape, T)
+    nx = x.shape[0] if x.ndim else 1
+    if x.size:
+        plan = _lib.FirPlan(np.ascontiguousarray(b, dtype=T))
+        plan.exec_dev(x.ptr, nx, x.size // nx, out.ptr, 0)
+        from .device import sync
+        sync()
+        plan.close()
+    return out
+
+
+def filt_(out, b, a, x=None, si=None):
+    """filt!(out, b, a, x), src/dspbase.jl:26-66.  FIR only (length(a) == 1); IIR is outside the hot path.  Also
+    filt!(out, f::DF2TFilter, x), filt!(out, f::PolynomialRatio, x) (src/Filters/filt.jl:17) and the deprecated
+    filt!(out, b, a, x, si) / filt!(out, f::PolynomialRatio, x, si) (src/deprecated.jl, si copied)."""
+    from . import df2t
+    if isinstance(b, df2t.DF2TFilter):
+        if x is not None:
+            raise ArgumentError("filt!(out, f::DF2TFilter, x) takes one signal")
+        return b.filt_(out, a)
+    if isinstance(b, df2t.PolynomialRatio):
+        if si is not None:
+            raise ArgumentError("filt!(out, f::PolynomialRatio, x, si) takes four arguments")
+        if x is not None:
+            return df2t.filt_deprecated_(out, b, None, a, x)
+        return filt_(out, b.coefb, b.coefa, a)
+    if si is not None:
+        return df2t.filt_deprecated_(out, b, a, x, si)
     b = np.atleast_1d(np.asarray(b))
     a = np.atleast_1d(np.asarray(a))
     x = np.asarray(x)

@@ -9,5 +9,9 @@ class DomainError(ValueError):
     """Julia DomainError (e.g. src/periodograms.jl:44-45, 397, 565)."""
 
 
+class InexactError(ValueError):
+    """Julia InexactError (a value that the destination eltype cannot hold, e.g. a complex sample in a real filter state)."""
+
+
 class DimensionMismatch(ValueError):
     """Julia DimensionMismatch (e.g. src/periodograms.jl:255, 735-737)."""

@@ -97,6 +97,29 @@ function filt!(out::Array{T}, b::Union{AbstractVector,Number}, a::Union{Abstract
 end
 filt(b, a, x::Array{T}) where {T<:GPUNumber} = filt!(similar(x), b, a, x)
 
+# DSP.filt!(out, f::DF2TFilter{<:PolynomialRatio}, x): src/Filters/filt.jl:157-181, FIR coefficient sets whose state and
+# signal share a GPU eltype the coefficients promote into (then the reference computes every muladd in that eltype).
+# The state is staged through the plan, so it is passed as both si_in and si_out and updated in place as the reference does.
+function filt!(out::Array{S,N}, f::Filters.DF2TFilter{<:Filters.PolynomialRatio,Array{S,N}}, x::Array{S,N}) where {S<:GPUNumber,N}
+    size(x) != size(out) && throw(ArgumentError("out size must match x"))
+    si = f.state
+    size(x)[2:end] != size(si)[2:end] && throw(ArgumentError("state size must match x"))
+    b = Filters.coefb(f.coef)
+    (length(Filters.coefa(f.coef)) == 1 && promote_type(eltype(b), S) == S) || return DSP.filt!(out, f, x)
+    iszero(length(x)) && return out
+    bT = convert(Vector{S}, b)
+    h = Ref{Ptr{Cvoid}}(C_NULL)
+    GC.@preserve bT check(ccall((:dspb200_fir_plan_create, libdspb200), Cint,
+        (Ref{Ptr{Cvoid}}, Cint, Ptr{Cvoid}, Int64), h, dtype_code(S), bT, length(bT)))
+    plan = Plan(h[], :dspb200_fir_plan_destroy)
+    nx = size(x, 1)
+    GC.@preserve x out si check(ccall((:dspb200_fir_exec_state, libdspb200), Cint,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Int64, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}), plan.ptr, x, nx, length(x) ÷ nx, si, si, out))
+    close!(plan)
+    return out
+end
+filt(f::Filters.DF2TFilter{<:Filters.PolynomialRatio,Array{S,N}}, x::Array{S,N}) where {S<:GPUNumber,N} = filt!(similar(x), f, x)
+
 # ------------------------------------------------------------------------------------------------ fftfilt / filt(h, x)
 # DSP.Filters.fftfilt(b, x[, nfft]) / fftfilt!: src/Filters/filt.jl:458-521
 function fftfilt!(out::Array{T}, b::Vector{T}, x::Array{T}, nfft::Integer=0) where {T<:GPUReal}

@@ -77,6 +77,21 @@ typedef struct dspb200_fir_plan dspb200_fir_plan;
 DSPB200_API int dspb200_fir_plan_create(dspb200_fir_plan** plan, int dtype, const void* b_host, int64_t nb);
 DSPB200_API int dspb200_fir_exec(dspb200_fir_plan* plan, const void* x, int64_t nx, int64_t ncols, void* out);
 DSPB200_API int dspb200_fir_exec_dev(dspb200_fir_plan* plan, const void* x, int64_t nx, int64_t ncols, void* out, void* stream);
+/* Stateful FIR: filt!(out, DF2TFilter(PolynomialRatio(b, 1), si), x) and the deprecated filt(b, 1, x, si)
+ * (src/Filters/filt.jl:157-181, src/deprecated.jl:80-101).  si_in / si_out hold the transposed direct-form state,
+ * (nb-1) x ncols column-major in the plan's dtype: si_in is the state before x, si_out receives the state after it,
+ * so feeding si_out to the next call filters a chunked stream bit-identically to one call over the whole stream.
+ * si_in == NULL means a zero state, si_out == NULL discards the final state.  nx == 0 passes the state through;
+ * nb == 1 has no state and computes out = x * b[1].  The _dev form takes device pointers, enqueues one kernel on
+ * `stream` and returns; there no two of x, out, si_in and si_out may overlap where one of them is written (x with out,
+ * si_in with si_out, a state buffer with x or out): DSPB200_EINVALID, because CTAs read the samples and state of their
+ * neighbours' outputs.  The host form stages x and the state through plan scratch, so there out may be x (in-place
+ * filtering, as filt!(out, f, x) allows) and si_out may be si_in.  (dspb200_fir_exec_dev has the same restriction on
+ * x and out; it is not checked there.) */
+DSPB200_API int dspb200_fir_exec_state(dspb200_fir_plan* plan, const void* x, int64_t nx, int64_t ncols, const void* si_in,
+                                       void* si_out, void* out);
+DSPB200_API int dspb200_fir_exec_state_dev(dspb200_fir_plan* plan, const void* x, int64_t nx, int64_t ncols, const void* si_in,
+                                           void* si_out, void* out, void* stream);
 DSPB200_API int dspb200_fir_plan_destroy(dspb200_fir_plan* plan);
 
 /* ------------------------------------------------------------------------------------------ overlap-save
