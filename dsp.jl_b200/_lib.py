@@ -107,6 +107,8 @@ SIGNATURES = {
     "dspb200_resample_arb_exec_dev": (_int, [_vp, _vp, _i64, _i64, _dbl, _dbl, _vp, _i64, _vp]),
     "dspb200_resample_arb_batch_exec": (_int, [_vp, _vp, _i64, _i64, _i64, _i64, _dbl, _dbl, _vp, _i64]),
     "dspb200_resample_arb_batch_exec_dev": (_int, [_vp, _vp, _i64, _i64, _i64, _i64, _dbl, _dbl, _vp, _i64, _vp]),
+    "dspb200_resample_stream_exec_dev": (_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _i64, _vp, _i64, _i64, _vp]),
+    "dspb200_resample_arb_stream_exec_dev": (_int, [_vp, _vp, _vp, _vp, _i64, _i64, _i64, _dbl, _dbl, _vp, _i64, _i64, _vp]),
     "dspb200_resample_plan_destroy": (_int, [_vp]),
 }
 for _name, (_res, _args) in SIGNATURES.items():
@@ -339,6 +341,11 @@ class ResamplePlan(_Plan):
         check(lib.dspb200_resample_exec_range_dev(self.handle, x_ptr, x_begin, nx_local, n0, phi0, out_ptr, j_begin,
                                                   nout_local, stream))
 
+    def stream_exec_dev(self, hist_in_ptr, hist_out_ptr, x_ptr, nx, ncols, input_deficit, phi0, out_ptr, ldo, nout, stream=0):
+        """One chunk of a streaming FIRFilter: device pointers, (tpp - 1) x ncols histories (hist_in None: zeros)."""
+        check(lib.dspb200_resample_stream_exec_dev(self.handle, hist_in_ptr, hist_out_ptr, x_ptr, int(nx), int(ncols),
+                                                   int(input_deficit), int(phi0), out_ptr, int(ldo), int(nout), stream))
+
 
 class ResampleArbPlan(_Plan):
     """FIRArbitrary plan: pfb and derivative bank of `h` split into `nphases` phases."""
@@ -369,6 +376,13 @@ class ResampleArbPlan(_Plan):
     def exec_batch_dev(self, x_ptr, nx, ldx, ncols, n0, acc0, delta, out_ptr, nout, stream=0):
         check(lib.dspb200_resample_arb_batch_exec_dev(self.handle, x_ptr, int(nx), int(ldx), int(ncols), int(n0), float(acc0),
                                                       float(delta), out_ptr, int(nout), stream))
+
+    def stream_exec_dev(self, hist_in_ptr, hist_out_ptr, x_ptr, nx, ncols, input_deficit, acc0, delta, out_ptr, ldo, nout,
+                        stream=0):
+        """One chunk of a streaming arbitrary-rate FIRFilter (see ResamplePlan.stream_exec_dev)."""
+        check(lib.dspb200_resample_arb_stream_exec_dev(self.handle, hist_in_ptr, hist_out_ptr, x_ptr, int(nx), int(ncols),
+                                                       int(input_deficit), float(acc0), float(delta), out_ptr, int(ldo),
+                                                       int(nout), stream))
 
 
 def conv_fft(u, v, nfft, out):

@@ -436,6 +436,16 @@ template <typename TR> __device__ __forceinline__ cx<TR> arb_mix(cx<TR> yu, cx<T
     return mkc<TR>((TR)fma((double)yu.x, alpha, (double)yl.x), (TR)fma((double)yu.y, alpha, (double)yl.y));
 }
 
+// Streaming (FIRFilter fed chunk by chunk): a call filters the virtual column v = [history (H = tpp - 1 samples); x (nx
+// samples)] of each channel, zero past its end, without building it.  Sample i of v for one channel: hc holds its history
+// (NULL: zeros), xc its chunk.
+template <typename EX>
+__device__ __forceinline__ EX rs_vsample(const EX* __restrict__ hc, const EX* __restrict__ xc, int64_t H, int64_t nx, int64_t i) {
+    if (i < H) return (hc != nullptr && i >= 0) ? hc[i] : rs_zero((EX*)nullptr);
+    i -= H;
+    return i < nx ? xc[i] : rs_zero((EX*)nullptr);
+}
+
 // P_j = acc0 + j*delta split into q = floor(P_j / Nphi) and r = P_j - q*Nphi in [0, Nphi).
 __device__ __forceinline__ void arb_phase(int64_t j, double N, double acc0, double delta, double* q_out, double* r_out) {
     const double jd = (double)j;
@@ -452,11 +462,12 @@ __device__ __forceinline__ void arb_phase(int64_t j, double N, double acc0, doub
 // Output j of one column xc (nx stored samples, zero elsewhere).  Its window is read from the staged span xs, which holds
 // samples [xs_begin, xs_begin + xs_len) of the column, when it lies inside it, else from xc with the bounds test.  A zero
 // sample multiplied in leaves the sums bit-identical to skipping it (an accumulator that starts at +0 never becomes -0),
-// so both sources give the same output.
-template <typename EX, typename TR, typename EO>
+// so both sources give the same output.  HIST: the column is the virtual column [hc; xc] (rs_vsample); xs_begin and
+// the window indices count from its origin.
+template <typename EX, typename TR, typename EO, bool HIST = false>
 __device__ __forceinline__ EO arb_output(int64_t j, const EX* __restrict__ xc, int64_t nx, const EX* xs, int64_t xs_begin,
                                          int xs_len, const TR* bank, const TR* dbank, int tpp, int nphases, int64_t n0,
-                                         double acc0, double delta) {
+                                         double acc0, double delta, const EX* __restrict__ hc = nullptr, int64_t hlen = 0) {
     double q, r;
     arb_phase(j, (double)nphases, acc0, delta, &q, &r);
     const double fl = floor(r);
@@ -478,7 +489,11 @@ __device__ __forceinline__ EO arb_output(int64_t j, const EX* __restrict__ xc, i
 #pragma unroll 1
         for (int t = 0; t < tpp; ++t) {
             const int64_t i = first + t;
-            if (i >= 0 && i < nx) {
+            if constexpr (HIST) {
+                const EO xv = rs_cvt<EO, EX>::get(rs_vsample(hc, xc, hlen, nx, i));
+                yl = rs_fma(hrow[t], xv, yl);
+                yu = rs_fma(drow[t], xv, yu);
+            } else if (i >= 0 && i < nx) {
                 const EO xv = rs_cvt<EO, EX>::get(xc[i]);
                 yl = rs_fma(hrow[t], xv, yl);
                 yu = rs_fma(drow[t], xv, yu);
@@ -495,13 +510,16 @@ __device__ __forceinline__ EO arb_output(int64_t j, const EX* __restrict__ xc, i
 // start is rounded down to a 16-byte boundary of the column; when the column base is 16-byte aligned (vec16) the interior
 // is copied with 16-byte cp.async.  Both tap banks are staged once per CTA when they fit (banks_in_smem), else read through
 // L1.  xs_len = 0 stages nothing: every window is then read from global memory.
+// HIST (streaming): column col is the virtual column [hist + col*hlen; x + col*ldx] (rs_vsample) and output column col is
+// out + col*ldo.  The span start is rounded relative to the chunk base, so the 16-byte copies stay aligned; the vectors
+// that straddle the history / chunk boundary are loaded element by element.
 constexpr int RS_ARB_NT = 256;
-template <typename EX, typename TR, typename EO>
+template <typename EX, typename TR, typename EO, bool HIST = false>
 __global__ void __launch_bounds__(RS_ARB_NT)
 resample_arb_batch_kernel(const EX* __restrict__ x, int64_t nx, int64_t ldx, const TR* __restrict__ pfb,
                           const TR* __restrict__ dpfb, int tpp, int nphases, int banks_in_smem, int64_t n0, double acc0,
                           double delta, EO* __restrict__ out, int64_t nout, int tile, int xs_len, int vec16,
-                          int64_t tiles_per_col, int64_t total_work) {
+                          int64_t tiles_per_col, int64_t total_work, const EX* __restrict__ hist, int64_t hlen, int64_t ldo) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr int V = 16 / (int)sizeof(EX);                          // samples per 16 bytes
     EX* xs = reinterpret_cast<EX*>(smem_raw);                        // xs_len samples, a multiple of 16 bytes
@@ -520,14 +538,34 @@ resample_arb_batch_kernel(const EX* __restrict__ x, int64_t nx, int64_t ldx, con
         const int64_t col = w / tiles_per_col;
         const int64_t j0 = (w - col * tiles_per_col) * tile;
         const EX* xc = x + col * ldx;
+        const EX* hc = (HIST && hist != nullptr) ? hist + col * hlen : nullptr;
         int64_t xs_begin = 0;
         if (xs_len > 0) {
             double q0, r0;
             arb_phase(j0, (double)nphases, acc0, delta, &q0, &r0);
             const int64_t gb = n0 + (int64_t)q0 - (tpp - 1);
-            xs_begin = gb - ((gb % V) + V) % V;
+            if constexpr (HIST) xs_begin = gb - (((gb - hlen) % V) + V) % V;
+            else xs_begin = gb - ((gb % V) + V) % V;
             __syncthreads();                                         // the previous item's windows have been read
-            if (vec16) {
+            if constexpr (HIST) {
+                if (vec16) {
+#pragma unroll 1
+                    for (int v = tid; v < xs_len / V; v += nth) {
+                        const int64_t i = xs_begin + (int64_t)v * V;
+                        if (i >= hlen && i + V <= hlen + nx) {
+                            __pipeline_memcpy_async(&xs[v * V], &xc[i - hlen], 16);
+                        } else {
+#pragma unroll
+                            for (int k = 0; k < V; ++k) xs[v * V + k] = rs_vsample(hc, xc, hlen, nx, i + k);
+                        }
+                    }
+                    __pipeline_commit();
+                    __pipeline_wait_prior(0);
+                } else {
+#pragma unroll 1
+                    for (int k = tid; k < xs_len; k += nth) xs[k] = rs_vsample(hc, xc, hlen, nx, xs_begin + k);
+                }
+            } else if (vec16) {
 #pragma unroll 1
                 for (int v = tid; v < xs_len / V; v += nth) {
                     const int64_t i = xs_begin + (int64_t)v * V;
@@ -553,9 +591,46 @@ resample_arb_batch_kernel(const EX* __restrict__ x, int64_t nx, int64_t ldx, con
             }
             __syncthreads();
         }
+        if constexpr (HIST) {
+            EO* oc = out + col * ldo;
+            for (int jl = tid; jl < tile && j0 + jl < nout; jl += nth)
+                oc[j0 + jl] = arb_output<EX, TR, EO, true>(j0 + jl, xc, nx, xs, xs_begin, xs_len, bank, dbank, tpp, nphases, n0,
+                                                           acc0, delta, hc, hlen);
+        } else {
         EO* oc = out + col * nout;
         for (int jl = tid; jl < tile && j0 + jl < nout; jl += nth)
             oc[j0 + jl] = arb_output<EX, TR, EO>(j0 + jl, xc, nx, xs, xs_begin, xs_len, bank, dbank, tpp, nphases, n0, acc0, delta);
+        }
+    }
+}
+
+// Launch 1 of a streaming call (dspb200_resample_stream_exec_dev, dspb200_resample_arb_stream_exec_dev), one 1-D grid-stride
+// pass over ncols * (j_seam + H) items: (a) the first j_seam outputs of every channel -- the ones whose window reaches into
+// the history -- with the accumulation order of resample_kernel (oldest sample first); (b) every channel's new history, the
+// last H samples of its virtual column.  x is nx x ncols (column stride nx), the histories H x ncols, out column c at
+// out + c*ldo.  The arbitrary-rate call uses (b) alone (j_seam = 0).
+template <typename EX, typename TR, typename EO>
+__global__ void __launch_bounds__(RS_NT)
+resample_stream_edge_kernel(const EX* __restrict__ hist_in, EX* __restrict__ hist_out, const EX* __restrict__ x, int64_t nx,
+                            int64_t ncols, const TR* __restrict__ pfb, int tpp, int64_t interp, int64_t decim, int64_t n0,
+                            int64_t phi0, EO* __restrict__ out, int64_t ldo, int64_t j_seam) {
+    const int64_t H = tpp - 1;
+    const int64_t nseam = j_seam * ncols, total = nseam + H * ncols;
+    for (int64_t w = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; w < total; w += (int64_t)gridDim.x * blockDim.x) {
+        if (w < nseam) {
+            const int64_t c = w / j_seam, j = w - c * j_seam;
+            const EX* hc = hist_in ? hist_in + c * H : nullptr;
+            const EX* xc = x + c * nx;
+            const int64_t p = phi0 + j * decim;
+            const int64_t first = n0 + p / interp - (tpp - 1);
+            const TR* hcol = pfb + (p % interp) * tpp;
+            EO acc = rs_zero((EO*)nullptr);
+            for (int r = 0; r < tpp; ++r) acc = rs_fma(hcol[r], rs_cvt<EO, EX>::get(rs_vsample(hc, xc, H, nx, first + r)), acc);
+            out[c * ldo + j] = acc;
+        } else {
+            const int64_t v = w - nseam, c = v / H, i = v - c * H;
+            hist_out[c * H + i] = rs_vsample(hist_in ? hist_in + c * H : nullptr, x + c * nx, H, nx, nx + i);
+        }
     }
 }
 
@@ -571,6 +646,7 @@ struct RsPlanImpl {
     bool arbitrary = false;
     size_t arb_occ_smem = 0;     // resident resample_arb_batch_kernel CTAs per SM for the last (smem, threads) launched
     int arb_occ_threads = 0, arb_per_sm = 0;
+    bool arb_occ_hist = false;
     int64_t tpp8 = 0;
     size_t smem_optin = 0;
     DevBuf in, out;
@@ -787,24 +863,25 @@ static RsArbTiling rs_arb_tiling(int64_t tpp, int64_t nphases, double delta, siz
     return t;
 }
 
-template <typename EX, typename TR, typename EO>
+template <typename EX, typename TR, typename EO, bool HIST>
 static int rs_arb_launch(RsPlanImpl* p, const void* x, int64_t nx, int64_t ldx, int64_t ncols, int64_t n0, double acc0,
-                         double delta, void* out, int64_t nout, cudaStream_t st) {
+                         double delta, void* out, int64_t nout, const void* hist, int64_t ldo, cudaStream_t st) {
     if (nout == 0 || ncols == 0) return DSPB200_OK;
     const RsArbTiling t = rs_arb_tiling(p->tpp, p->interp, delta, sizeof(EX), sizeof(TR));
     DSP_REQUIRE(t.smem <= p->smem_optin, "arbitrary-rate tile needs %zu bytes of shared memory", t.smem);
-    auto kern = resample_arb_batch_kernel<EX, TR, EO>;
+    auto kern = resample_arb_batch_kernel<EX, TR, EO, HIST>;
     static bool attr_set = false;                                    // per instantiation
     if (!attr_set) {
         DSP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_optin));
         attr_set = true;
     }
-    if (p->arb_occ_smem != t.smem || p->arb_occ_threads != t.threads) {
+    if (p->arb_occ_smem != t.smem || p->arb_occ_threads != t.threads || p->arb_occ_hist != HIST) {
         int n = 0;
         DSP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, t.threads, t.smem));
         p->arb_per_sm = n < 1 ? 1 : n;
         p->arb_occ_smem = t.smem;
         p->arb_occ_threads = t.threads;
+        p->arb_occ_hist = HIST;
     }
     const int64_t tiles_per_col = cdiv(nout, t.tile), total = tiles_per_col * ncols;
     int64_t grid = (int64_t)device_sm_count() * p->arb_per_sm;
@@ -812,24 +889,71 @@ static int rs_arb_launch(RsPlanImpl* p, const void* x, int64_t nx, int64_t ldx, 
     const int vec16 = ((uintptr_t)x % 16 == 0) && ((size_t)ldx * sizeof(EX)) % 16 == 0;
     kern<<<(unsigned)grid, t.threads, t.smem, st>>>((const EX*)x, nx, ldx, (const TR*)p->d_pfb, (const TR*)p->d_dpfb,
                                                     (int)p->tpp, (int)p->interp, t.banks_in_smem, n0, acc0, delta, (EO*)out,
-                                                    nout, t.tile, t.xs_len, vec16, tiles_per_col, total);
+                                                    nout, t.tile, t.xs_len, vec16, tiles_per_col, total, (const EX*)hist,
+                                                    p->tpp - 1, ldo);
     DSP_LAUNCH_OK();
     return DSPB200_OK;
 }
 
+// Launch 1 of a streaming call: the seam outputs (j < j_seam) and the new history of every channel.
+template <typename EX, typename TR, typename EO>
+static int rs_stream_edge_launch(RsPlanImpl* p, const void* hist_in, void* hist_out, const void* x, int64_t nx, int64_t ncols,
+                                 int64_t n0, int64_t phi0, void* out, int64_t ldo, int64_t j_seam, cudaStream_t st) {
+    const int64_t total = (j_seam + p->tpp - 1) * ncols;
+    if (total == 0) return DSPB200_OK;
+    int64_t grid = cdiv(total, RS_NT);
+    const int64_t cap = (int64_t)device_sm_count() * 8;
+    if (grid > cap) grid = cap;
+    resample_stream_edge_kernel<EX, TR, EO><<<(unsigned)grid, RS_NT, 0, st>>>(
+        (const EX*)hist_in, (EX*)hist_out, (const EX*)x, nx, ncols, (const TR*)p->d_pfb, (int)p->tpp, p->interp, p->decim, n0,
+        phi0, (EO*)out, ldo, j_seam);
+    DSP_LAUNCH_OK();
+    return DSPB200_OK;
+}
+
+template <typename EX_, typename TR_, typename EO_> struct RsTypes { using EX = EX_; using TR = TR_; using EO = EO_; };
+
+// f(RsTypes<EX, TR, EO>()) for the plan's (input, arithmetic, output) element types
+template <class F> static int rs_with_types(const RsPlanImpl* p, F&& f) {
+    const bool o64 = dtype_is_f64(p->dtype_out);
+    switch (p->dtype_x) {
+        case DSPB200_F32: return o64 ? f(RsTypes<float, double, double>()) : f(RsTypes<float, float, float>());
+        case DSPB200_F64: return f(RsTypes<double, double, double>());
+        case DSPB200_C32: return o64 ? f(RsTypes<cx<float>, double, cx<double>>()) : f(RsTypes<cx<float>, float, cx<float>>());
+        default: return f(RsTypes<cx<double>, double, cx<double>>());
+    }
+}
+
 static int rs_arb_run(RsPlanImpl* p, const void* x, int64_t nx, int64_t ldx, int64_t ncols, int64_t n0, double acc0,
                       double delta, void* out, int64_t nout, cudaStream_t st) {
-    const bool o64 = p->dtype_out == DSPB200_F64 || p->dtype_out == DSPB200_C64;
-    switch (p->dtype_x) {
-        case DSPB200_F32:
-            return o64 ? rs_arb_launch<float, double, double>(p, x, nx, ldx, ncols, n0, acc0, delta, out, nout, st)
-                       : rs_arb_launch<float, float, float>(p, x, nx, ldx, ncols, n0, acc0, delta, out, nout, st);
-        case DSPB200_F64: return rs_arb_launch<double, double, double>(p, x, nx, ldx, ncols, n0, acc0, delta, out, nout, st);
-        case DSPB200_C32:
-            return o64 ? rs_arb_launch<cx<float>, double, cx<double>>(p, x, nx, ldx, ncols, n0, acc0, delta, out, nout, st)
-                       : rs_arb_launch<cx<float>, float, cx<float>>(p, x, nx, ldx, ncols, n0, acc0, delta, out, nout, st);
-        default: return rs_arb_launch<cx<double>, double, cx<double>>(p, x, nx, ldx, ncols, n0, acc0, delta, out, nout, st);
-    }
+    return rs_with_types(p, [&](auto t) -> int {
+        using T = decltype(t);
+        return rs_arb_launch<typename T::EX, typename T::TR, typename T::EO, false>(p, x, nx, ldx, ncols, n0, acc0, delta, out,
+                                                                                    nout, nullptr, nout, st);
+    });
+}
+
+// Checks shared by the two streaming entry points; *j_seam (rational plans) = outputs whose window reaches into the history.
+static int rs_stream_check(const RsPlanImpl* p, const void* hist_in, const void* hist_out, const void* x, int64_t nx,
+                           int64_t ncols, int64_t input_deficit, void* out, int64_t ldo, int64_t nout) {
+    DSP_REQUIRE(nx >= 0 && ncols >= 0 && nout >= 0, "negative size");
+    DSP_REQUIRE(input_deficit >= 1, "input_deficit must be >= 1");
+    DSP_REQUIRE(ldo >= nout, "output column stride ldo < nout");
+    DSP_REQUIRE(nx > 0 || nout == 0, "an empty chunk completes no output");
+    const int64_t H = p->tpp - 1;
+    const size_t sx = dtype_size(p->dtype_x), so = dtype_size(p->dtype_out);
+    const size_t hbytes = (size_t)(H * ncols) * sx, xbytes = (size_t)(nx * ncols) * sx;
+    const size_t obytes = (ncols && nout) ? (size_t)((ncols - 1) * ldo + nout) * so : 0;
+    // the kernels read the samples, history and outputs of other channels' threads: no written buffer may overlap another
+    auto overlap = [](const void* a, size_t na, const void* b, size_t nb_) {
+        return a && b && na && nb_ && (const char*)a < (const char*)b + nb_ && (const char*)b < (const char*)a + na;
+    };
+    DSP_REQUIRE(!overlap(hist_out, hbytes, hist_in, hbytes) && !overlap(hist_out, hbytes, x, xbytes) &&
+                !overlap(hist_out, hbytes, out, obytes), "hist_out overlaps hist_in, x or out");
+    DSP_REQUIRE(!overlap(out, obytes, x, xbytes) && !overlap(out, obytes, hist_in, hbytes), "out overlaps x or a history buffer");
+    if (nx == 0 || ncols == 0) return DSPB200_OK;
+    DSP_REQUIRE(x != nullptr && (out != nullptr || nout == 0) && (hist_out != nullptr || H == 0), "NULL argument");
+    return DSPB200_OK;
 }
 
 struct dspb200_resample_plan {
@@ -1020,6 +1144,57 @@ int dspb200_resample_arb_batch_exec(dspb200_resample_plan* plan, const void* x, 
 int dspb200_resample_arb_exec(dspb200_resample_plan* plan, const void* x, int64_t nx, int64_t n0, double acc0, double delta,
                               void* out, int64_t nout) {
     return dspb200_resample_arb_batch_exec(plan, x, nx, nx, 1, n0, acc0, delta, out, nout);
+}
+
+// Streaming FIRFilter, rational kinds: launch 1 = seam outputs + new history (resample_stream_edge_kernel), launch 2 = the
+// family rs_launch picks for outputs j_seam .. nout-1, on the chunk alone (x_begin = H: their windows lie inside it).
+int dspb200_resample_stream_exec_dev(dspb200_resample_plan* plan, const void* hist_in, void* hist_out, const void* x, int64_t nx,
+                                     int64_t ncols, int64_t input_deficit, int64_t phi0, void* out, int64_t ldo, int64_t nout,
+                                     void* stream) {
+    DSP_RANGE("dspb200_resample_stream_exec_dev");
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    RsPlanImpl* p = &plan->impl;
+    DSP_REQUIRE(!p->arbitrary, "an arbitrary-rate plan streams through dspb200_resample_arb_stream_exec_dev");
+    DSP_REQUIRE(phi0 >= 0 && phi0 < p->interp, "bad initial phase");
+    DSP_TRY(rs_stream_check(p, hist_in, hist_out, x, nx, ncols, input_deficit, out, ldo, nout));
+    if (nx == 0 || ncols == 0) return DSPB200_OK;
+    const int64_t H = p->tpp - 1, n0 = H + input_deficit - 1, I = p->interp, D = p->decim;
+    // output j reads the history iff its oldest sample input_deficit - 1 + (phi0 + j*D) / I lies below H
+    const int64_t K = H - input_deficit + 1;
+    int64_t j_seam = (K > 0 && I * K > phi0) ? (I * K - phi0 + D - 1) / D : 0;
+    if (j_seam > nout) j_seam = nout;
+    cudaStream_t st = (cudaStream_t)stream;
+    return rs_with_types(p, [&](auto t) -> int {
+        using T = decltype(t);
+        DSP_TRY((rs_stream_edge_launch<typename T::EX, typename T::TR, typename T::EO>(p, hist_in, hist_out, x, nx, ncols, n0, phi0,
+                                                                                     out, ldo, j_seam, st)));
+        if (nout == j_seam) return DSPB200_OK;
+        RsArgs a{x, H, nx, nx, (char*)out + (size_t)j_seam * sizeof(typename T::EO), j_seam, nout - j_seam, ldo, n0, phi0, ncols};
+        return rs_launch<typename T::EX, typename T::TR, typename T::EO>(p, a, st);
+    });
+}
+
+// Streaming FIRFilter, arbitrary rate: the HIST instance of resample_arb_batch_kernel reads the virtual column; the edge
+// kernel writes the new history (j_seam = 0).
+int dspb200_resample_arb_stream_exec_dev(dspb200_resample_plan* plan, const void* hist_in, void* hist_out, const void* x,
+                                         int64_t nx, int64_t ncols, int64_t input_deficit, double acc0, double delta, void* out,
+                                         int64_t ldo, int64_t nout, void* stream) {
+    DSP_RANGE("dspb200_resample_arb_stream_exec_dev");
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    RsPlanImpl* p = &plan->impl;
+    DSP_REQUIRE(p->arbitrary, "not an arbitrary-rate plan");
+    DSP_REQUIRE(delta > 0.0 && acc0 >= 0.0 && acc0 < (double)p->interp, "bad phase state");
+    DSP_TRY(rs_stream_check(p, hist_in, hist_out, x, nx, ncols, input_deficit, out, ldo, nout));
+    if (nx == 0 || ncols == 0) return DSPB200_OK;
+    const int64_t H = p->tpp - 1, n0 = H + input_deficit - 1;
+    cudaStream_t st = (cudaStream_t)stream;
+    return rs_with_types(p, [&](auto t) -> int {
+        using T = decltype(t);
+        DSP_TRY((rs_arb_launch<typename T::EX, typename T::TR, typename T::EO, true>(p, x, nx, nx, ncols, n0, acc0, delta, out, nout,
+                                                                                    hist_in, ldo, st)));
+        return rs_stream_edge_launch<typename T::EX, typename T::TR, typename T::EO>(p, hist_in, hist_out, x, nx, ncols, n0, 0,
+                                                                                   nullptr, 0, 0, st);
+    });
 }
 
 int dspb200_resample_plan_destroy(dspb200_resample_plan* plan) {

@@ -56,8 +56,14 @@ def _cols(x, dt):
 def filt(b, a, x=None, si=None):
     """filt(b, a, x) (src/dspbase.jl:14-15) and, with two arguments, Filters.filt(h, x) (src/Filters/filt.jl:445-446),
     filt(f::DF2TFilter, x) and filt(f::PolynomialRatio, x) (src/Filters/filt.jl:30, 215-224).  The deprecated
-    filt(b, a, x, si) and filt(f::PolynomialRatio, x, si) (src/deprecated.jl) filter from the initial state si (copied)."""
+    filt(b, a, x, si) and filt(f::PolynomialRatio, x, si) (src/deprecated.jl) filter from the initial state si (copied).
+    filt(f::FIRFilter, x) streams x through the stateful polyphase filter (src/Filters/stream_filt.jl:627-637)."""
     from . import df2t
+    from .filters import FIRFilter
+    if isinstance(b, FIRFilter):
+        if x is not None:
+            raise ArgumentError("filt(f::FIRFilter, x) takes one signal")
+        return b.filt(a)
     if isinstance(b, df2t.DF2TFilter):
         if x is not None:
             raise ArgumentError("filt(f::DF2TFilter, x) takes one signal")
@@ -120,8 +126,14 @@ def _filt_device(b, a, x):
 def filt_(out, b, a, x=None, si=None):
     """filt!(out, b, a, x), src/dspbase.jl:26-66.  FIR only (length(a) == 1); IIR is outside the hot path.  Also
     filt!(out, f::DF2TFilter, x), filt!(out, f::PolynomialRatio, x) (src/Filters/filt.jl:17) and the deprecated
-    filt!(out, b, a, x, si) / filt!(out, f::PolynomialRatio, x, si) (src/deprecated.jl, si copied)."""
+    filt!(out, b, a, x, si) / filt!(out, f::PolynomialRatio, x, si) (src/deprecated.jl, si copied).
+    filt!(buffer, f::FIRFilter, x) returns the number of outputs written (src/Filters/stream_filt.jl:409-625)."""
     from . import df2t
+    from .filters import FIRFilter
+    if isinstance(b, FIRFilter):
+        if x is not None:
+            raise ArgumentError("filt!(buffer, f::FIRFilter, x) takes one signal")
+        return b.filt_(out, a)
     if isinstance(b, df2t.DF2TFilter):
         if x is not None:
             raise ArgumentError("filt!(out, f::DF2TFilter, x) takes one signal")

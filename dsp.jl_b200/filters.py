@@ -1,6 +1,7 @@
 """FIR application and polyphase resampling front ends (reference src/Filters/filt.jl:431-555,
 src/Filters/stream_filt.jl, src/Filters/design.jl:547-559, 694-720), backed by libdspb200."""
 import math
+from collections import namedtuple
 from fractions import Fraction
 
 import numpy as np
@@ -184,6 +185,9 @@ def inputlength(outputlength_, ratio, initial_phi, round_up=False):
     return -((-num) // ratio.numerator) if round_up else num // ratio.numerator
 
 
+_Step = namedtuple("_Step", "nout n0 phase0 j_seam phi_idx input_deficit phi_accumulator")
+
+
 class FIRFilter:
     """FIRFilter(h, ratio=1): stateful single-rate / interpolating / decimating / rational polyphase FIR filter,
     src/Filters/stream_filt.jl:137-178 (kernels :8-78).  State carried across `filt` calls exactly as the
@@ -194,9 +198,17 @@ class FIRFilter:
     FIRFilter(h, rate::float, nphases=32) is the arbitrary-rate filter (FIRArbitrary, :92-134, 193-205): polyphase bank
     plus derivative bank with linear interpolation between phases; state `phi_accumulator` / `input_deficit`.  The
     per-call phase sequence acc0 + j*delta is evaluated exactly (rational arithmetic on the host for the counts,
-    double-double on the device), see resample.cu.  `h=None` designs the taps with resample_filter(rate, nphases)."""
+    double-double on the device), see resample.cu.  `h=None` designs the taps with resample_filter(rate, nphases).
 
-    def __init__(self, h, ratio=1, nphases=32):
+    device=True keeps the history in device memory: the filter takes DeviceArray chunks, a vector (nx,) or a column-major
+    (nx, nchan) matrix whose channels share the one phase state (an extension: the reference filters vectors), and
+    returns DeviceArrays.  A chunk costs at most two kernel launches, no host synchronisation and no host <-> device
+    copy; the kernels read the virtual column [history; x] without building it.  The first chunk fixes the eltype and
+    the channel count; `reset()` drops them with the history.  `history` is then the current (tpp - 1)-sample device
+    buffer (None before the first launch).  A host filter refuses DeviceArrays and a device filter host arrays."""
+
+    def __init__(self, h, ratio=1, nphases=32, *, device=False):
+        self.device = bool(device)
         if isinstance(ratio, (float, np.floating)):
             self._init_arbitrary(h, float(ratio), int(nphases))
             return
@@ -245,11 +257,14 @@ class FIRFilter:
         self.reset()
 
     def reset(self):
-        """reset!, src/Filters/stream_filt.jl:247-276."""
+        """reset!, src/Filters/stream_filt.jl:247-276.  A device filter also drops its history buffers, eltype and
+        channel count."""
         self.phi_idx = 1
         self.input_deficit = 1
         self.history = None
         self.phi_accumulator = 0.0
+        self._dev_key = None          # device form: (eltype, channel shape) fixed by the first chunk
+        self._hist = None             # device form: [current, next] history buffers
         return self
 
     @property
@@ -298,64 +313,138 @@ class FIRFilter:
         v = inputlength(outlen, self.ratio, self.phi_idx if self.kind != "decimator" else 1, round_up)
         return v + self.input_deficit - 1
 
+    def _step(self, phi_idx, input_deficit, phi_accumulator, xlen):
+        """Bookkeeping of one filt! call on xlen samples from the state (phi_idx, input_deficit, phi_accumulator), shared by
+        the host and the device form (src/Filters/stream_filt.jl:476-515, 522-560, 579-625).  Returns a _Step: `nout`
+        outputs; `n0`, the index in [history; x] of output 0's newest sample; `phase0`, the 0-based start phase (rational
+        kinds) or the phase accumulator (arbitrary); `j_seam`, the number of outputs whose window reaches into the history
+        (rational kinds; the arbitrary-rate kernel reads [history; x] itself, so 0 there); and the state after the call.
+        Output j's oldest sample in [history; x] is input_deficit - 1 + (phase0 + j*D) // I, so it reads the history iff
+        (phase0 + j*D) // I < history_len - input_deficit + 1."""
+        H = self.history_len
+        n0 = H + input_deficit - 1
+        if xlen < input_deficit:                                                              # :484-488, :590-594
+            return _Step(0, n0, phi_accumulator if self.kind == "arbitrary" else 0, 0, phi_idx, input_deficit - xlen,
+                         phi_accumulator)
+        if self.kind == "arbitrary":
+            nout, deficit, acc = _arb_advance(phi_accumulator, input_deficit, self.delta, self.nphases, xlen)
+            return _Step(nout, n0, phi_accumulator, 0, 1 + math.floor(acc), deficit, acc)
+        I, D = self.interpolation, self.decimation
+        phased = self.kind in ("rational", "interpolator")
+        phi0 = phi_idx - 1 if phased else 0
+        nout = outputlength(xlen - input_deficit + 1, self.ratio, phi0 + 1) if self.kind != "standard" else xlen
+        total = phi0 + nout * D                                            # phase recurrence after nout outputs
+        deficit = 1 if self.kind == "interpolator" else input_deficit + total // I - xlen     # :463, :511
+        K = H - input_deficit + 1
+        j_seam = min(nout, -(-(I * K - phi0) // D)) if K > 0 and I * K > phi0 else 0
+        return _Step(nout, n0, phi0, j_seam, total % I + 1 if phased else phi_idx, deficit, phi_accumulator)
+
+    def _commit(self, st):
+        self.phi_idx, self.input_deficit, self.phi_accumulator = st.phi_idx, st.input_deficit, st.phi_accumulator
+
+    def _plan(self, xdt):
+        if xdt not in self._plans:
+            self._plans[xdt] = (_lib.ResampleArbPlan(xdt, self.h, self.nphases) if self.kind == "arbitrary"
+                                else _lib.ResamplePlan(xdt, self.h, self.interpolation, self.decimation))
+        return self._plans[xdt]
+
     def filt(self, x):
         """filt(self::FIRFilter, x), src/Filters/stream_filt.jl:627-637 (+ the filt! loops :409-560)."""
+        if self.device:
+            return self._filt_device(None, x)
+        return self._filt_host(x)[0]
+
+    def filt_(self, buffer, x):
+        """filt!(buffer, self::FIRFilter, x), src/Filters/stream_filt.jl:409-625: writes the call's outputs to the first
+        elements of `buffer` (its first `nout` rows for a device matrix) and returns their number.  A buffer shorter than
+        the call's output raises ArgumentError before the state changes; so does, for a device filter, a buffer that
+        overlaps x."""
+        if self.device:
+            return self._filt_device(buffer, x)
+        if isinstance(buffer, DeviceArray):
+            raise ArgumentError("a host FIRFilter filters host arrays (construct it with device=True)")
+        return self._filt_host(x, buffer)[1]
+
+    def _filt_host(self, x, buffer=None):
+        if isinstance(x, DeviceArray):
+            raise ArgumentError("a host FIRFilter filters host arrays (construct it with device=True)")
         x = np.asarray(x)
         if x.ndim != 1:
             raise ArgumentError("FIRFilter filters vectors")
         xdt = _gpu_dtype(_promote(x))
         x = np.ascontiguousarray(x, dtype=xdt)
-        if self.kind == "arbitrary":
-            return self._filt_arbitrary(x, xdt)
-        if xdt not in self._plans:
-            self._plans[xdt] = _lib.ResamplePlan(xdt, self.h, self.interpolation, self.decimation)
-        plan = self._plans[xdt]
+        xlen = x.size
+        st = self._step(self.phi_idx, self.input_deficit, self.phi_accumulator, xlen)
+        if buffer is not None and len(buffer) < st.nout:
+            raise ArgumentError(f"buffer is too small: the call produces {st.nout} outputs, buffer holds {len(buffer)}")
+        plan = self._plan(xdt)
         if self.history is None or self.history.dtype != xdt:
             self.history = np.zeros(self.history_len, dtype=xdt)          # history = zeros(historyLen), :175
-        xlen = x.size
-        I, D = self.interpolation, self.decimation
-        if xlen < self.input_deficit:                                      # :484-488
+        if xlen < self.input_deficit:                                      # :484-488, :590-594
             self.history = self._shiftin(self.history, x)
-            self.input_deficit -= xlen
-            return np.zeros(0, dtype=plan.out_dtype)
-        phi0 = self.phi_idx - 1 if self.kind in ("rational", "interpolator") else 0
-        nout = outputlength(xlen - self.input_deficit + 1, self.ratio, phi0 + 1) if self.kind != "standard" else xlen
+            self._commit(st)
+            return np.zeros(0, dtype=plan.out_dtype), 0
         xe = np.concatenate([self.history, x])
-        n0 = self.history_len + self.input_deficit - 1                     # index in [history; x] of the first output's newest sample
-        out = np.empty(nout, dtype=plan.out_dtype)
-        plan.exec(xe, xe.size, 1, n0, phi0, out, nout)
-        total = phi0 + nout * D                                            # phase recurrence after nout outputs
-        self.input_deficit = self.input_deficit + total // I - xlen        # :511
-        if self.kind in ("rational", "interpolator"):
-            self.phi_idx = total % I + 1
-        if self.kind == "interpolator":
-            self.input_deficit = 1                                         # :463
-        self.history = self._shiftin(self.history, x)                      # :512
-        return out
+        out = np.empty(st.nout, dtype=plan.out_dtype)
+        if self.kind == "arbitrary":                                       # :579-625
+            plan.exec(xe, xe.size, st.n0, st.phase0, self.delta, out, st.nout)
+        else:
+            plan.exec(xe, xe.size, 1, st.n0, st.phase0, out, st.nout)
+        self._commit(st)
+        self.history = self._shiftin(self.history, x)                      # :512, :621
+        if buffer is not None:
+            buffer[:st.nout] = out
+        return out, st.nout
 
-    def _filt_arbitrary(self, x, xdt):
-        """filt!(buffer, ::FIRFilter{FIRArbitrary}, x), src/Filters/stream_filt.jl:579-625.  Output j of the call sits at
-        total phase acc + j*delta; the loop `while xIdx <= xLen` produces exactly the j with
-        inputDeficit + floor((acc + j*delta) / Nphi) <= xLen, counted here in exact rational arithmetic."""
-        if xdt not in self._plans:
-            self._plans[xdt] = _lib.ResampleArbPlan(xdt, self.h, self.nphases)
-        plan = self._plans[xdt]
-        if self.history is None or self.history.dtype != xdt:
-            self.history = np.zeros(self.history_len, dtype=xdt)
-        xlen = x.size
-        if xlen < self.input_deficit:                                                         # :590-594
-            self.history = self._shiftin(self.history, x)
-            self.input_deficit -= xlen
-            return np.zeros(0, dtype=plan.out_dtype)
-        nout, new_deficit, new_acc = _arb_advance(self.phi_accumulator, self.input_deficit, self.delta, self.nphases, xlen)
-        xe = np.concatenate([self.history, x])
-        n0 = self.history_len + self.input_deficit - 1
-        out = np.empty(nout, dtype=plan.out_dtype)
-        plan.exec(xe, xe.size, n0, self.phi_accumulator, self.delta, out, nout)
-        self.input_deficit, self.phi_accumulator = new_deficit, new_acc
-        self.phi_idx = 1 + math.floor(self.phi_accumulator)
-        self.history = self._shiftin(self.history, x)            # :621
-        return out
+    def _filt_device(self, buffer, x):
+        """One chunk through dspb200_resample_(arb_)stream_exec_dev: every check happens before the first launch."""
+        if not isinstance(x, DeviceArray):
+            raise ArgumentError("a device FIRFilter filters DeviceArrays (construct it without device=True for host arrays)")
+        if x.ndim not in (1, 2):
+            raise ArgumentError("a device FIRFilter filters a vector or a len x nchan DeviceArray")
+        key = (x.dtype, x.shape[1:])
+        if self._dev_key is not None and key != self._dev_key:
+            raise ArgumentError(f"this device FIRFilter streams {self._dev_key[0]} chunks of channel shape {self._dev_key[1]}; "
+                                f"got {x.dtype} {x.shape[1:]} (reset() starts a new stream)")
+        plan = self._plan(x.dtype)
+        nx = x.shape[0]
+        nchan = x.shape[1] if x.ndim == 2 else 1
+        st = self._step(self.phi_idx, self.input_deficit, self.phi_accumulator, nx)
+        hshape = (self.history_len,) + x.shape[1:]
+        hist = self._hist or [None, DeviceArray(hshape, x.dtype)]
+
+        def overlap(a, b):
+            return a is not None and a.nbytes and b.nbytes and a.ptr < b.ptr + b.nbytes and b.ptr < a.ptr + a.nbytes
+
+        if buffer is None:
+            out = DeviceArray((st.nout,) + x.shape[1:], plan.out_dtype)
+        else:
+            if not isinstance(buffer, DeviceArray):
+                raise ArgumentError("a device FIRFilter writes into a DeviceArray buffer")
+            if buffer.dtype != plan.out_dtype or buffer.shape[1:] != x.shape[1:]:
+                raise ArgumentError(f"buffer must be a {plan.out_dtype} DeviceArray of channel shape {x.shape[1:]}")
+            if buffer.shape[0] < st.nout:
+                raise ArgumentError(f"buffer is too small: the call produces {st.nout} outputs, buffer holds {buffer.shape[0]}")
+            if overlap(buffer, x) or overlap(hist[0], buffer) or overlap(hist[1], buffer):
+                raise ArgumentError("a device FIRFilter cannot filter in place: buffer must not overlap x")
+            out = buffer
+        if self._hist is None:
+            self._dev_key, self._hist = key, hist
+        if nx and nchan:
+            cur, nxt = hist
+            ldo = out.shape[0]
+            if self.kind == "arbitrary":
+                plan.stream_exec_dev(cur.ptr if cur is not None else None, nxt.ptr, x.ptr, nx, nchan, self.input_deficit,
+                                     st.phase0, self.delta, out.ptr, ldo, st.nout, 0)
+            else:
+                plan.stream_exec_dev(cur.ptr if cur is not None else None, nxt.ptr, x.ptr, nx, nchan, self.input_deficit,
+                                     st.phase0, out.ptr, ldo, st.nout, 0)
+            if cur is None:                                                # the first launch: zero history in, none to reuse
+                cur = DeviceArray(hshape, x.dtype)
+            self._hist = [nxt, cur]
+            self.history = nxt
+        self._commit(st)
+        return out if buffer is None else st.nout
 
     @staticmethod
     def _shiftin(a, b):

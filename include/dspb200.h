@@ -285,6 +285,27 @@ DSPB200_API int dspb200_resample_arb_batch_exec(dspb200_resample_plan* plan, con
 DSPB200_API int dspb200_resample_arb_batch_exec_dev(dspb200_resample_plan* plan, const void* x, int64_t nx, int64_t ldx,
                                                     int64_t ncols, int64_t n0, double acc0, double delta, void* out,
                                                     int64_t nout, void* stream);
+/* Streaming FIRFilter (filt!(buffer, self::FIRFilter, x), src/Filters/stream_filt.jl:137-403, 409-625) on ncols channels
+ * that share one phase state; device pointers, enqueued on `stream`, no synchronisation.  A call filters each channel's
+ * virtual column [history; x] (history: the plan's tpp - 1 samples, x: nx samples) from the state (input_deficit >= 1 and
+ * phi0 in [0, interp) -- 0-based phiIdx -- or acc0 = phiAccumulator in [0, nphases)), exactly as the reference's filt! on
+ * that channel, and writes the nout outputs the host computed from the same state (outputlength) to out[c*ldo + j].
+ * x is nx x ncols column-major; hist_in / hist_out are (tpp - 1) x ncols column-major in x's element type: hist_in is the
+ * history before x (NULL: zeros), hist_out receives the last tpp - 1 samples of [history; x].  Chunks fed one after the
+ * other with the returned state give outputs bit-identical to the reference's filt! on each channel.
+ * DSPB200_EINVALID before any launch when hist_out overlaps hist_in, x or out, when out overlaps x or a history buffer,
+ * when ldo < nout, or when nx == 0 with nout > 0.  nout == 0 with nx > 0 only updates the history (a chunk shorter than
+ * inputDeficit, :484-488, :590-594); nx == 0 or ncols == 0 launches nothing.
+ * Rational plans (dspb200_resample_plan_create): at most two launches -- the outputs whose window reaches into the
+ * history together with the new history, then the rest on the chunk through the same kernels as dspb200_resample_exec_dev.
+ * Arbitrary-rate plans (dspb200_resample_arb_plan_create): the batched kernel reads [history; x] itself, plus one launch
+ * for the history. */
+DSPB200_API int dspb200_resample_stream_exec_dev(dspb200_resample_plan* plan, const void* hist_in, void* hist_out, const void* x,
+                                                 int64_t nx, int64_t ncols, int64_t input_deficit, int64_t phi0, void* out,
+                                                 int64_t ldo, int64_t nout, void* stream);
+DSPB200_API int dspb200_resample_arb_stream_exec_dev(dspb200_resample_plan* plan, const void* hist_in, void* hist_out,
+                                                     const void* x, int64_t nx, int64_t ncols, int64_t input_deficit, double acc0,
+                                                     double delta, void* out, int64_t ldo, int64_t nout, void* stream);
 DSPB200_API int dspb200_resample_plan_destroy(dspb200_resample_plan* plan);
 
 #ifdef __cplusplus
