@@ -60,6 +60,8 @@ SIGNATURES = {
     "dspb200_os_exec": (_int, [_vp, _vp, _i64, _i64, _vp, _i64]),
     "dspb200_os_exec_dev": (_int, [_vp, _vp, _i64, _i64, _vp, _i64, _vp]),
     "dspb200_os_exec_range_dev": (_int, [_vp, _vp, _i64, _i64, _vp, _i64, _i64, _vp]),
+    "dspb200_os_exec_state": (_int, [_vp, _vp, _i64, _i64, _vp, _vp, _vp]),
+    "dspb200_os_exec_state_dev": (_int, [_vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp]),
     "dspb200_os_plan_destroy": (_int, [_vp]),
     "dspb200_conv_fft_exec": (_int, [_int, _vp, _i64, _vp, _i64, _i64, _vp]),
     "dspb200_conv_direct_exec": (_int, [_int, _vp, _i64, _vp, _i64, _vp]),
@@ -221,6 +223,14 @@ class OsPlan(_Plan):
 
     def exec_range_dev(self, u_ptr, u_begin, nu_local, out_ptr, out_begin, out_count, stream=0):
         check(lib.dspb200_os_exec_range_dev(self.handle, u_ptr, u_begin, nu_local, out_ptr, out_begin, out_count, stream))
+
+    def exec_state(self, x, nx, ncols, si_in, si_out, out):
+        """Stateful overlap-save (FirPlan.exec_state's arguments and state): host arrays, Fortran-ordered."""
+        check(lib.dspb200_os_exec_state(self.handle, ptr(x), nx, ncols, None if si_in is None else ptr(si_in),
+                                        None if si_out is None else ptr(si_out), ptr(out)))
+
+    def exec_state_dev(self, x_ptr, nx, ncols, si_in_ptr, si_out_ptr, out_ptr, stream=0):
+        check(lib.dspb200_os_exec_state_dev(self.handle, x_ptr, nx, ncols, si_in_ptr, si_out_ptr, out_ptr, stream))
 
 
 class SpecPlan(_Plan):

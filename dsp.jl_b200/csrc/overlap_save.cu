@@ -30,6 +30,7 @@ struct OsPlanImpl {
     void* d_t256 = nullptr;
     int sm_count = 0;               // device_sm_count() at plan creation
     int fused_per_sm = 0;   // resident CTAs per SM of this plan's fused kernel (occupancy calculator, asked once)
+    int fused_state_per_sm = 0;     // the same for its stateful instance
     void* d_H = nullptr;    // natural order; fused: cx<T>[nfft] pre-scaled by 1/nfft; generic: nfft or nfft/2+1 bins
     // generic
     cufftHandle fwd = 0, inv = 0;
@@ -124,6 +125,33 @@ template <typename E> struct OsUnit {
     int jlo, jhi, jend, jzero;
     int nvm1, L;
 };
+
+// Stateful calls (DF2TFilter, dspb200_os_exec_state_dev): a column's call computes the outputs o in [0, nx + nv - 1) of
+// conv(v, x); o < nv - 1 adds the incoming transposed direct-form state si_in[o], o >= nx is the outgoing state
+// si_out[o - nx], the rest is out[o].  si_in / si_out hold nv - 1 elements per column; si_in may be NULL (zero state); without
+// si_out the call computes only the nx outputs.  Only edge units touch the state: an interior unit's outputs lie in
+// [nv - 1, nx).  The stateless instances take the empty struct, so their parameters and code are those of before.
+template <typename E, bool STATE> struct OsState {};
+template <typename E> struct OsState<E, true> {
+    const E* si_in;
+    E* si_out;
+    int64_t nx;
+};
+// The state geometry of an edge unit of a stateful call: slot j's output is s0 + j; si_in / si_out are shifted so that index
+// j addresses that output's state entry; slots j < jsi take incoming state, slots j >= jnx are outgoing state.  It is
+// computed just before the last pass (os_fused_kernel's state_geometry), not carried through the transforms' registers.
+template <typename E> struct OsUnitState {
+    const E* si_in;
+    E* si_out;
+    int jsi, jnx;
+};
+struct OsNoState {};
+template <typename E> __device__ __forceinline__ void os_put_state(const OsUnit<E>& g, const OsUnitState<E>& s, int j, E v) {
+    if (j < s.jsi) v = v + s.si_in[j];
+    if (j < s.jnx) g.out[j] = v;
+    else s.si_out[j] = v;
+}
+
 __device__ __forceinline__ int os_clamp(int64_t v) {
     return (int)(v < -(int64_t(1) << 30) ? -(int64_t(1) << 30) : (v > (int64_t(1) << 30) ? (int64_t(1) << 30) : v));
 }
@@ -165,11 +193,12 @@ struct OsStage {
 };
 
 // One unit.  staged: its input span is (being) copied to OsStage::head; next_u: slot 0 of the next unit when that one
-// is to be staged (os_fused_kernel decides), else null.  Both only in staged kernels.
-template <typename T, int N, bool CPLX, int NT, bool INTERIOR, int ITERS>
+// is to be staged (os_fused_kernel decides), else null.  Both only in staged kernels.  STATE: only the edge units' stores
+// change (os_put_state, with the OsUnitState that state_geometry() returns).
+template <typename T, int N, bool CPLX, int NT, bool INTERIOR, int ITERS, bool STATE, typename SG>
 __device__ __forceinline__ void os_unit(const FftCtx<T>& ctx, int tid, const OsUnit<typename os_elt<T, CPLX>::type>& g,
                                         const cx<T>* __restrict__ H, OsStage& st, bool staged,
-                                        const typename os_elt<T, CPLX>::type* __restrict__ next_u) {
+                                        const typename os_elt<T, CPLX>::type* __restrict__ next_u, const SG& state_geometry) {
     using E = typename os_elt<T, CPLX>::type;
     constexpr int Q = fft_plan_traits<N>::Q;
     constexpr bool STAGED = os_threads<T, N, CPLX>::staged;
@@ -231,6 +260,9 @@ __device__ __forceinline__ void os_unit(const FftCtx<T>& ctx, int tid, const OsU
     __syncthreads();
     fft_middle<T, N, NT>(ctx, tid);
     constexpr int RL = fft_plan_traits<N>::RL, NBF = 16 / RL;
+    using SGeom = std::conditional_t<STATE && !INTERIOR, OsUnitState<E>, OsNoState>;
+    SGeom sg{};
+    if constexpr (STATE && !INTERIOR) sg = state_geometry();
     // output of slot j (y: swapped domain, result = (y.y, y.x))
     auto put = [&](int j, cx<T> y) {
 #if DSP_PROBE & 8
@@ -239,12 +271,16 @@ __device__ __forceinline__ void os_unit(const FftCtx<T>& ctx, int tid, const OsU
         if (j < g.nvm1) return;
         if constexpr (CPLX) {
             if constexpr (INTERIOR) g.out[j] = mkc<T>(y.y, y.x);
+            else if constexpr (STATE) { if (j < g.jend) os_put_state(g, sg, j, mkc<T>(y.y, y.x)); }
             else if (j < g.jend) g.out[j] = (j < g.jzero) ? mkc<T>(y.y, y.x) : mkc<T>(T(0), T(0));
         } else {
             const int jb = j + g.L;
             if constexpr (INTERIOR) {
                 g.out[j] = y.y;
                 g.out[jb] = y.x;
+            } else if constexpr (STATE) {
+                if (j < g.jend) os_put_state(g, sg, j, y.y);
+                if (jb < g.jend) os_put_state(g, sg, jb, y.x);
             } else {
                 if (j < g.jend) g.out[j] = (j < g.jzero) ? y.y : T(0);
                 if (jb < g.jend) g.out[jb] = (jb < g.jzero) ? y.x : T(0);
@@ -298,12 +334,13 @@ __device__ __forceinline__ void os_unit(const FftCtx<T>& ctx, int tid, const OsU
     }
 }
 
-template <typename T, int N, bool CPLX>
+template <typename T, int N, bool CPLX, bool STATE>
 __global__ void __launch_bounds__((os_threads<T, N, CPLX>::value), (os_threads<T, N, CPLX>::minblocks))
 os_fused_kernel(const void* __restrict__ u_, int64_t u_begin, int64_t nu_local, int64_t u_col_stride,
                 void* __restrict__ out_, int64_t out_begin, int64_t out_count, int64_t out_col_stride,
                 int64_t zero_from, int nv, int64_t units_per_col, int64_t total_units, const cx<T>* __restrict__ gtl,
-                const cx<T>* __restrict__ g16, const cx<T>* __restrict__ g256, const cx<T>* __restrict__ H) {
+                const cx<T>* __restrict__ g16, const cx<T>* __restrict__ g256, const cx<T>* __restrict__ H,
+                const OsState<typename os_elt<T, CPLX>::type, STATE> sa) {
     constexpr int NT = os_threads<T, N, CPLX>::value;
     constexpr int Q = fft_plan_traits<N>::Q;
     constexpr int ITERS = (Q + NT - 1) / NT;
@@ -350,6 +387,20 @@ os_fused_kernel(const void* __restrict__ u_, int64_t u_begin, int64_t nu_local, 
         g.L = L;
         return g.jlo <= 0 && g.jhi >= span && g.jend >= span && g.jzero >= span;
     };
+    // STATE: the state geometry of (edge) unit gu, in the same coordinates (OsUnitState)
+    auto state_geometry = [&](int64_t gu) {
+        OsUnitState<E> s{};
+        if constexpr (STATE) {
+            const int64_t col = onecol ? 0 : gu / units_per_col;
+            const int64_t unit = gu - col * units_per_col;
+            const int64_t s0 = out_begin + (CPLX ? unit : 2 * unit) * L - (nv - 1);
+            s.si_in = sa.si_in + col * (nv - 1) + s0;
+            s.si_out = sa.si_out + col * (nv - 1) + (s0 - sa.nx);
+            s.jsi = sa.si_in ? os_clamp((nv - 1) - s0) : -(1 << 30);
+            s.jnx = os_clamp(sa.nx - s0);
+        }
+        return s;
+    };
     // pull the input range of unit gn into L2 (16-byte aligned sub-range, clipped to the stored signal)
     auto l2_prefetch = [&](int64_t gn) {
         if (tid == 0 && gn < total_units) {
@@ -393,8 +444,9 @@ os_fused_kernel(const void* __restrict__ u_, int64_t u_begin, int64_t nu_local, 
         OsUnit<E> g;
         const bool interior = geometry(gu, g);
         const E* next_u = stage_src(gu + gridDim.x);
-        if (interior) os_unit<T, N, CPLX, NT, true, ITERS>(ctx, tid, g, H, st, staged, next_u);
-        else os_unit<T, N, CPLX, NT, false, ITERS>(ctx, tid, g, H, st, staged, next_u);
+        auto sgeom = [&]() { return state_geometry(gu); };
+        if (interior) os_unit<T, N, CPLX, NT, true, ITERS, STATE>(ctx, tid, g, H, st, staged, next_u, sgeom);
+        else os_unit<T, N, CPLX, NT, false, ITERS, STATE>(ctx, tid, g, H, st, staged, next_u, sgeom);
         staged = next_u != nullptr;
     }
 }
@@ -546,10 +598,11 @@ __global__ void nd_os_scatter_kernel(const E* __restrict__ td, OsNd g, int64_t b
     }
 }
 
-template <typename T, bool CPLX>
+// STATE: sa holds one column's state (OsState), and m is that column's output index (out_begin == 0)
+template <typename T, bool CPLX, bool STATE>
 __global__ void os_scatter_kernel(const void* __restrict__ td_, int64_t m_first, int64_t L, int64_t nv, int64_t nfft,
                                   int64_t nblk, void* __restrict__ out_, int64_t out_begin, int64_t out_end,
-                                  int64_t zero_from) {
+                                  int64_t zero_from, const OsState<typename os_elt<T, CPLX>::type, STATE> sa) {
     using E = typename os_elt<T, CPLX>::type;
     const E* td = reinterpret_cast<const E*>(td_);
     E* out = reinterpret_cast<E*>(out_);
@@ -560,6 +613,13 @@ __global__ void os_scatter_kernel(const void* __restrict__ td_, int64_t m_first,
         if (m < out_end) {
             E v = td[b * nfft + (nv - 1) + j];
             if (m >= zero_from) { if constexpr (CPLX) v = mkc<T>(T(0), T(0)); else v = T(0); }
+            if constexpr (STATE) {
+                if (sa.si_in && m < nv - 1) v = v + sa.si_in[m];
+                if (m >= sa.nx) {
+                    sa.si_out[m - sa.nx] = v;
+                    continue;
+                }
+            }
             out[m - out_begin] = v;
         }
     }
@@ -635,43 +695,61 @@ struct OsRange {
     int64_t zero_from, ncols;
 };
 
-template <typename T, int N, bool CPLX>
-static int launch_os_fused(OsPlanImpl* p, const OsRange& a, cudaStream_t st) {
+// state of a stateful call (OsState, untyped): si_in / si_out hold nv - 1 elements per column
+struct OsStateArgs {
+    const void* si_in;
+    void* si_out;
+    int64_t nx;
+};
+// The stateful entry plans with nfft = 0 (auto_nfft), so it reaches the fused sizes from 1024 up only.
+constexpr int OS_STATE_MIN_NFFT = 1024;
+// the kernel argument for the state entries from element `off` on (a column's state in the generic path)
+template <typename E, bool STATE> static OsState<E, STATE> os_state_arg(const OsStateArgs& s, int64_t off) {
+    OsState<E, STATE> r{};
+    if constexpr (STATE)
+        r = {s.si_in ? reinterpret_cast<const E*>(s.si_in) + off : nullptr, s.si_out ? reinterpret_cast<E*>(s.si_out) + off : nullptr, s.nx};
+    return r;
+}
+
+template <typename T, int N, bool CPLX, bool STATE>
+static int launch_os_fused(OsPlanImpl* p, const OsRange& a, const OsStateArgs& s, cudaStream_t st) {
+    using E = typename os_elt<T, CPLX>::type;
     constexpr int NT = os_threads<T, N, CPLX>::value;
     const size_t smem = os_smem_bytes<T, N, CPLX>();
-    auto kern = os_fused_kernel<T, N, CPLX>;
+    auto kern = os_fused_kernel<T, N, CPLX, STATE>;
+    const OsState<E, STATE> sa = os_state_arg<E, STATE>(s, 0);
     const int64_t nblk = cdiv(a.out_count, p->L);
     const int64_t upc = CPLX ? nblk : (nblk + 1) / 2;
     const int64_t units = upc * a.ncols;
     if (units < 1) return DSPB200_OK;
     // persistent grid: one resident wave (CTAs per SM from the occupancy calculator: shared memory and register cap)
-    if (p->fused_per_sm < 1) {
+    int& per_sm = STATE ? p->fused_state_per_sm : p->fused_per_sm;
+    if (per_sm < 1) {
         DSP_TRY(set_smem(kern, smem));
         int per = 1;
         DSP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, kern, NT, smem));
-        p->fused_per_sm = per < 1 ? 1 : per;
+        per_sm = per < 1 ? 1 : per;
     }
-    const int per_sm = p->fused_per_sm;
     const int64_t cap = (int64_t)p->sm_count * per_sm;
     const int64_t blocks = units < cap ? units : cap;
     DSP_CUDA(launch_pdl(kern, (unsigned)blocks, NT, smem, st, a.u, a.u_begin, a.nu_local, a.u_col_stride, a.out, a.out_begin,
                         a.out_count, a.out_col_stride, a.zero_from, (int)p->nv, upc, units,
                         reinterpret_cast<const cx<T>*>(p->d_tw), reinterpret_cast<const cx<T>*>(p->d_t16),
-                        reinterpret_cast<const cx<T>*>(p->d_t256), reinterpret_cast<const cx<T>*>(p->d_H)));
+                        reinterpret_cast<const cx<T>*>(p->d_t256), reinterpret_cast<const cx<T>*>(p->d_H), sa));
     DSP_LAUNCH_OK();
     return DSPB200_OK;
 }
 
-template <typename T> static int os_fused_dispatch(OsPlanImpl* p, const OsRange& a, cudaStream_t st) {
+template <typename T, bool STATE> static int os_fused_dispatch(OsPlanImpl* p, const OsRange& a, const OsStateArgs& s, cudaStream_t st) {
     switch (p->nfft) {
-#define X(NN)                                                                                   \
-    case NN:                                                                                    \
-        if constexpr (sizeof(T) == 8 && NN > 8192) break;                                       \
-        else return p->cplx ? launch_os_fused<T, NN, true>(p, a, st) : launch_os_fused<T, NN, false>(p, a, st);
+#define X(NN)                                                                                                       \
+    case NN:                                                                                                        \
+        if constexpr ((sizeof(T) == 8 && NN > 8192) || (STATE && NN < OS_STATE_MIN_NFFT)) break;                    \
+        else return p->cplx ? launch_os_fused<T, NN, true, STATE>(p, a, s, st) : launch_os_fused<T, NN, false, STATE>(p, a, s, st);
         DSP_OS_SIZES(X)
 #undef X
     }
-    set_error("no fused overlap-save kernel for nfft=%lld", (long long)p->nfft);
+    set_error("no fused %soverlap-save kernel for nfft=%lld", STATE ? "stateful " : "", (long long)p->nfft);
     return DSPB200_EUNSUPPORTED;
 }
 
@@ -760,7 +838,7 @@ static int make_plans(bool cplx, bool f64, int64_t nfft, int64_t batch, cufftHan
     return DSPB200_OK;
 }
 
-template <typename T> static int os_generic_run(OsPlanImpl* p, const OsRange& a, cudaStream_t st) {
+template <typename T, bool STATE> static int os_generic_run(OsPlanImpl* p, const OsRange& a, const OsStateArgs& s, cudaStream_t st) {
     const int threads = 256;
     for (int64_t c = 0; c < a.ncols; ++c) {
         const char* ucol = (const char*)a.u + (size_t)(c * a.u_col_stride) * dtype_size(p->dtype);
@@ -777,19 +855,20 @@ template <typename T> static int os_generic_run(OsPlanImpl* p, const OsRange& a,
             os_cmul_kernel<T><<<grid_for(p->batch * p->nbins, threads), threads, 0, st>>>(reinterpret_cast<cx<T>*>(p->fd.p), reinterpret_cast<const cx<T>*>(p->d_H), p->nbins, p->batch);
             DSP_LAUNCH_OK();
             DSP_TRY(generic_exec_inv(p, p->inv, p->fd.p, p->td.p, st));
-            if (p->cplx) os_scatter_kernel<T, true><<<grid_for(nblk * p->L, threads), threads, 0, st>>>(p->td.p, m_first, p->L, p->nv, p->nfft, nblk, ocol, a.out_begin, a.out_begin + a.out_count, a.zero_from);
-            else os_scatter_kernel<T, false><<<grid_for(nblk * p->L, threads), threads, 0, st>>>(p->td.p, m_first, p->L, p->nv, p->nfft, nblk, ocol, a.out_begin, a.out_begin + a.out_count, a.zero_from);
+            if (p->cplx) os_scatter_kernel<T, true, STATE><<<grid_for(nblk * p->L, threads), threads, 0, st>>>(p->td.p, m_first, p->L, p->nv, p->nfft, nblk, ocol, a.out_begin, a.out_begin + a.out_count, a.zero_from, os_state_arg<cx<T>, STATE>(s, c * (p->nv - 1)));
+            else os_scatter_kernel<T, false, STATE><<<grid_for(nblk * p->L, threads), threads, 0, st>>>(p->td.p, m_first, p->L, p->nv, p->nfft, nblk, ocol, a.out_begin, a.out_begin + a.out_count, a.zero_from, os_state_arg<T, STATE>(s, c * (p->nv - 1)));
             DSP_LAUNCH_OK();
         }
     }
     return DSPB200_OK;
 }
 
-static int os_run(OsPlanImpl* p, const OsRange& a, cudaStream_t st) {
+template <bool STATE> static int os_run(OsPlanImpl* p, const OsRange& a, const OsStateArgs& s, cudaStream_t st) {
     if (a.out_count <= 0 || a.ncols <= 0) return DSPB200_OK;
-    if (p->fused) return p->f64 ? os_fused_dispatch<double>(p, a, st) : os_fused_dispatch<float>(p, a, st);
-    return p->f64 ? os_generic_run<double>(p, a, st) : os_generic_run<float>(p, a, st);
+    if (p->fused) return p->f64 ? os_fused_dispatch<double, STATE>(p, a, s, st) : os_fused_dispatch<float, STATE>(p, a, s, st);
+    return p->f64 ? os_generic_run<double, STATE>(p, a, s, st) : os_generic_run<float, STATE>(p, a, s, st);
 }
+static int os_run(OsPlanImpl* p, const OsRange& a, cudaStream_t st) { return os_run<false>(p, a, OsStateArgs{}, st); }
 
 static int64_t auto_nfft(int64_t nv, bool f64) {
     const int64_t nmax = f64 ? 8192 : 16384;
@@ -1112,6 +1191,46 @@ int dspb200_os_exec_range_dev(dspb200_os_plan* plan, const void* u_local, int64_
     return os_run(p, a, (cudaStream_t)stream);
 }
 
+// Stateful overlap-save (fftfilt(f::DF2TFilter, x)): outputs [0, nx + nv - 1) of each column, the first nv - 1 plus si_in,
+// the last nv - 1 into si_out (OsState).  One fused launch, or the generic path's launches per column.
+int dspb200_os_exec_state_dev(dspb200_os_plan* plan, const void* x, int64_t nx, int64_t ncols, const void* si_in, void* si_out,
+                              void* out, void* stream) {
+    DSP_RANGE("dspb200_os_exec_state_dev");
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    DSP_REQUIRE(nx >= 0 && ncols >= 0, "negative size");
+    OsPlanImpl* p = &plan->impl;
+    const int64_t ns = p->nv - 1;
+    const size_t sbytes = (size_t)(ns * ncols) * dtype_size(p->dtype);
+    const size_t xbytes = (size_t)(nx * ncols) * dtype_size(p->dtype);
+    // a column's first unit reads si_in while its last units write si_out, and units read the samples behind their
+    // neighbours' outputs: a buffer that is written must not overlap one that is read (or the other written one)
+    auto overlap = [](const void* a, size_t na, const void* b, size_t nb_) {
+        return a && b && na && nb_ && (const char*)a < (const char*)b + nb_ && (const char*)b < (const char*)a + na;
+    };
+    DSP_REQUIRE(!overlap(si_in, sbytes, si_out, sbytes), "si_in and si_out overlap");
+    DSP_REQUIRE(!overlap(x, xbytes, out, xbytes), "x and out overlap (filtering in place needs the host form)");
+    DSP_REQUIRE(!overlap(x, xbytes, si_out, sbytes) && !overlap(si_in, sbytes, out, xbytes) && !overlap(out, xbytes, si_out, sbytes),
+                "a state buffer overlaps x or out");
+    if (ncols == 0) return DSPB200_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (nx == 0) {                                                       // the state passes through unchanged
+        if (si_out && sbytes) {
+            if (si_in) DSP_CUDA(cudaMemcpyAsync(si_out, si_in, sbytes, cudaMemcpyDeviceToDevice, st));
+            else DSP_CUDA(cudaMemsetAsync(si_out, 0, sbytes, st));
+        }
+        return DSPB200_OK;
+    }
+    DSP_REQUIRE(x && out, "NULL argument");
+    if (p->fused && p->nfft < OS_STATE_MIN_NFFT) {
+        set_error("no stateful overlap-save kernel for nfft=%lld: the stateful form takes plans with nfft = 0 (library choice)",
+                  (long long)p->nfft);
+        return DSPB200_EUNSUPPORTED;
+    }
+    if (ns == 0) { si_in = nullptr; si_out = nullptr; }                  // nv == 1: no state
+    OsRange a{x, 0, nx, nx, out, 0, nx + (si_out ? ns : 0), nx, INT64_MAX, ncols};
+    return os_run<true>(p, a, OsStateArgs{si_in, si_out, nx}, st);
+}
+
 // Host pointers.  One long column is streamed: chunk c+1 is copied in while chunk c is convolved and chunk
 // c-1 is copied out (three streams, two buffers each); otherwise copy in -> run -> copy out.
 int dspb200_os_exec(dspb200_os_plan* plan, const void* u, int64_t nu, int64_t ncols, void* out, int64_t nout) {
@@ -1159,6 +1278,42 @@ int dspb200_os_exec(dspb200_os_plan* plan, const void* u, int64_t nu, int64_t nc
     if (in_bytes) DSP_CUDA(cudaMemcpyAsync(p->in[0].p, u, in_bytes, cudaMemcpyHostToDevice, p->s_exec));
     DSP_TRY(dspb200_os_exec_dev(plan, p->in[0].p, nu, ncols, p->out[0].p, nout, p->s_exec));
     DSP_CUDA(cudaMemcpyAsync(out, p->out[0].p, out_bytes, cudaMemcpyDeviceToHost, p->s_exec));
+    DSP_CUDA(cudaStreamSynchronize(p->s_exec));
+    return DSPB200_OK;
+}
+
+// Host pointers: x and the state are staged through plan scratch (x in in[0], [si_in | si_out] in in[1]), so out may be x and
+// si_out may be si_in.
+int dspb200_os_exec_state(dspb200_os_plan* plan, const void* x, int64_t nx, int64_t ncols, const void* si_in, void* si_out,
+                          void* out) {
+    DSP_RANGE("dspb200_os_exec_state");
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    DSP_REQUIRE(nx >= 0 && ncols >= 0, "negative size");
+    if (ncols == 0) return DSPB200_OK;
+    DSP_REQUIRE(nx == 0 || (x && out), "NULL argument");
+    OsPlanImpl* p = &plan->impl;
+    const size_t es = dtype_size(p->dtype);
+    const size_t bytes = (size_t)(nx * ncols) * es, sbytes = (size_t)((p->nv - 1) * ncols) * es;
+    if (nx == 0) {                                                       // the state passes through unchanged
+        if (si_out && sbytes && si_out != si_in) {
+            if (si_in) memmove(si_out, si_in, sbytes);
+            else memset(si_out, 0, sbytes);
+        }
+        return DSPB200_OK;
+    }
+    DSP_CUDA(cudaSetDevice(p->device));
+    DSP_TRY(ensure_streams(p));
+    DSP_TRY(p->in[0].reserve(bytes));
+    DSP_TRY(p->out[0].reserve(bytes));
+    DSP_TRY(p->in[1].reserve(2 * sbytes + 16));
+    char* d_si_in = (char*)p->in[1].p;
+    char* d_si_out = d_si_in + sbytes;
+    DSP_CUDA(cudaMemcpyAsync(p->in[0].p, x, bytes, cudaMemcpyHostToDevice, p->s_exec));
+    if (si_in && sbytes) DSP_CUDA(cudaMemcpyAsync(d_si_in, si_in, sbytes, cudaMemcpyHostToDevice, p->s_exec));
+    DSP_TRY(dspb200_os_exec_state_dev(plan, p->in[0].p, nx, ncols, si_in ? d_si_in : nullptr, si_out ? d_si_out : nullptr,
+                                      p->out[0].p, p->s_exec));
+    DSP_CUDA(cudaMemcpyAsync(out, p->out[0].p, bytes, cudaMemcpyDeviceToHost, p->s_exec));
+    if (si_out && sbytes) DSP_CUDA(cudaMemcpyAsync(si_out, d_si_out, sbytes, cudaMemcpyDeviceToHost, p->s_exec));
     DSP_CUDA(cudaStreamSynchronize(p->s_exec));
     return DSPB200_OK;
 }

@@ -1,5 +1,6 @@
 """PolynomialRatio and the stateful FIR filter DF2TFilter (src/Filters/coefficients.jl:66-216, src/Filters/filt.jl:17-30,
-100-224, src/deprecated.jl:1-101), backed by the stateful instances of the tiled FIR kernel (dspb200_fir_exec_state*).
+100-224, src/deprecated.jl:1-101), backed by the stateful instances of the tiled FIR kernel (dspb200_fir_exec_state*);
+fftfilt(f::DF2TFilter, x) runs the same filter on the stateful overlap-save instances (dspb200_os_exec_state*).
 
 In transposed direct form the FIR state is the partial multiply-add chain of the next nb - 1 outputs, so a signal
 filtered block by block through one DF2TFilter gives bit-identical results to one call over the whole signal.  The GPU
@@ -86,7 +87,8 @@ class DF2TFilter:
     Residency is fixed at construction.  A host filter keeps `state` as a numpy array (the `si` passed in, as the
     reference keeps its array) and updates it in place.  An `si` that is a DeviceArray, or device=True, keeps the state in
     device memory: the filter takes DeviceArray chunks of the state's eltype, returns DeviceArrays and launches one kernel
-    per non-empty chunk, alternating between two state buffers; `state` is the current one.  A DeviceArray `si` becomes
+    per non-empty chunk (fftfilt beyond the fused transform sizes: five per block batch and channel), alternating between
+    two state buffers; `state` is the current one.  A DeviceArray `si` becomes
     the first of the two buffers, so after an odd number of calls it holds an older state: read `f.state`, not `si`.
     A device call cannot filter in place: `out` must not overlap `x` (the host filter can)."""
 
@@ -127,6 +129,7 @@ class DF2TFilter:
             raise ArgumentError("length of state vector must match filter order")
         self._si = [si, DeviceArray(si.shape, si.dtype) if self.device else None]
         self._plan = None
+        self._os = None
 
     @property
     def state(self):
@@ -157,6 +160,11 @@ class DF2TFilter:
             self._plan = _lib.FirPlan(np.ascontiguousarray(self.coef.coefb, dtype=S))
         return self._plan
 
+    def _os_plan(self, S):
+        if self._os is None:
+            self._os = _lib.OsPlan(np.ascontiguousarray(self.coef.coefb, dtype=S), 0)
+        return self._os
+
     def _check_shapes(self, out, x):
         if tuple(x.shape) != tuple(out.shape):
             raise ArgumentError("out size must match x")
@@ -165,35 +173,54 @@ class DF2TFilter:
 
     def filt(self, x):
         """filt(f::DF2TFilter, x), src/Filters/filt.jl:215-224: output eltype promote_type(eltype(state), eltype(x))."""
+        return self._apply(x, self._fir_plan)
+
+    def filt_(self, out, x):
+        """filt!(out, f::DF2TFilter, x), src/Filters/filt.jl:157-181."""
+        return self._apply_(out, x, self._fir_plan)
+
+    def fftfilt(self, x):
+        """fftfilt(f::DF2TFilter, x): the same stateful filter as filt(f, x), computed by overlap-save FFT convolution
+        (dspb200_os_exec_state*).  The state is the same transposed direct-form state, so filt and fftfilt may alternate on
+        one filter chunk by chunk.  filt is bit-identical to the reference's loop; fftfilt is within FFT rounding of it and
+        costs about the same per output whatever the filter length.  Like the other GPU paths (and unlike the reference's
+        real-only fftfilt) it takes Float32, Float64, ComplexF32 and ComplexF64, with filt's eltype rules."""
+        return self._apply(x, self._os_plan)
+
+    def fftfilt_(self, out, x):
+        """fftfilt!(out, f::DF2TFilter, x): fftfilt(f, x) into out (see fftfilt)."""
+        return self._apply_(out, x, self._os_plan)
+
+    def _apply(self, x, plan):
+        """filt / fftfilt: `plan(S)` is the plan whose exec_state / exec_state_dev runs the chunk."""
         if self.device:
             if not isinstance(x, DeviceArray):
                 raise ArgumentError("a DF2TFilter with device-resident state filters DeviceArrays")
             S = self._eltype(x.dtype)
-            return self._filt_device(DeviceArray(x.shape, S), x, S)
+            return self._filt_device(DeviceArray(x.shape, S), x, S, plan)
         if isinstance(x, DeviceArray):
             raise ArgumentError("a DF2TFilter with host state filters host arrays (construct it with device=True)")
         x = np.asarray(x)
         S = self._eltype(x.dtype)
-        return self._filt_host(np.empty(x.shape, dtype=S, order="F"), x, S)
+        return self._filt_host(np.empty(x.shape, dtype=S, order="F"), x, S, plan)
 
-    def filt_(self, out, x):
-        """filt!(out, f::DF2TFilter, x), src/Filters/filt.jl:157-181."""
+    def _apply_(self, out, x, plan):
         if self.device:
             if not (isinstance(x, DeviceArray) and isinstance(out, DeviceArray)):
                 raise ArgumentError("a DF2TFilter with device-resident state filters DeviceArrays into DeviceArrays")
             S = self._eltype(x.dtype)
             if out.dtype != S:
                 raise ArgumentError(f"out must have the state's eltype {S}")
-            return self._filt_device(out, x, S)
+            return self._filt_device(out, x, S, plan)
         if isinstance(x, DeviceArray) or isinstance(out, DeviceArray):
             raise ArgumentError("a DF2TFilter with host state filters host arrays (construct it with device=True)")
         x = np.asarray(x)
         S = self._eltype(x.dtype)
         if S.kind == "c" and np.dtype(out.dtype).kind != "c":
             raise InexactError(f"a {S} filter output cannot be stored in a real `out` (InexactError in the reference)")
-        return self._filt_host(out, x, S)
+        return self._filt_host(out, x, S, plan)
 
-    def _filt_host(self, out, x, S):
+    def _filt_host(self, out, x, S, plan):
         self._check_shapes(out, x)
         nx = x.shape[0]
         ns = self.nstate
@@ -203,13 +230,13 @@ class DF2TFilter:
         res = np.empty((nx, ncols), dtype=S, order="F")
         si = np.asfortranarray(self.state.reshape(ns, ncols), dtype=S) if ns else None
         so = np.empty((ns, ncols), dtype=S, order="F") if ns else None
-        self._fir_plan(S).exec_state(xS, nx, ncols, si, so, res)
+        plan(S).exec_state(xS, nx, ncols, si, so, res)
         out[...] = res.reshape(x.shape)          # column c <-> trailing index c in C order, for x and the state alike
         if ns:
             self.state[...] = so.reshape(self.state.shape)
         return out
 
-    def _filt_device(self, out, x, S):
+    def _filt_device(self, out, x, S, plan):
         self._check_shapes(out, x)
         if x.dtype != S:
             raise ArgumentError(f"device chunks must have the state's eltype {S} (got {x.dtype})")
@@ -224,7 +251,7 @@ class DF2TFilter:
         nx = x.shape[0]
         if nx == 0 or x.size == 0:
             return out
-        self._fir_plan(S).exec_state_dev(x.ptr, nx, x.size // nx, cur.ptr, nxt.ptr, out.ptr, 0)
+        plan(S).exec_state_dev(x.ptr, nx, x.size // nx, cur.ptr, nxt.ptr, out.ptr, 0)
         self._si = [nxt, cur]
         return out
 

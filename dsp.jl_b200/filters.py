@@ -7,6 +7,7 @@ from fractions import Fraction
 import numpy as np
 
 from . import _lib
+from .df2t import DF2TFilter
 from .device import DeviceArray
 from .dspbase import SMALL_FILT_CUTOFF, _cols, _gpu_dtype, _os_plan, _promote, filt_ as _filt_ba, optimalfftfiltlength
 from .errors import ArgumentError, DomainError
@@ -37,7 +38,12 @@ def _require_real(b, x):
 def fftfilt(b, x, nfft=None):
     """fftfilt(b, x[, nfft]), src/Filters/filt.jl:458-461: real overlap-save along axis 0 of every column.
     nfft=None lets the library choose the block transform (the reference default is the CPU cost model
-    optimalfftfiltlength); an explicit nfft is honoured."""
+    optimalfftfiltlength); an explicit nfft is honoured.
+    fftfilt(f::DF2TFilter, x) is the stateful form (DF2TFilter.fftfilt): filt(f, x) by overlap-save, carrying f's state."""
+    if isinstance(b, DF2TFilter):
+        if nfft is not None:
+            raise ArgumentError("fftfilt(f::DF2TFilter, x) takes no nfft (the library chooses the block transform)")
+        return b.fftfilt(x)
     b = np.asarray(b)
     if isinstance(x, DeviceArray):                       # device pipeline form: same-length overlap-save, stays in HBM
         if np.iscomplexobj(b) or x.dtype.kind == "c":
@@ -54,7 +60,11 @@ def fftfilt(b, x, nfft=None):
 
 
 def fftfilt_(out, b, x, nfft=None):
-    """fftfilt!(out, b, x[, nfft]), src/Filters/filt.jl:468-476."""
+    """fftfilt!(out, b, x[, nfft]), src/Filters/filt.jl:468-476; fftfilt!(out, f::DF2TFilter, x) is the stateful form."""
+    if isinstance(b, DF2TFilter):
+        if nfft is not None:
+            raise ArgumentError("fftfilt!(out, f::DF2TFilter, x) takes no nfft (the library chooses the block transform)")
+        return b.fftfilt_(out, x)
     b = np.asarray(b)
     x = np.asarray(x)
     _require_real(b, x)

@@ -133,6 +133,26 @@ function fftfilt!(out::Array{T}, b::Vector{T}, x::Array{T}, nfft::Integer=0) whe
     return out
 end
 fftfilt(b::Vector{T}, x::Array{T}, nfft::Integer=0) where {T<:GPUReal} = fftfilt!(similar(x), b, x, nfft)
+# fftfilt!(out, f::DF2TFilter{<:PolynomialRatio}, x) (an extension, not in DSP.jl): filt!(out, f, x) computed by overlap-save,
+# with the same state (updated in place through the host form's staging), within FFT rounding of filt!.  FIR coefficients
+# of the state's GPU eltype, as for filt! above; the block transform is the library's choice.
+function fftfilt!(out::Array{S,N}, f::Filters.DF2TFilter{<:Filters.PolynomialRatio,Array{S,N}}, x::Array{S,N}) where {S<:GPUNumber,N}
+    size(x) != size(out) && throw(ArgumentError("out size must match x"))
+    si = f.state
+    size(x)[2:end] != size(si)[2:end] && throw(ArgumentError("state size must match x"))
+    b = Filters.coefb(f.coef)
+    length(Filters.coefa(f.coef)) == 1 || throw(ArgumentError("fftfilt! takes FIR coefficients (length(coefa) == 1)"))
+    promote_type(eltype(b), S) == S || throw(ArgumentError("the coefficients must promote into the state's eltype $S"))
+    iszero(length(x)) && return out
+    plan = os_plan(convert(Vector{S}, b), 0)
+    nx = size(x, 1)
+    GC.@preserve x out si check(ccall((:dspb200_os_exec_state, libdspb200), Cint,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Int64, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}), plan.ptr, x, nx, length(x) ÷ nx, si, si, out))
+    close!(plan)
+    return out
+end
+fftfilt(f::Filters.DF2TFilter{<:Filters.PolynomialRatio,Array{S,N}}, x::Array{S,N}) where {S<:GPUNumber,N} =
+    fftfilt!(similar(x), f, x)
 tdfilt(h::Vector{T}, x::Array{T}) where {T<:GPUNumber} = filt(h, one(T), x)            # src/Filters/filt.jl:431-433
 # filt(h, x): src/Filters/filt.jl:525-555 (Real x Real with more than 66 taps -> overlap-save)
 filt(h::Vector{T}, x::Array{T}) where {T<:GPUReal} =

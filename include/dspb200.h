@@ -116,6 +116,22 @@ DSPB200_API int dspb200_os_exec_dev(dspb200_os_plan* plan, const void* u, int64_
  * [u_begin, u_begin+nu_local) are stored at `u_local` (everything outside is zero).  No collective. */
 DSPB200_API int dspb200_os_exec_range_dev(dspb200_os_plan* plan, const void* u_local, int64_t u_begin, int64_t nu_local,
                               void* out_local, int64_t out_begin, int64_t out_count, void* stream);
+/* Stateful overlap-save: fftfilt(f::DF2TFilter, x) / fftfilt!(out, f::DF2TFilter, x), the overlap-save counterpart of
+ * dspb200_fir_exec_state with the same state: si_in / si_out hold the transposed direct-form FIR state, (nv-1) x ncols
+ * column-major in the plan's dtype.  Per column, with full = conv(v, x) (nx + nv - 1 outputs), full[i] += si_in[i] for
+ * i < nv-1, out = full[0 .. nx-1] and si_out = full[nx .. nx+nv-2]; so a chunked stream fed back its si_out equals the
+ * stateful FIR filter within FFT rounding, and the two entry points may alternate on one state.  si_in == NULL means a zero
+ * state, si_out == NULL discards the final state.  nx == 0 passes the state through; nv == 1 has no state.  Takes plans made
+ * with nfft = 0 (a fused plan with nfft < 1024 gives DSPB200_EUNSUPPORTED).  The _dev form takes device pointers, enqueues
+ * one kernel on `stream` (fused sizes; the generic path launches per column) and returns; there no two of x, out, si_in and
+ * si_out may overlap where one of them is written (x with out, si_in with si_out, a state buffer with x or out):
+ * DSPB200_EINVALID before any launch, because a column's first unit reads si_in while its last units write si_out, and
+ * units read the samples behind their neighbours' outputs.  The host form stages x and the state through plan scratch, so
+ * there out may be x and si_out may be si_in. */
+DSPB200_API int dspb200_os_exec_state(dspb200_os_plan* plan, const void* x, int64_t nx, int64_t ncols, const void* si_in,
+                                      void* si_out, void* out);
+DSPB200_API int dspb200_os_exec_state_dev(dspb200_os_plan* plan, const void* x, int64_t nx, int64_t ncols, const void* si_in,
+                                          void* si_out, void* out, void* stream);
 DSPB200_API int dspb200_os_plan_destroy(dspb200_os_plan* plan);
 
 /* conv(u, v; algorithm=:fft_simple) / _conv_kern_fft!: src/dspbase.jl:611-644 -- one FFT pair of size
