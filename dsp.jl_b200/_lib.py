@@ -83,6 +83,8 @@ SIGNATURES = {
     "dspb200_welch_begin_dev": (_int, [_vp, _vp]),
     "dspb200_welch_accumulate_dev": (_int, [_vp, _vp, _i64, _i64, _i64, _i64, _vp]),
     "dspb200_welch_finalize_dev": (_int, [_vp, _dbl, _vp, _vp]),
+    "dspb200_spec_plan_pin_welch": (_int, [_vp, _int, _int, _int, _i64]),
+    "dspb200_spec_plan_welch_config": (_int, [_vp, _int, _int, C.POINTER(_int), C.POINTER(_int), C.POINTER(_i64)]),
     "dspb200_filt_welch_exec": (_int, [_vp, _vp, _vp, _i64, _dbl, _vp]),
     "dspb200_os_plan_geometry": (_int, [_vp, C.POINTER(_int), C.POINTER(_i64), C.POINTER(_i64)]),
     "dspb200_spec_plan_geometry": (_int, [_vp, C.POINTER(_int), C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_i64)]),
@@ -274,6 +276,18 @@ class SpecPlan(_Plan):
 
     def welch_finalize_dev(self, r, out_ptr, stream=0):
         check(lib.dspb200_welch_finalize_dev(self.handle, float(r), out_ptr, stream))
+
+    def pin_welch(self, batched, mode, groups, vctas=0):
+        """Testing aid: run the fused Welch kernel instance (mode, groups) on `vctas` virtual CTAs (0: one resident wave);
+        mode < 0 unpins.  Unaligned calls run mode 0, one group (dspb200_spec_plan_pin_welch)."""
+        check(lib.dspb200_spec_plan_pin_welch(self.handle, 1 if batched else 0, int(mode), int(groups), int(vctas)))
+
+    def welch_config(self, batched, aligned):
+        """(mode, groups, virtual CTAs) of the last fused Welch launch of that form and alignment class; groups = 0: none."""
+        m, g, v = _int(0), _int(0), _i64(0)
+        check(lib.dspb200_spec_plan_welch_config(self.handle, 1 if batched else 0, 1 if aligned else 0, C.byref(m), C.byref(g),
+                                                 C.byref(v)))
+        return m.value, g.value, v.value
 
     def filt_welch_ptr(self, os_plan, x_ptr, n, r, out_ptr):
         check(lib.dspb200_filt_welch_exec(os_plan.handle, self.handle, x_ptr, int(n), float(r), out_ptr))

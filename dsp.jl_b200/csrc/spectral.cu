@@ -40,7 +40,9 @@ struct SpecPlanImpl {
     DevBuf tmp;                   // multitaper spectrogram: one taper's PSD matrix
     // launch configuration of the fused Welch kernel, chosen once per (plan, alignment class): the selection walks up to nine
     // kernel instances through cudaFuncSetAttribute + the occupancy calculator (tens of microseconds per launch otherwise)
-    struct WelchCfg { void* kern = nullptr; size_t smem = 0; int g = 0, per_sm = 0, threads = 0; };
+    // (mode: MODE of the instance; vctas: virtual CTAs pinned by dspb200_spec_plan_pin_welch, 0 = one resident wave;
+    //  used: virtual CTAs of the last launch, 0 = none yet)
+    struct WelchCfg { void* kern = nullptr; size_t smem = 0; int g = 0, per_sm = 0, threads = 0, mode = -1; int64_t vctas = 0, used = 0; };
     WelchCfg welch_cfg[2];        // [0]: unaligned segments (direct loads), [1]: TMA-capable
     int nparts = 0;               // CTAs of the Welch kernel == rows of `partial`
     int rows_used = 0;            // rows of `partial` written since welch_begin (host bookkeeping, stream order = call order)
@@ -73,6 +75,11 @@ template <typename T> struct win_t { using type = double; };
 template <> struct win_t<float> { using type = float2; };
 __device__ __forceinline__ double win_mul(double v, double w) { return v * w; }
 __device__ __forceinline__ float win_mul(float v, float2 w) { return fmaf(v, w.x, v * w.y); }
+
+// out + val rounded once per operation: the accumulate form of a PSD store (psd_only == 3) must give the eltype sum of the
+// two stored values, which a contraction of val's product into the add (one FMA, one rounding) would not
+__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
 
 template <typename T, bool CPLX> struct in_type { using type = T; };
 template <typename T> struct in_type<T, true> { using type = cx<T>; };
@@ -212,16 +219,19 @@ welch_fused_kernel(const void* __restrict__ s_, int64_t seg0, int64_t nseg, int6
             }
         };
         // first pass: the staged samples are read and transformed, then -- one barrier later, which also ends the
-        // previous unit's last pass -- stored; once every thread is past its reads the staging buffer is refilled with
-        // the next unit while the remaining passes run
+        // previous unit's last pass -- stored; once every thread is past its reads (the barrier after the pass: with two
+        // first-pass iterations, N = 16384, the second one reads after the pass's own barrier) the staging buffer is
+        // refilled with the next unit while the remaining passes run -- behind a proxy fence, which orders those
+        // generic-proxy reads before the bulk copy's async-proxy writes
         fft_first_pass<T, N, NT, true>(ctx, tid, ld0, scope);
+        scope.sync();
         if constexpr (TMA) {
             if (tid == 0 && u + 1 < u1) {
+                fence_proxy_async_shared();
                 mbar_expect_tx(bar, unit_bytes(u + 1));
                 tma_load_1d(stage, unit_src(u + 1), unit_bytes(u + 1), bar);
             }
         }
-        scope.sync();
         fft_middle<T, N, NT>(ctx, tid, scope);
 #pragma unroll
         for (int it = 0; it < ITL; ++it) {
@@ -401,18 +411,19 @@ welch_batch_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t nse
                 }
             };
             fft_first_pass<T, N, NT, true>(ctx, tid, ld0, scope);
+            scope.sync();                               // every read of the staging buffer is done (welch_fused_kernel)
             if constexpr (TMA) {
                 // the next unit: the following one of this item, else the first one of the next item
                 if (tid == 0) {
                     int64_t nc = c, nu = u + 1, nub = ub;
                     if (nu == ub && item + 1 < i1) item_range(item + 1, nc, nu, nub);
                     if (nu < nub) {
+                        fence_proxy_async_shared();
                         mbar_expect_tx(bar, unit_bytes(nu));
                         tma_load_1d(stage, unit_src(nc, nu), unit_bytes(nu), bar);
                     }
                 }
             }
-            scope.sync();
             fft_middle<T, N, NT>(ctx, tid, scope);
 #pragma unroll
             for (int it = 0; it < ITL; ++it) {
@@ -489,7 +500,7 @@ __device__ __forceinline__ void stft_emit(const cx<T>* __restrict__ sm, void* __
     constexpr int NT = fft_threads<N>::value;
     // ACC: PSD columns are ADDED to what `out` holds (multitaper spectrogram: one launch per taper, no separate add pass).
     // Compile time: as a run-time predicate the read-modify-write put a scoreboard wait in front of every store (ncu).
-    auto put = [&](T* ptr, T val) { if constexpr (ACC) *ptr = *ptr + val; else *ptr = val; };
+    auto put = [&](T* ptr, T val) { if constexpr (ACC) *ptr = add_rn(*ptr, val); else *ptr = val; };
     const bool hasB = HASB < 0 ? hasB_rt : (HASB != 0);
     const bool onesided = ONES < 0 ? (onesided_rt != 0) : (ONES != 0);
     // `edge`: the bin is DC or Nyquist (scaled by m1 even in a one-sided PSD, src/periodograms.jl:142-172)
@@ -577,8 +588,8 @@ __device__ __forceinline__ void stft_unit(const FftCtx<T>& ctx, cx<T>* sm, int t
     };
     // (the barrier inside the first pass also ends the previous unit's emit step)
     fft_first_pass<T, N, NT, true>(ctx, tid, ld0);
-    issue_next();                                        // every thread has read the staging buffer: refill it
     __syncthreads();
+    issue_next();                                        // every thread has read the staging buffer: refill it
     fft_middle<T, N, NT>(ctx, tid);
 #pragma unroll
     for (int it = 0; it < ITL; ++it) {
@@ -662,6 +673,7 @@ stft_fused_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, i
         auto issue_next = [&]() {
             if constexpr (TMA) {
                 if (tid == 0 && gu + 1 < u1) {
+                    fence_proxy_async_shared();          // after the generic-proxy reads of the staging buffer
                     mbar_expect_tx(bar, bytes_of(nuin));
                     tma_load_1d(stage, src_of(nchan, nuin), bytes_of(nuin), bar);
                 }
@@ -779,6 +791,7 @@ stft_w1k_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int
         }
         __syncwarp();                                   // every lane has read the staging buffer (and the previous unit's spectrum)
         if (lane == 0 && gu + 1 < u1) {                 // refill it with the next unit while this one is transformed
+            fence_proxy_async_shared();
             mbar_expect_tx(bar, bytes_of(nuin));
             tma_load_1d(stage, src_of(nchan, nuin), bytes_of(nuin), bar);
         }
@@ -808,7 +821,7 @@ stft_w1k_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int
         //  in front of every one of them)
         auto emit_all = [&](auto acc_) {
             constexpr bool ACC = decltype(acc_)::value;
-            auto put = [&](T* ptr, T val) { if constexpr (ACC) *ptr = *ptr + val; else *ptr = val; };
+            auto put = [&](T* ptr, T val) { if constexpr (ACC) *ptr = add_rn(*ptr, val); else *ptr = val; };
             auto emit = [&](int kk, cx<T> zk, cx<T> zm, bool edge) {
                 if (psd_only) {
                     T* out = reinterpret_cast<T*>(out_);
@@ -1062,13 +1075,14 @@ static int launch_welch_fused(SpecPlanImpl* p, const void* s, int64_t seg0, int6
     if (cached.kern != nullptr) {
         const int64_t cap = (int64_t)p->sm_count * cached.per_sm;
         const int64_t want = cdiv(units, cached.g);
-        const int grid = (int)(want < cap ? want : cap);
+        const int grid = cached.vctas ? (int)(cached.vctas / cached.g) : (int)(want < cap ? want : cap);
         DSP_CUDA(launch_pdl(reinterpret_cast<Kern>(cached.kern), (unsigned)grid, (unsigned)cached.threads, cached.smem, st,
                             s, seg0, nseg, p->hop, (int)p->n, sample_offset, win, reinterpret_cast<const cx<T>*>(p->d_tw),
                             reinterpret_cast<const cx<T>*>(p->d_t16), reinterpret_cast<const cx<T>*>(p->d_t256),
                             reinterpret_cast<T*>(p->partial.p), p->rows_used));
         DSP_LAUNCH_OK();
         if (grid * cached.g > p->rows_used) p->rows_used = grid * cached.g;
+        cached.used = (int64_t)grid * cached.g;
         return DSPB200_OK;
     }
     // candidates are offered in order of preference (measured sweep); the first one that
@@ -1113,7 +1127,7 @@ static int launch_welch_fused(SpecPlanImpl* p, const void* s, int64_t seg0, int6
     DSP_REQUIRE(best.k != nullptr, "no Welch kernel configuration fits (nfft=%lld)", (long long)p->nfft);
     DSP_TRY(set_smem(best.k, best.smem));              // (the last candidate examined may have left a different limit)
     cached.kern = reinterpret_cast<void*>(best.k); cached.smem = best.smem; cached.g = best.g; cached.per_sm = best.per_sm;
-    cached.threads = NT * best.g;
+    cached.threads = NT * best.g; cached.mode = best.mode;
     // one wave of persistent CTAs: exactly the number that is co-resident; (CTAs x groups) never exceeds the rows of `partial`
     const int64_t cap = (int64_t)p->sm_count * best.per_sm;
     const int64_t want = cdiv(units, best.g);
@@ -1123,6 +1137,7 @@ static int launch_welch_fused(SpecPlanImpl* p, const void* s, int64_t seg0, int6
                         reinterpret_cast<const cx<T>*>(p->d_t256), reinterpret_cast<T*>(p->partial.p), p->rows_used));
     DSP_LAUNCH_OK();
     if (grid * best.g > p->rows_used) p->rows_used = grid * best.g;
+    cached.used = (int64_t)grid * best.g;
     return DSPB200_OK;
 }
 
@@ -1173,9 +1188,9 @@ static int launch_welch_batch(SpecPlanImpl* p, const void* s, int64_t len, int64
     const W* win = reinterpret_cast<const W*>(p->d_window);
     SpecPlanImpl::WelchCfg& cfg = p->welch_batch_cfg[aligned ? 1 : 0];
     if (cfg.kern == nullptr) {
-        struct Cand { Kern k; size_t smem; int g, warps, per_sm; };
-        Cand best{nullptr, 0, 0, -1, 0};
-        auto consider = [&](Kern kn, size_t smem, int g) -> int {
+        struct Cand { Kern k; size_t smem; int mode, g, warps, per_sm; };
+        Cand best{nullptr, 0, 0, 0, -1, 0};
+        auto consider = [&](Kern kn, size_t smem, int mode, int g) -> int {
             if (best.warps >= 12) return DSPB200_OK;
             if (smem > p->smem_optin) return DSPB200_OK;
             DSP_TRY(set_smem(kn, smem));
@@ -1183,11 +1198,12 @@ static int launch_welch_batch(SpecPlanImpl* p, const void* s, int64_t len, int64
             DSP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kn, NT * g, smem));
             if (per_sm < 1) return DSPB200_OK;
             const int warps = per_sm * g * NT / 32;
-            if (warps > best.warps) best = Cand{kn, smem, g, warps, per_sm};
+            if (warps > best.warps) best = Cand{kn, smem, mode, g, warps, per_sm};
             return DSPB200_OK;
         };
-#define DSP_WELCH_CAND(MODE_, G_) \
-    DSP_TRY(consider(welch_batch_kernel<T, N, CPLX, MODE_, G_>, welch_layout<T, N, CPLX, MODE_>::total(p->n, p->hop, G_), G_))
+#define DSP_WELCH_CAND(MODE_, G_)                                                                                    \
+    DSP_TRY(consider(welch_batch_kernel<T, N, CPLX, MODE_, G_>, welch_layout<T, N, CPLX, MODE_>::total(p->n, p->hop, G_), \
+                     MODE_, G_))
         constexpr bool WREGOK = sizeof(T) == 4 && N <= 4096;
         if (aligned) {
             if (win) {
@@ -1210,10 +1226,10 @@ static int launch_welch_batch(SpecPlanImpl* p, const void* s, int64_t len, int64
         DSP_REQUIRE(best.k != nullptr, "no batched Welch kernel configuration fits (nfft=%lld)", (long long)p->nfft);
         DSP_TRY(set_smem(best.k, best.smem));
         cfg.kern = reinterpret_cast<void*>(best.k); cfg.smem = best.smem; cfg.g = best.g; cfg.per_sm = best.per_sm;
-        cfg.threads = NT * best.g;
+        cfg.threads = NT * best.g; cfg.mode = best.mode;
     }
     const int64_t upc = CPLX ? k : (k + 1) / 2;
-    const int64_t cap = (int64_t)p->sm_count * cfg.per_sm;           // resident CTAs: one wave
+    const int64_t cap = cfg.vctas ? cfg.vctas / cfg.g : (int64_t)p->sm_count * cfg.per_sm;   // resident CTAs: one wave
     const int64_t nv = cap * cfg.g;                                   // resident virtual CTAs
     const int64_t rows_cap = (int64_t)(WELCH_BATCH_SCRATCH / ((size_t)N * sizeof(T)));
     const int64_t gc_max = nchan < rows_cap ? nchan : rows_cap;
@@ -1232,6 +1248,7 @@ static int launch_welch_batch(SpecPlanImpl* p, const void* s, int64_t len, int64
                             (const void*)((const In*)s + c0 * len), len, k, upc, per, (int)slices, nitems, p->hop, (int)p->n,
                             win, tw, g16, g256, reinterpret_cast<T*>(p->bpartial.p)));
         DSP_LAUNCH_OK();
+        cfg.used = (int64_t)grid * cfg.g;
         const int nw = slices < 32 ? (int)slices : 32;
         welch_batch_finalize_kernel<T, N><<<dim3((unsigned)cdiv(p->nout, 32), (unsigned)gc), 32 * nw, 0, st>>>(
             reinterpret_cast<const T*>(p->bpartial.p), (int)slices, reinterpret_cast<T*>(out) + c0 * p->nout, (int)p->nout,
@@ -1248,7 +1265,10 @@ static int launch_stft_fused(SpecPlanImpl* p, const void* s, int64_t len, int64_
     using In = typename in_type<T, CPLX>::type;
     const size_t base = (size_t)fft_smem_elems<T, N>() * sizeof(cx<T>);
     const size_t stage = (size_t)(CPLX ? p->n : p->hop + p->n) * sizeof(In) + 16;
-    const bool tma = ((uintptr_t)s % 16 == 0) && ((len * sizeof(In)) % 16 == 0 || nchan == 1) &&
+    // Float32, N = 1024: every call that meets the TMA alignment conditions runs stft_w1k_kernel (its shared memory is at
+    // most about 84 KB), so the fallback below is the direct-load instance alone
+    constexpr bool W1K = sizeof(T) == 4 && N == 1024;
+    const bool tma = !W1K && ((uintptr_t)s % 16 == 0) && ((len * sizeof(In)) % 16 == 0 || nchan == 1) &&
                      ((p->hop * sizeof(In)) % 16 == 0) && ((p->n * sizeof(In)) % 16 == 0) &&
                      (base + stage <= p->smem_optin) && (base + stage <= 100 * 1024 || N >= 8192);   // N >= 8192: one CTA per SM anyway
     const size_t smem = tma ? base + stage : base;
@@ -1256,7 +1276,7 @@ static int launch_stft_fused(SpecPlanImpl* p, const void* s, int64_t len, int64_
     const int64_t units = upc * nchan;
     if (units < 1) return DSPB200_OK;
     const auto* w = reinterpret_cast<const typename win_t<T>::type*>(p->d_window);
-    if constexpr (sizeof(T) == 4 && N == 1024) {
+    if constexpr (W1K) {
         // one warp per unit (stft_w1k_kernel): needs the TMA alignment conditions
         const bool aligned = ((uintptr_t)s % 16 == 0) && ((len * sizeof(In)) % 16 == 0 || nchan == 1) &&
                              ((p->hop * sizeof(In)) % 16 == 0) && ((p->n * sizeof(In)) % 16 == 0);
@@ -1290,7 +1310,9 @@ static int launch_stft_fused(SpecPlanImpl* p, const void* s, int64_t len, int64_
     // window presence is a compile-time property of the Float32 kernels (predicated-off window products still issue)
     constexpr bool SPEC = sizeof(T) == 4;
     Kern kern;
-    if constexpr (SPEC) {
+    if constexpr (W1K) {
+        kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, false, 1> : (Kern)stft_fused_kernel<T, N, CPLX, false, 0>;
+    } else if constexpr (SPEC) {
         if (tma) kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, true, 1> : (Kern)stft_fused_kernel<T, N, CPLX, true, 0>;
         else kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, false, 1> : (Kern)stft_fused_kernel<T, N, CPLX, false, 0>;
     } else {
@@ -1323,10 +1345,14 @@ template <typename T> static int welch_fused_dispatch(SpecPlanImpl* p, const voi
 }
 template <typename T> static int welch_finalize_dispatch(SpecPlanImpl* p, double r, void* out, cudaStream_t st) {
     switch (p->nfft) {
-#define X(NN) case NN: return launch_welch_finalize<T, NN>(p, r, out, st);
+#define X(NN)                                                                                               \
+    case NN:                                                                                                \
+        if constexpr (sizeof(T) == 8 && NN > 8192) break;                                                   \
+        else return launch_welch_finalize<T, NN>(p, r, out, st);
         DSP_FUSED_SIZES(X)
 #undef X
     }
+    set_error("no fused Welch kernel for nfft=%lld", (long long)p->nfft);
     return DSPB200_EUNSUPPORTED;
 }
 template <typename T> static int welch_batch_dispatch(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan, int64_t k,
@@ -1337,6 +1363,86 @@ template <typename T> static int welch_batch_dispatch(SpecPlanImpl* p, const voi
         if constexpr (sizeof(T) == 8 && NN > 8192) break;                                                   \
         else return p->cplx ? launch_welch_batch<T, NN, true>(p, s, len, nchan, k, r, out, st)              \
                             : launch_welch_batch<T, NN, false>(p, s, len, nchan, k, r, out, st);
+        DSP_FUSED_SIZES(X)
+#undef X
+    }
+    set_error("no fused Welch kernel for nfft=%lld", (long long)p->nfft);
+    return DSPB200_EUNSUPPORTED;
+}
+
+// Pinned Welch launch configuration (dspb200_spec_plan_pin_welch, a testing aid).  The instances are exactly the candidates
+// of the preference lists in launch_welch_fused / launch_welch_batch: nothing is compiled for the hook alone.
+template <typename T, int N, bool CPLX, bool BATCH> static void* welch_instance(int mode, int g) {
+    constexpr bool MULTI = sizeof(T) == 4 && N >= 1024 && N <= 4096;
+    constexpr bool WREGOK = sizeof(T) == 4 && N <= 4096;
+#define DSP_WELCH_INST(MODE_, G_)                                                                       \
+    if (mode == MODE_ && g == G_)                                                                       \
+        return BATCH ? reinterpret_cast<void*>(welch_batch_kernel<T, N, CPLX, MODE_, G_>)               \
+                     : reinterpret_cast<void*>(welch_fused_kernel<T, N, CPLX, MODE_, G_>);
+    DSP_WELCH_INST(0, 1) DSP_WELCH_INST(1, 1) DSP_WELCH_INST(2, 1)
+    if constexpr (WREGOK) { DSP_WELCH_INST(3, 1) }
+    if constexpr (MULTI) {
+        DSP_WELCH_INST(1, 2) DSP_WELCH_INST(2, 2)
+        if constexpr (CPLX) { DSP_WELCH_INST(3, 2) }
+        else { DSP_WELCH_INST(1, 3) DSP_WELCH_INST(2, 3) }
+    }
+#undef DSP_WELCH_INST
+    return nullptr;
+}
+template <typename T, int N, bool CPLX> static size_t welch_smem(int mode, int64_t n, int64_t hop, int g) {
+    switch (mode) {
+    case 0: return welch_layout<T, N, CPLX, 0>::total(n, hop, g);
+    case 1: return welch_layout<T, N, CPLX, 1>::total(n, hop, g);
+    case 2: return welch_layout<T, N, CPLX, 2>::total(n, hop, g);
+    default: return welch_layout<T, N, CPLX, 3>::total(n, hop, g);
+    }
+}
+// Fills both alignment classes of the cache: aligned calls get (mode, g), unaligned ones MODE 0, G = 1; both `vctas`.
+template <typename T, int N, bool CPLX>
+static int welch_pin(SpecPlanImpl* p, bool batched, int mode, int g, int64_t vctas) {
+    constexpr int NT = fft_threads<N>::value;
+    SpecPlanImpl::WelchCfg pinned[2];
+    for (int a = 0; a < 2; ++a) {
+        const int m = a ? mode : 0, gg = a ? g : 1;
+        void* k = batched ? welch_instance<T, N, CPLX, true>(m, gg) : welch_instance<T, N, CPLX, false>(m, gg);
+        if (k == nullptr) {
+            set_error("no Welch kernel instance MODE %d, G %d for this plan (nfft=%lld)", m, gg, (long long)N);
+            return DSPB200_EUNSUPPORTED;
+        }
+        if (m >= 2 && p->d_window == nullptr) {           // MODE 2 / 3 stage the window table
+            set_error("Welch MODE %d needs a window", m);
+            return DSPB200_EUNSUPPORTED;
+        }
+        const size_t smem = welch_smem<T, N, CPLX>(m, p->n, p->hop, gg);
+        if (smem > p->smem_optin) {
+            set_error("Welch MODE %d, G %d needs %zu bytes of shared memory (limit %zu)", m, gg, smem, p->smem_optin);
+            return DSPB200_EUNSUPPORTED;
+        }
+        DSP_TRY(set_smem(k, smem));
+        int per_sm = 0;
+        DSP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, NT * gg, smem));
+        // (one resident wave of the single-signal kernel never has more virtual CTAs than `partial` has rows)
+        if (!batched && vctas == 0 && (int64_t)per_sm * gg * p->sm_count > p->nparts)
+            per_sm = (int)(p->nparts / ((int64_t)gg * p->sm_count));
+        if (per_sm < 1) {
+            set_error("Welch MODE %d, G %d does not fit an SM", m, gg);
+            return DSPB200_EUNSUPPORTED;
+        }
+        pinned[a].kern = k; pinned[a].smem = smem; pinned[a].g = gg; pinned[a].per_sm = per_sm; pinned[a].threads = NT * gg;
+        pinned[a].mode = m; pinned[a].vctas = vctas;
+    }
+    SpecPlanImpl::WelchCfg* cfg = batched ? p->welch_batch_cfg : p->welch_cfg;
+    cfg[0] = pinned[0];
+    cfg[1] = pinned[1];
+    return DSPB200_OK;
+}
+template <typename T> static int welch_pin_dispatch(SpecPlanImpl* p, bool batched, int mode, int g, int64_t vctas) {
+    switch (p->nfft) {
+#define X(NN)                                                                                               \
+    case NN:                                                                                                \
+        if constexpr (sizeof(T) == 8 && NN > 8192) break;                                                   \
+        else return p->cplx ? welch_pin<T, NN, true>(p, batched, mode, g, vctas)                            \
+                            : welch_pin<T, NN, false>(p, batched, mode, g, vctas);
         DSP_FUSED_SIZES(X)
 #undef X
     }
@@ -1787,6 +1893,40 @@ int dspb200_welch_finalize_dev(dspb200_spec_plan* plan, double r, void* out, voi
     DSP_REQUIRE(plan && out, "NULL argument");
     DSP_REQUIRE(r != 0.0, "r must be nonzero");
     return welch_finalize(&plan->impl, r, out, (cudaStream_t)stream);
+}
+
+// Testing aid: run one chosen fused Welch instance on a chosen number of virtual CTAs (the kernels have no grid-wide
+// synchronisation, so a grid larger than one resident wave is as correct as one wave)
+int dspb200_spec_plan_pin_welch(dspb200_spec_plan* plan, int batched, int mode, int groups, int64_t vctas) {
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    SpecPlanImpl* p = &plan->impl;
+    SpecPlanImpl::WelchCfg* cfg = batched ? p->welch_batch_cfg : p->welch_cfg;
+    if (mode < 0) {                                      // unpin: the next call selects as before
+        cfg[0] = SpecPlanImpl::WelchCfg{};
+        cfg[1] = SpecPlanImpl::WelchCfg{};
+        return DSPB200_OK;
+    }
+    if (!p->fused || groups < 1) {
+        set_error("no fused Welch kernel instance MODE %d, G %d for this plan", mode, groups);
+        return DSPB200_EUNSUPPORTED;
+    }
+    DSP_REQUIRE(vctas >= 0 && vctas % groups == 0, "vctas (%lld) must be a non-negative multiple of groups (%d)",
+                (long long)vctas, groups);
+    DSP_REQUIRE(batched || vctas <= p->nparts, "vctas (%lld) exceeds the plan's %d partial rows", (long long)vctas, p->nparts);
+    DSP_CUDA(cudaSetDevice(p->device));
+    return p->f64 ? welch_pin_dispatch<double>(p, batched != 0, mode, groups, vctas)
+                  : welch_pin_dispatch<float>(p, batched != 0, mode, groups, vctas);
+}
+
+int dspb200_spec_plan_welch_config(const dspb200_spec_plan* plan, int batched, int aligned, int* mode, int* groups,
+                                   int64_t* vctas) {
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    const SpecPlanImpl::WelchCfg& c = (batched ? plan->impl.welch_batch_cfg : plan->impl.welch_cfg)[aligned ? 1 : 0];
+    const bool ran = c.kern != nullptr && c.used > 0;
+    if (mode) *mode = ran ? c.mode : -1;
+    if (groups) *groups = ran ? c.g : 0;
+    if (vctas) *vctas = ran ? c.used : 0;
+    return DSPB200_OK;
 }
 
 int dspb200_welch_exec_dev(dspb200_spec_plan* plan, const void* s, int64_t len, double r, void* out, void* stream) {

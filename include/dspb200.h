@@ -210,6 +210,23 @@ DSPB200_API int dspb200_welch_begin_dev(dspb200_spec_plan* plan, void* stream);
 DSPB200_API int dspb200_welch_accumulate_dev(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t sample_offset,
                                  int64_t seg_begin, int64_t seg_end, void* stream);
 DSPB200_API int dspb200_welch_finalize_dev(dspb200_spec_plan* plan, double r, void* out, void* stream);
+/* Testing aid: pin the fused Welch launch configuration of `plan` (batched = 0: the single-signal kernel of the calls above,
+ * 1: the batched kernel of dspb200_welch_batch_exec(_dev)).  Each plan picks, per alignment class, one instance of
+ * MODE (0 direct loads, 1 TMA staging, 2 TMA + window in shared memory, 3 TMA + window in registers) x G (thread groups
+ * per CTA, 1..3) on its first call; pinning replaces that choice, so that a test can run every instance on the same data.
+ * A pinned TMA mode (1-3) applies to calls whose segments are 16-byte aligned; the others run MODE 0, G = 1.
+ * mode < 0 unpins (the next call selects as before).  vctas > 0 fixes the number of virtual CTAs (CTAs x G; the grid is
+ * vctas / groups, and need not fit one resident wave), 0 keeps the occupancy-derived grid; in the batched form it replaces
+ * the resident virtual-CTA count the channels are sliced for.  DSPB200_EUNSUPPORTED: not a fused plan, no such instance
+ * for the plan's (dtype, nfft), or its shared memory exceeds the opt-in limit for the plan's n and hop.
+ * DSPB200_EINVALID: vctas < 0 or not a multiple of groups, or more virtual CTAs than the plan has partial rows
+ * (single-signal form).  Pinning does not change what is computed, only which instance and grid compute it. */
+DSPB200_API int dspb200_spec_plan_pin_welch(dspb200_spec_plan* plan, int batched, int mode, int groups, int64_t vctas);
+/* The configuration the last fused Welch call of the given form and alignment class (0 unaligned, 1 aligned) used:
+ * mode, groups and virtual CTAs of its launch.  *groups = 0 (mode -1, vctas 0) when no such call has run since the plan
+ * was created or last pinned / unpinned. */
+DSPB200_API int dspb200_spec_plan_welch_config(const dspb200_spec_plan* plan, int batched, int aligned, int* mode, int* groups,
+                                               int64_t* vctas);
 /* welch_pgram(filt(b, x), config) as ONE host-pointer call (src/dspbase.jl:14-15 + src/periodograms.jl:702-759): x[n] on the
  * host (pinned memory lets the copies overlap), out[nout] on the host.  The stream goes through the GPU in chunks: the H2D copy
  * of chunk c+1 overlaps the overlap-save convolution of chunk c (os plan: taps b, dtype of x) and the Welch accumulation of
