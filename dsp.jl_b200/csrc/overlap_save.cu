@@ -527,24 +527,30 @@ __global__ void nd_copy_kernel(const E* __restrict__ src, Dims3 s, E* __restrict
     }
 }
 
-// _conv_td!, src/dspbase.jl:646-660, N-D: out[k] = sum over m of u[m] * v[k - m] (muladd), one output per thread
+// _conv_td!, src/dspbase.jl:646-660, N-D: out[k] = sum of u[m] * v[n] over m + n = k, one output per thread.  The reference
+// loops `for m in CartesianIndices(u), n in CartesianIndices(v)` when size(u,1) <= size(v,1), else with n outer: every
+// output sums its products in the column-major order of the outer array's index (dim 1 fastest), each step
+// muladd(u[m], v[n], acc).  The walk below is over that array (w), the other one (o) read at k - j.
 template <typename T, bool CPLX>
 __global__ void conv_direct_nd_kernel(const void* __restrict__ u_, Dims3 su, const void* __restrict__ v_, Dims3 sv,
                                       void* __restrict__ out_) {
     using E = typename os_elt<T, CPLX>::type;
-    const E* u = reinterpret_cast<const E*>(u_);
-    const E* v = reinterpret_cast<const E*>(v_);
+    const bool walk_u = su.n[0] <= sv.n[0];
+    const E* w = reinterpret_cast<const E*>(walk_u ? u_ : v_);
+    const E* o = reinterpret_cast<const E*>(walk_u ? v_ : u_);
+    const Dims3 sw = walk_u ? su : sv, so = walk_u ? sv : su;
     E* out = reinterpret_cast<E*>(out_);
     const int64_t o0 = su.n[0] + sv.n[0] - 1, o1 = su.n[1] + sv.n[1] - 1, o2 = su.n[2] + sv.n[2] - 1;
     const int64_t total = o0 * o1 * o2;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         const int64_t k0 = i % o0, k1 = (i / o0) % o1, k2 = i / (o0 * o1);
         T ar = T(0), ai = T(0);
-        for (int64_t m2 = max(k2 - (sv.n[2] - 1), (int64_t)0); m2 <= min(k2, su.n[2] - 1); ++m2)
-            for (int64_t m1 = max(k1 - (sv.n[1] - 1), (int64_t)0); m1 <= min(k1, su.n[1] - 1); ++m1)
-                for (int64_t m0 = max(k0 - (sv.n[0] - 1), (int64_t)0); m0 <= min(k0, su.n[0] - 1); ++m0) {
-                    const E a = u[m0 + su.n[0] * (m1 + su.n[1] * m2)];
-                    const E b = v[(k0 - m0) + sv.n[0] * ((k1 - m1) + sv.n[1] * (k2 - m2))];
+        for (int64_t m2 = max(k2 - (so.n[2] - 1), (int64_t)0); m2 <= min(k2, sw.n[2] - 1); ++m2)
+            for (int64_t m1 = max(k1 - (so.n[1] - 1), (int64_t)0); m1 <= min(k1, sw.n[1] - 1); ++m1)
+                for (int64_t m0 = max(k0 - (so.n[0] - 1), (int64_t)0); m0 <= min(k0, sw.n[0] - 1); ++m0) {
+                    const E p = w[m0 + sw.n[0] * (m1 + sw.n[1] * m2)];
+                    const E q = o[(k0 - m0) + so.n[0] * ((k1 - m1) + so.n[1] * (k2 - m2))];
+                    const E a = walk_u ? p : q, b = walk_u ? q : p;     // a = u[m], b = v[n]: muladd(a, b, acc)
                     if constexpr (CPLX) {
                         ar = fma(a.x, b.x, fma(-a.y, b.y, ar));
                         ai = fma(a.x, b.y, fma(a.y, b.x, ai));
@@ -647,29 +653,34 @@ __global__ void scale_cplx_kernel(cx<T>* __restrict__ X, int64_t n, T scale) {
         X[i] = cscale(X[i], scale);
 }
 
-// direct convolution, src/dspbase.jl:646-660: out[k] = sum_n large[n] * small[k-n], n ascending, muladd
+// direct convolution, src/dspbase.jl:646-660, 1-D.  The reference loops `for m in u, n in v` when length(u) <= length(v)
+// and `for n in v, m in u` otherwise; the first iterator is the outer one, so every output sums its products in ascending
+// index of the SHORTER array (u on a tie), each step muladd(u[m], v[n], acc): the walk below, one output per thread.
 template <typename T, bool CPLX>
-__global__ void conv_direct_kernel(const void* __restrict__ large_, int64_t nl, const void* __restrict__ small_,
-                                   int64_t ns, void* __restrict__ out_) {
+__global__ void conv_direct_kernel(const void* __restrict__ u_, int64_t nu, const void* __restrict__ v_, int64_t nv,
+                                   void* __restrict__ out_) {
     using E = typename os_elt<T, CPLX>::type;
-    const E* large = reinterpret_cast<const E*>(large_);
-    const E* small = reinterpret_cast<const E*>(small_);
+    const bool walk_u = nu <= nv;
+    const E* w = reinterpret_cast<const E*>(walk_u ? u_ : v_);          // the array whose index is the outer loop
+    const E* o = reinterpret_cast<const E*>(walk_u ? v_ : u_);
+    const int64_t nw = walk_u ? nu : nv, no = walk_u ? nv : nu;
     E* out = reinterpret_cast<E*>(out_);
-    const int64_t nout = nl + ns - 1;
+    const int64_t nout = nu + nv - 1;
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nout; k += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t lo = k - (ns - 1) > 0 ? k - (ns - 1) : 0;
-        const int64_t hi = k < nl - 1 ? k : nl - 1;
+        const int64_t lo = k - (no - 1) > 0 ? k - (no - 1) : 0;
+        const int64_t hi = k < nw - 1 ? k : nw - 1;
         if constexpr (CPLX) {
             cx<T> acc = mkc<T>(T(0), T(0));
-            for (int64_t n = lo; n <= hi; ++n) {
-                const cx<T> a = large[n], b = small[k - n];
+            for (int64_t j = lo; j <= hi; ++j) {
+                const cx<T> p = w[j], q = o[k - j];
+                const cx<T> a = walk_u ? p : q, b = walk_u ? q : p;      // a = u[m], b = v[n]: Base.muladd(a, b, acc)
                 acc.x = fma(a.x, b.x, fma(-a.y, b.y, acc.x));
                 acc.y = fma(a.x, b.y, fma(a.y, b.x, acc.y));
             }
             out[k] = acc;
         } else {
             T acc = T(0);
-            for (int64_t n = lo; n <= hi; ++n) acc = fma(large[n], small[k - n], acc);
+            for (int64_t j = lo; j <= hi; ++j) acc = fma(w[j], o[k - j], acc);
             out[k] = acc;
         }
     }
@@ -1507,15 +1518,12 @@ int dspb200_conv_direct_exec(int dtype, const void* u, int64_t nu, const void* v
         DSP_TRY(du.reserve((size_t)nu * esz)); DSP_TRY(dv.reserve((size_t)nv * esz)); DSP_TRY(dout.reserve((size_t)nout * esz));
         DSP_CUDA(cudaMemcpy(du.p, u, (size_t)nu * esz, cudaMemcpyHostToDevice));
         DSP_CUDA(cudaMemcpy(dv.p, v, (size_t)nv * esz, cudaMemcpyHostToDevice));
-        const void* large = nu >= nv ? du.p : dv.p;
-        const void* small = nu >= nv ? dv.p : du.p;
-        const int64_t nl = nu >= nv ? nu : nv, ns = nu >= nv ? nv : nu;
         const int threads = 128, g = grid_for(nout, threads);
         switch (dtype) {
-            case DSPB200_F32: conv_direct_kernel<float, false><<<g, threads>>>(large, nl, small, ns, dout.p); break;
-            case DSPB200_F64: conv_direct_kernel<double, false><<<g, threads>>>(large, nl, small, ns, dout.p); break;
-            case DSPB200_C32: conv_direct_kernel<float, true><<<g, threads>>>(large, nl, small, ns, dout.p); break;
-            default: conv_direct_kernel<double, true><<<g, threads>>>(large, nl, small, ns, dout.p); break;
+            case DSPB200_F32: conv_direct_kernel<float, false><<<g, threads>>>(du.p, nu, dv.p, nv, dout.p); break;
+            case DSPB200_F64: conv_direct_kernel<double, false><<<g, threads>>>(du.p, nu, dv.p, nv, dout.p); break;
+            case DSPB200_C32: conv_direct_kernel<float, true><<<g, threads>>>(du.p, nu, dv.p, nv, dout.p); break;
+            default: conv_direct_kernel<double, true><<<g, threads>>>(du.p, nu, dv.p, nv, dout.p); break;
         }
         DSP_LAUNCH_OK();
         DSP_CUDA(cudaMemcpy(out, dout.p, (size_t)nout * esz, cudaMemcpyDeviceToHost));

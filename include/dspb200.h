@@ -137,7 +137,9 @@ DSPB200_API int dspb200_os_plan_destroy(dspb200_os_plan* plan);
 /* conv(u, v; algorithm=:fft_simple) / _conv_kern_fft!: src/dspbase.jl:611-644 -- one FFT pair of size
  * nfft >= nu+nv-1 (the host passes nextfastfft(nu+nv-1), src/util.jl:134); out has nu+nv-1 samples. */
 DSPB200_API int dspb200_conv_fft_exec(int dtype, const void* u, int64_t nu, const void* v, int64_t nv, int64_t nfft, void* out);
-/* conv(u, v; algorithm=:direct) / _conv_td!: src/dspbase.jl:646-660 -- direct muladd convolution. */
+/* conv(u, v; algorithm=:direct) / _conv_td!: src/dspbase.jl:646-660 -- direct muladd convolution in the reference's order:
+ * each output sums its products in ascending index of the shorter of u and v (u when nu == nv), each one
+ * muladd(u[m], v[n], acc), so the result is bit-identical to the reference's loop on FMA hardware. */
 DSPB200_API int dspb200_conv_direct_exec(int dtype, const void* u, int64_t nu, const void* v, int64_t nv, void* out);
 
 /* conv(u, v; algorithm) for matrices and rank-3 arrays: src/dspbase.jl:611-660 (_conv_kern_fft!, _conv_td!), 709-757.

@@ -41,6 +41,69 @@ def fma_f32(a, b, c):
     return s.astype(np.float32)
 
 
+def _two_sum(a, b):
+    """s = a + b rounded, and the exact error e: s + e == a + b (Knuth's TwoSum, any order of magnitude)."""
+    s = a + b
+    bb = s - a
+    return s, (a - (s - bb)) + (b - bb)
+
+
+def _split(a):
+    """Veltkamp split: a == hi + lo exactly, hi and lo with at most 26 significant bits each."""
+    t = a * 134217729.0                         # 2^27 + 1
+    hi = t - (t - a)
+    return hi, a - hi
+
+
+def fma_f64(a, b, c):
+    """Exact Float64 fused multiply-add, vectorised: round_f64(a*b + c) with ONE rounding (Boldo & Melquiond, "Emulation
+    of FMA and correctly rounded sums: proved algorithms using rounding to odd", IEEE TC 2008).  a*b = uh + ul exactly
+    (Dekker's TwoProduct over a Veltkamp split); c + uh = th + tl exactly (TwoSum); v = tl + ul rounded to odd (the
+    rounded sum, moved one ulp towards the TwoSum error when it is inexact and even); result th + v rounded once.
+    Valid domain: finite a, b, c whose magnitudes, and that of a*b, are zero or within [2^-900, 2^900] -- so no split,
+    product or sum overflows and every low part is a normal number (no subnormal results)."""
+    a = np.asarray(a, dtype=np.float64)
+    b = np.asarray(b, dtype=np.float64)
+    c = np.asarray(c, dtype=np.float64)
+    uh = a * b
+    ah, al = _split(a)
+    bh, bl = _split(b)
+    ul = ((ah * bh - uh) + ah * bl + al * bh) + al * bl
+    th, tl = _two_sum(c, uh)
+    v, e = _two_sum(tl, ul)
+    odd = (v.view(np.int64) & 1) == 1
+    fix = (e != 0) & ~odd
+    if np.any(fix):
+        v = np.where(fix, np.nextafter(v, np.where(e > 0, np.inf, -np.inf)), v)
+    return th + v
+
+
+def cmuladd(z, w, x):
+    """Base.muladd(z::Complex, w::Complex, x::Complex) (base/complex.jl), vectorised, for complex64 / complex128:
+    Complex(muladd(zr, wr, -muladd(zi, wi, -xr)), muladd(zr, wi, muladd(zi, wr, xi))), each muladd an exact fma."""
+    z, w, x = np.asarray(z), np.asarray(w), np.asarray(x)
+    T = np.result_type(z, w, x)
+    f = fma_f32 if T == np.complex64 else fma_f64
+    re = f(z.real, w.real, -f(z.imag, w.imag, -x.real))
+    im = f(z.real, w.imag, f(z.imag, w.real, x.imag))
+    out = np.empty(np.broadcast(z, w, x).shape, dtype=T)
+    out.real, out.imag = re, im
+    return out
+
+
+def muladd(a, b, c, T):
+    """muladd(a, b, c) in eltype T as Julia evaluates it on FMA hardware: one exact fma for Float32 / Float64, Base.muladd
+    for Complex, plain a*b + c otherwise (integers: exact)."""
+    T = np.dtype(T)
+    if T == np.float32:
+        return fma_f32(a, b, c)
+    if T == np.float64:
+        return fma_f64(a, b, c)
+    if T in (np.complex64, np.complex128):
+        return cmuladd(np.asarray(a, dtype=T), np.asarray(b, dtype=T), np.asarray(c, dtype=T))
+    return (np.asarray(a, dtype=T) * np.asarray(b, dtype=T) + np.asarray(c, dtype=T)).astype(T)
+
+
 def filt_fir_literal(b, x):
     """Literal transposed direct-form-II loop, src/dspbase.jl:95-105 (one column).
 
@@ -259,20 +322,12 @@ def conv_kern_fft(u, v, f64=False):
 
 
 def conv_td(u, v):
-    """_conv_td!, src/dspbase.jl:646-660: direct O(MN) muladd convolution in promote_type."""
+    """_conv_td!, src/dspbase.jl:646-660: direct O(MN) muladd convolution in promote_type (exact for integers)."""
     u = np.asarray(u)
     v = np.asarray(v)
-    T = promote(u.dtype, v.dtype)
     if len(u) == 0 or len(v) == 0:
-        return np.zeros(max(len(u) + len(v) - 1, 0), dtype=T)
-    out = np.zeros(len(u) + len(v) - 1, dtype=T)
-    small, large = (u, v) if len(u) <= len(v) else (v, u)
-    # outer loop over the longer array's index? reference: if size(u,1) <= size(v,1): for m in u, n in v
-    # (column-major comprehension order: the LAST iterator varies slowest -> n outer, m inner).
-    # Either way each out[k] accumulates its products in ascending index of the outer array.
-    for n in range(len(large)):
-        out[n: n + len(small)] = (small.astype(T) * T.type(large[n]) + out[n: n + len(small)]).astype(T)
-    return out
+        return np.zeros(max(len(u) + len(v) - 1, 0), dtype=promote(u.dtype, v.dtype))
+    return conv_td_nd(u, v)
 
 
 def conv(u, v, algorithm="auto", f64=False):
@@ -340,10 +395,19 @@ def conv_td_nd(u, v):
     u = u.reshape(u.shape + (1,) * (nd - u.ndim))
     v = v.reshape(v.shape + (1,) * (nd - v.ndim))
     T = promote(u.dtype, v.dtype)
+    u, v = u.astype(T), v.astype(T)
     out = np.zeros(tuple(a + b - 1 for a, b in zip(u.shape, v.shape)), dtype=T)
-    for m in np.ndindex(*u.shape):
-        sl = tuple(slice(i, i + n) for i, n in zip(m, v.shape))
-        out[sl] += u[m] * v.astype(T)
+    # `for m in CartesianIndices(u), n in CartesianIndices(v)` when size(u,1) <= size(v,1), else n outer: the FIRST
+    # iterator is the outer loop, and CartesianIndices run in column-major order (dim 1 fastest).  One step per outer
+    # index adds that index's product to every output it reaches, so each output sums in the outer array's order.
+    if u.shape[0] <= v.shape[0]:
+        for m in (idx[::-1] for idx in np.ndindex(*u.shape[::-1])):
+            sl = tuple(slice(i, i + n) for i, n in zip(m, v.shape))
+            out[sl] = muladd(u[m], v, out[sl], T)
+    else:
+        for n in (idx[::-1] for idx in np.ndindex(*v.shape[::-1])):
+            sl = tuple(slice(i, i + k) for i, k in zip(n, u.shape))
+            out[sl] = muladd(u, v[n], out[sl], T)
     return out
 
 
