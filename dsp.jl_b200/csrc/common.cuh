@@ -6,6 +6,7 @@
 #include <stdio.h>
 #include <string.h>
 #include <stdarg.h>
+#include <initializer_list>
 #include <type_traits>
 
 #include "../../include/dspb200.h"
@@ -101,6 +102,75 @@ struct DevBuf {
     }
     void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 };
+
+// *d = a new device copy of h's bytes (plan constructors: taps, twiddle tables)
+int upload(void** d, const void* h, size_t bytes);
+// the fused FFT kernels' tables for nfft points (fft_core.cuh): last-pass twiddles, radix-16 and radix-256 tables
+int upload_fft_tables(int64_t nfft, bool f64, void** d_tw, void** d_t16, void** d_t256);
+
+// Creates *s, a non-blocking stream, unless it exists (the private streams of a plan's host-pointer entry points).
+inline int ensure_stream(cudaStream_t* s) {
+    if (!*s) DSP_CUDA(cudaStreamCreateWithFlags(s, cudaStreamNonBlocking));
+    return DSPB200_OK;
+}
+
+// Waits for `st` whether or not `rc` reports a failure, so that no error return leaves work that reads or writes the
+// caller's memory in flight.  Returns rc, or the synchronisation's error when rc is DSPB200_OK.
+int settle(cudaStream_t st, int rc);
+
+inline bool ranges_overlap(const void* a, size_t na, const void* b, size_t nb) {
+    return a && b && na && nb && (const char*)a < (const char*)b + nb && (const char*)b < (const char*)a + na;
+}
+
+// Host-pointer entry points are staging around their device-pointer twins: reserve the device buffers (16 bytes at least,
+// so that every staged pointer is valid), queue the host-to-device copies on `st`, run dev() (usually the twin, reading
+// the buffers' pointers), queue the device-to-host copies, and return once `st` is idle, on success and failure alike.
+struct HostIn { const void* src; size_t bytes; DevBuf* buf; };
+struct HostOut { void* dst; size_t bytes; DevBuf* buf; };
+template <class F>
+int run_staged(cudaStream_t st, std::initializer_list<HostIn> in, std::initializer_list<HostOut> out, F&& dev) {
+    auto queue = [&]() -> int {
+        for (const HostIn& h : in) DSP_TRY(h.buf->reserve(h.bytes ? h.bytes : 16));
+        for (const HostOut& h : out) DSP_TRY(h.buf->reserve(h.bytes ? h.bytes : 16));
+        for (const HostIn& h : in)
+            if (h.bytes) DSP_CUDA(cudaMemcpyAsync(h.buf->p, h.src, h.bytes, cudaMemcpyHostToDevice, st));
+        DSP_TRY(dev());
+        for (const HostOut& h : out)
+            if (h.bytes) DSP_CUDA(cudaMemcpyAsync(h.dst, h.buf->p, h.bytes, cudaMemcpyDeviceToHost, st));
+        return DSPB200_OK;
+    };
+    return settle(st, queue());
+}
+
+// Stateful FIR and overlap-save calls (DF2TFilter): ns state elements of esz bytes per column, in si_in (NULL: zero state)
+// and out to si_out (NULL: not wanted).
+// Device form: the size and overlap checks -- CTAs read the samples, halo and state behind other CTAs' outputs, so a
+// buffer that is written must not overlap one that is read (or the other written one) -- and, for nx == 0, the state
+// passed through on `st`.  The caller returns after this when nx == 0 or ncols == 0.
+int state_prologue_dev(const void* x, int64_t nx, int64_t ncols, const void* si_in, void* si_out, void* out, int64_t ns,
+                       size_t esz, cudaStream_t st);
+// Host form, for a plan P with `device`, `s_exec` and ensure_streams(P*): x and the state are staged apart (bx, bout, bsi,
+// bso), so out may be x and si_out may be si_in; nx == 0 passes the state through on the host.
+// dev(d_x, d_si_in, d_si_out, d_out) runs the device form on p->s_exec.
+template <class P, class F>
+int exec_state_host(P* p, const void* x, int64_t nx, int64_t ncols, const void* si_in, void* si_out, void* out, int64_t ns,
+                    size_t esz, DevBuf& bx, DevBuf& bout, DevBuf& bsi, DevBuf& bso, F&& dev) {
+    DSP_REQUIRE(nx >= 0 && ncols >= 0, "negative size");
+    if (ncols == 0) return DSPB200_OK;
+    DSP_REQUIRE(nx == 0 || (x && out), "NULL argument");
+    const size_t bytes = (size_t)(nx * ncols) * esz, sbytes = (size_t)(ns * ncols) * esz;
+    if (nx == 0) {
+        if (si_out && sbytes && si_out != si_in) {
+            if (si_in) memmove(si_out, si_in, sbytes);
+            else memset(si_out, 0, sbytes);
+        }
+        return DSPB200_OK;
+    }
+    DSP_TRY(ensure_streams(p));
+    return run_staged(p->s_exec, {{x, bytes, &bx}, {si_in, si_in ? sbytes : 0, &bsi}},
+                      {{out, bytes, &bout}, {si_out, si_out ? sbytes : 0, &bso}},
+                      [&] { return dev(bx.p, si_in ? bsi.p : nullptr, si_out ? bso.p : nullptr, bout.p); });
+}
 
 int device_sm_count();
 void count_launch(int n = 1);

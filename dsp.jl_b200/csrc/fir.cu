@@ -14,7 +14,6 @@
 // nx + j as si_out[j].  Filtering in chunks is therefore bit-identical to filtering in one call.
 #include "common.cuh"
 #include "fir_tile.cuh"
-#include <cstring>
 #include <new>
 
 namespace dspb200 {
@@ -103,9 +102,15 @@ struct FirPlanImpl {
     int64_t nb = 0;
     int device = 0;
     void* d_b = nullptr;
-    DevBuf in, out, state;
-    cudaStream_t stream = nullptr;
+    DevBuf in, out, si_in, si_out;
+    cudaStream_t s_exec = nullptr;
 };
+
+// makes the plan's device current and creates its stream on first use
+static int ensure_streams(FirPlanImpl* p) {
+    DSP_CUDA(cudaSetDevice(p->device));
+    return ensure_stream(&p->s_exec);
+}
 
 }  // namespace dspb200
 
@@ -128,10 +133,9 @@ int dspb200_fir_plan_create(dspb200_fir_plan** plan, int dtype, const void* b_ho
     DSP_REQUIRE(h != nullptr, "out of host memory");
     FirPlanImpl* p = &h->impl;
     p->dtype = dtype; p->nb = nb;
-    cudaError_t e = cudaGetDevice(&p->device);
-    if (e == cudaSuccess) e = cudaMalloc(&p->d_b, (size_t)nb * dtype_size(dtype));
-    if (e == cudaSuccess) e = cudaMemcpy(p->d_b, b_host, (size_t)nb * dtype_size(dtype), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { const int rc = cuda_fail(e, "tap upload", __FILE__, __LINE__); dspb200_fir_plan_destroy(h); return rc; }
+    const cudaError_t e = cudaGetDevice(&p->device);
+    const int rc = e != cudaSuccess ? cuda_fail(e, "cudaGetDevice", __FILE__, __LINE__) : upload(&p->d_b, b_host, (size_t)nb * dtype_size(dtype));
+    if (rc != DSPB200_OK) { dspb200_fir_plan_destroy(h); return rc; }
     *plan = h;
     return DSPB200_OK;
 }
@@ -150,30 +154,11 @@ int dspb200_fir_exec_state_dev(dspb200_fir_plan* plan, const void* x, int64_t nx
                                void* out, void* stream) {
     DSP_RANGE("dspb200_fir_exec_state_dev");
     DSP_REQUIRE(plan != nullptr, "plan is NULL");
-    DSP_REQUIRE(nx >= 0 && ncols >= 0, "negative size");
     FirPlanImpl* p = &plan->impl;
     const int64_t ns = p->nb - 1;
-    const size_t sbytes = (size_t)(ns * ncols) * dtype_size(p->dtype);
-    const size_t xbytes = (size_t)(nx * ncols) * dtype_size(p->dtype);
-    // Every CTA reads its samples and the tap halo of the tile before it, and the state, while other CTAs write: a buffer
-    // that is written must not overlap one that is read (or the other written one).
-    auto overlap = [](const void* a, size_t na, const void* b, size_t nb_) {
-        return a && b && na && nb_ && (const char*)a < (const char*)b + nb_ && (const char*)b < (const char*)a + na;
-    };
-    DSP_REQUIRE(!overlap(si_in, sbytes, si_out, sbytes), "si_in and si_out overlap");
-    DSP_REQUIRE(!overlap(x, xbytes, out, xbytes), "x and out overlap (filtering in place needs the host form)");
-    DSP_REQUIRE(!overlap(x, xbytes, si_out, sbytes) && !overlap(si_in, sbytes, out, xbytes) && !overlap(out, xbytes, si_out, sbytes),
-                "a state buffer overlaps x or out");
-    if (ncols == 0) return DSPB200_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    if (nx == 0) {                                                       // the state passes through unchanged
-        if (si_out && sbytes) {
-            if (si_in) DSP_CUDA(cudaMemcpyAsync(si_out, si_in, sbytes, cudaMemcpyDeviceToDevice, st));
-            else DSP_CUDA(cudaMemsetAsync(si_out, 0, sbytes, st));
-        }
-        return DSPB200_OK;
-    }
-    DSP_REQUIRE(x && out, "NULL argument");
+    DSP_TRY(state_prologue_dev(x, nx, ncols, si_in, si_out, out, ns, dtype_size(p->dtype), st));
+    if (nx == 0 || ncols == 0) return DSPB200_OK;
     if (ns == 0)                                                         // nb == 1: no state, out = x * b[1] (src/Filters/filt.jl:161-162)
         return fir_dispatch<false>(p->dtype, x, nx, nx, ncols, p->d_b, 1, out, nullptr, nullptr, st);
     return fir_dispatch<true>(p->dtype, x, nx, nx + ns, ncols, p->d_b, (int)p->nb, out, si_in, si_out, st);
@@ -183,34 +168,11 @@ int dspb200_fir_exec_state(dspb200_fir_plan* plan, const void* x, int64_t nx, in
                            void* out) {
     DSP_RANGE("dspb200_fir_exec_state");
     DSP_REQUIRE(plan != nullptr, "plan is NULL");
-    DSP_REQUIRE(nx >= 0 && ncols >= 0, "negative size");
-    if (ncols == 0) return DSPB200_OK;
-    DSP_REQUIRE(nx == 0 || (x && out), "NULL argument");
     FirPlanImpl* p = &plan->impl;
-    const size_t es = dtype_size(p->dtype);
-    const size_t bytes = (size_t)(nx * ncols) * es, sbytes = (size_t)((p->nb - 1) * ncols) * es;
-    if (nx == 0) {                                                       // the state passes through unchanged
-        if (si_out && sbytes && si_out != si_in) {
-            if (si_in) memmove(si_out, si_in, sbytes);
-            else memset(si_out, 0, sbytes);
-        }
-        return DSPB200_OK;
-    }
-    DSP_CUDA(cudaSetDevice(p->device));
-    if (!p->stream) DSP_CUDA(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
-    DSP_TRY(p->in.reserve(bytes));
-    DSP_TRY(p->out.reserve(bytes));
-    DSP_TRY(p->state.reserve(2 * sbytes + 16));                          // [si_in | si_out]: staged apart, so the host pointers may alias
-    char* d_si_in = (char*)p->state.p;
-    char* d_si_out = d_si_in + sbytes;
-    DSP_CUDA(cudaMemcpyAsync(p->in.p, x, bytes, cudaMemcpyHostToDevice, p->stream));
-    if (si_in && sbytes) DSP_CUDA(cudaMemcpyAsync(d_si_in, si_in, sbytes, cudaMemcpyHostToDevice, p->stream));
-    DSP_TRY(dspb200_fir_exec_state_dev(plan, p->in.p, nx, ncols, si_in ? d_si_in : nullptr, si_out ? d_si_out : nullptr, p->out.p,
-                                       p->stream));
-    DSP_CUDA(cudaMemcpyAsync(out, p->out.p, bytes, cudaMemcpyDeviceToHost, p->stream));
-    if (si_out && sbytes) DSP_CUDA(cudaMemcpyAsync(si_out, d_si_out, sbytes, cudaMemcpyDeviceToHost, p->stream));
-    DSP_CUDA(cudaStreamSynchronize(p->stream));
-    return DSPB200_OK;
+    return exec_state_host(p, x, nx, ncols, si_in, si_out, out, p->nb - 1, dtype_size(p->dtype), p->in, p->out, p->si_in,
+                           p->si_out, [&](const void* d_x, const void* d_si_in, void* d_si_out, void* d_out) {
+                               return dspb200_fir_exec_state_dev(plan, d_x, nx, ncols, d_si_in, d_si_out, d_out, p->s_exec);
+                           });
 }
 
 int dspb200_fir_exec(dspb200_fir_plan* plan, const void* x, int64_t nx, int64_t ncols, void* out) {
@@ -220,24 +182,18 @@ int dspb200_fir_exec(dspb200_fir_plan* plan, const void* x, int64_t nx, int64_t 
     if (nx == 0 || ncols == 0) return DSPB200_OK;
     DSP_REQUIRE(x && out, "NULL argument");
     FirPlanImpl* p = &plan->impl;
-    DSP_CUDA(cudaSetDevice(p->device));
-    if (!p->stream) DSP_CUDA(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
+    DSP_TRY(ensure_streams(p));
     const size_t bytes = (size_t)(nx * ncols) * dtype_size(p->dtype);
-    DSP_TRY(p->in.reserve(bytes));
-    DSP_TRY(p->out.reserve(bytes));
-    DSP_CUDA(cudaMemcpyAsync(p->in.p, x, bytes, cudaMemcpyHostToDevice, p->stream));
-    DSP_TRY(dspb200_fir_exec_dev(plan, p->in.p, nx, ncols, p->out.p, p->stream));
-    DSP_CUDA(cudaMemcpyAsync(out, p->out.p, bytes, cudaMemcpyDeviceToHost, p->stream));
-    DSP_CUDA(cudaStreamSynchronize(p->stream));
-    return DSPB200_OK;
+    return run_staged(p->s_exec, {{x, bytes, &p->in}}, {{out, bytes, &p->out}},
+                      [&] { return dspb200_fir_exec_dev(plan, p->in.p, nx, ncols, p->out.p, p->s_exec); });
 }
 
 int dspb200_fir_plan_destroy(dspb200_fir_plan* plan) {
     if (!plan) return DSPB200_OK;
     FirPlanImpl* p = &plan->impl;
     if (p->d_b) cudaFree(p->d_b);
-    p->in.release(); p->out.release(); p->state.release();
-    if (p->stream) cudaStreamDestroy(p->stream);
+    p->in.release(); p->out.release(); p->si_in.release(); p->si_out.release();
+    if (p->s_exec) cudaStreamDestroy(p->s_exec);
     delete plan;
     return DSPB200_OK;
 }

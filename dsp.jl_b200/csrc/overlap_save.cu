@@ -15,7 +15,6 @@
 #include <math.h>
 #include <stdlib.h>
 #include <new>
-#include <vector>
 
 namespace dspb200 {
 
@@ -896,17 +895,18 @@ static int64_t auto_nfft(int64_t nv, bool f64) {
     return n;
 }
 
+// makes the plan's device current and creates its streams and events on first use (s_exec last: it marks the set complete)
 static int ensure_streams(OsPlanImpl* p) {
+    DSP_CUDA(cudaSetDevice(p->device));
     if (p->s_exec) return DSPB200_OK;
-    DSP_CUDA(cudaStreamCreateWithFlags(&p->s_in, cudaStreamNonBlocking));
-    DSP_CUDA(cudaStreamCreateWithFlags(&p->s_exec, cudaStreamNonBlocking));
-    DSP_CUDA(cudaStreamCreateWithFlags(&p->s_out, cudaStreamNonBlocking));
+    DSP_TRY(ensure_stream(&p->s_in));
+    DSP_TRY(ensure_stream(&p->s_out));
     for (int i = 0; i < 2; ++i) {
-        DSP_CUDA(cudaEventCreateWithFlags(&p->ev_in[i], cudaEventDisableTiming));
-        DSP_CUDA(cudaEventCreateWithFlags(&p->ev_exec[i], cudaEventDisableTiming));
-        DSP_CUDA(cudaEventCreateWithFlags(&p->ev_out[i], cudaEventDisableTiming));
+        if (!p->ev_in[i]) DSP_CUDA(cudaEventCreateWithFlags(&p->ev_in[i], cudaEventDisableTiming));
+        if (!p->ev_exec[i]) DSP_CUDA(cudaEventCreateWithFlags(&p->ev_exec[i], cudaEventDisableTiming));
+        if (!p->ev_out[i]) DSP_CUDA(cudaEventCreateWithFlags(&p->ev_out[i], cudaEventDisableTiming));
     }
-    return DSPB200_OK;
+    return ensure_stream(&p->s_exec);
 }
 
 }  // namespace dspb200
@@ -1042,13 +1042,7 @@ static int conv_nd_dispatch(int dtype, int mode, int rank, const int64_t* usize,
 static int conv_nd_run_dev(int dtype, int mode, int rank, const int64_t* usize, const void* d_u, const int64_t* vsize, const void* d_v,
                            const int64_t* nffts, void* d_out, cudaStream_t st) {
     ConvenienceLock lock;
-    int rc = conv_nd_dispatch(dtype, mode, rank, usize, d_u, vsize, d_v, nffts, d_out, st);
-    if (rc == DSPB200_OK) {
-        cudaError_t e = cudaStreamSynchronize(st);
-        if (e != cudaSuccess) rc = cuda_fail(e, "cudaStreamSynchronize", __FILE__, __LINE__);
-    } else {
-        cudaStreamSynchronize(st);
-    }
+    const int rc = settle(st, conv_nd_dispatch(dtype, mode, rank, usize, d_u, vsize, d_v, nffts, d_out, st));
     scratch_trim((size_t)256 << 20);                             // plans and small buffers stay cached for the next call
     return rc;
 }
@@ -1061,16 +1055,8 @@ static int conv_nd_run_host(int dtype, int mode, int rank, const int64_t* usize,
     const size_t esz = dtype_size(dtype);
     ConvenienceLock lock;
     DevBuf &du = scratch_buf(0), &dv = scratch_buf(1), &dout = scratch_buf(2);
-    auto body = [&]() -> int {
-        DSP_TRY(du.reserve((size_t)nu * esz)); DSP_TRY(dv.reserve((size_t)nv * esz)); DSP_TRY(dout.reserve((size_t)no * esz));
-        DSP_CUDA(cudaMemcpy(du.p, u, (size_t)nu * esz, cudaMemcpyHostToDevice));
-        DSP_CUDA(cudaMemcpy(dv.p, v, (size_t)nv * esz, cudaMemcpyHostToDevice));
-        DSP_TRY(conv_nd_dispatch(dtype, mode, rank, usize, du.p, vsize, dv.p, nffts, dout.p, 0));
-        DSP_CUDA(cudaMemcpy(out, dout.p, (size_t)no * esz, cudaMemcpyDeviceToHost));
-        return DSPB200_OK;
-    };
-    const int rc = body();
-    if (rc != DSPB200_OK) cudaDeviceSynchronize();
+    const int rc = run_staged(0, {{u, (size_t)nu * esz, &du}, {v, (size_t)nv * esz, &dv}}, {{out, (size_t)no * esz, &dout}},
+                              [&] { return conv_nd_dispatch(dtype, mode, rank, usize, du.p, vsize, dv.p, nffts, dout.p, 0); });
     scratch_trim((size_t)256 << 20);
     return rc;
 }
@@ -1098,27 +1084,15 @@ int dspb200_os_plan_create(dspb200_os_plan** plan, int dtype, const void* v_host
     void* d_v = nullptr;
     do {
         cudaError_t e = cudaGetDevice(&p->device);
-        if (e == cudaSuccess) e = cudaMalloc(&d_v, (size_t)nv * esz);
-        if (e == cudaSuccess) e = cudaMemcpy(d_v, v_host, (size_t)nv * esz, cudaMemcpyHostToDevice);
-        if (e != cudaSuccess) { rc = cuda_fail(e, "filter upload", __FILE__, __LINE__); break; }
+        if (e != cudaSuccess) { rc = cuda_fail(e, "cudaGetDevice", __FILE__, __LINE__); break; }
+        rc = upload(&d_v, v_host, (size_t)nv * esz);
+        if (rc != DSPB200_OK) break;
         if (p->fused) {
-            std::vector<unsigned char> tw((size_t)(fft_tl_len_rt(p->nfft) + 1) * csz), t16((size_t)fft_tw16_len(p->nfft) * csz), t256((size_t)fft_tw256_len(p->nfft) * csz);
-            if (p->f64) {
-                fft_fill_tl<double>((cx<double>*)tw.data(), p->nfft);
-                fft_fill_tables<double>((cx<double>*)t16.data(), (cx<double>*)t256.data(), p->nfft);
-            } else {
-                fft_fill_tl<float>((cx<float>*)tw.data(), p->nfft);
-                fft_fill_tables<float>((cx<float>*)t16.data(), (cx<float>*)t256.data(), p->nfft);
-            }
             p->sm_count = device_sm_count();
-            e = cudaMalloc(&p->d_tw, tw.size());
-            if (e == cudaSuccess) e = cudaMemcpy(p->d_tw, tw.data(), tw.size(), cudaMemcpyHostToDevice);
-            if (e == cudaSuccess) e = cudaMalloc(&p->d_t16, t16.size());
-            if (e == cudaSuccess) e = cudaMemcpy(p->d_t16, t16.data(), t16.size(), cudaMemcpyHostToDevice);
-            if (e == cudaSuccess) e = cudaMalloc(&p->d_t256, t256.size());
-            if (e == cudaSuccess) e = cudaMemcpy(p->d_t256, t256.data(), t256.size(), cudaMemcpyHostToDevice);
-            if (e == cudaSuccess) e = cudaMalloc(&p->d_H, (size_t)p->nfft * csz);
-            if (e != cudaSuccess) { rc = cuda_fail(e, "twiddle upload", __FILE__, __LINE__); break; }
+            rc = upload_fft_tables(p->nfft, p->f64, &p->d_tw, &p->d_t16, &p->d_t256);
+            if (rc != DSPB200_OK) break;
+            e = cudaMalloc(&p->d_H, (size_t)p->nfft * csz);
+            if (e != cudaSuccess) { rc = cuda_fail(e, "cudaMalloc(H)", __FILE__, __LINE__); break; }
             rc = p->f64 ? os_filter_dispatch<double>(p, d_v) : os_filter_dispatch<float>(p, d_v);
         } else {
             p->nbins = p->cplx ? p->nfft : p->nfft / 2 + 1;
@@ -1208,30 +1182,11 @@ int dspb200_os_exec_state_dev(dspb200_os_plan* plan, const void* x, int64_t nx, 
                               void* out, void* stream) {
     DSP_RANGE("dspb200_os_exec_state_dev");
     DSP_REQUIRE(plan != nullptr, "plan is NULL");
-    DSP_REQUIRE(nx >= 0 && ncols >= 0, "negative size");
     OsPlanImpl* p = &plan->impl;
     const int64_t ns = p->nv - 1;
-    const size_t sbytes = (size_t)(ns * ncols) * dtype_size(p->dtype);
-    const size_t xbytes = (size_t)(nx * ncols) * dtype_size(p->dtype);
-    // a column's first unit reads si_in while its last units write si_out, and units read the samples behind their
-    // neighbours' outputs: a buffer that is written must not overlap one that is read (or the other written one)
-    auto overlap = [](const void* a, size_t na, const void* b, size_t nb_) {
-        return a && b && na && nb_ && (const char*)a < (const char*)b + nb_ && (const char*)b < (const char*)a + na;
-    };
-    DSP_REQUIRE(!overlap(si_in, sbytes, si_out, sbytes), "si_in and si_out overlap");
-    DSP_REQUIRE(!overlap(x, xbytes, out, xbytes), "x and out overlap (filtering in place needs the host form)");
-    DSP_REQUIRE(!overlap(x, xbytes, si_out, sbytes) && !overlap(si_in, sbytes, out, xbytes) && !overlap(out, xbytes, si_out, sbytes),
-                "a state buffer overlaps x or out");
-    if (ncols == 0) return DSPB200_OK;
     cudaStream_t st = (cudaStream_t)stream;
-    if (nx == 0) {                                                       // the state passes through unchanged
-        if (si_out && sbytes) {
-            if (si_in) DSP_CUDA(cudaMemcpyAsync(si_out, si_in, sbytes, cudaMemcpyDeviceToDevice, st));
-            else DSP_CUDA(cudaMemsetAsync(si_out, 0, sbytes, st));
-        }
-        return DSPB200_OK;
-    }
-    DSP_REQUIRE(x && out, "NULL argument");
+    DSP_TRY(state_prologue_dev(x, nx, ncols, si_in, si_out, out, ns, dtype_size(p->dtype), st));
+    if (nx == 0 || ncols == 0) return DSPB200_OK;
     if (p->fused && p->nfft < OS_STATE_MIN_NFFT) {
         set_error("no stateful overlap-save kernel for nfft=%lld: the stateful form takes plans with nfft = 0 (library choice)",
                   (long long)p->nfft);
@@ -1251,7 +1206,6 @@ int dspb200_os_exec(dspb200_os_plan* plan, const void* u, int64_t nu, int64_t nc
     if (nout == 0 || ncols == 0) return DSPB200_OK;
     DSP_REQUIRE(out != nullptr && (u != nullptr || nu == 0), "NULL argument");
     OsPlanImpl* p = &plan->impl;
-    DSP_CUDA(cudaSetDevice(p->device));
     DSP_TRY(ensure_streams(p));
     const size_t esz = dtype_size(p->dtype);
     const int64_t chunk_out = ((int64_t(32) << 20) / (int64_t)esz / p->L + 1) * p->L;   // ~32 MiB, whole blocks
@@ -1283,50 +1237,20 @@ int dspb200_os_exec(dspb200_os_plan* plan, const void* u, int64_t nu, int64_t nc
         DSP_CUDA(cudaStreamSynchronize(p->s_exec));
         return DSPB200_OK;
     }
-    const size_t in_bytes = (size_t)(nu * ncols) * esz, out_bytes = (size_t)(nout * ncols) * esz;
-    DSP_TRY(p->in[0].reserve(in_bytes ? in_bytes : 16));
-    DSP_TRY(p->out[0].reserve(out_bytes));
-    if (in_bytes) DSP_CUDA(cudaMemcpyAsync(p->in[0].p, u, in_bytes, cudaMemcpyHostToDevice, p->s_exec));
-    DSP_TRY(dspb200_os_exec_dev(plan, p->in[0].p, nu, ncols, p->out[0].p, nout, p->s_exec));
-    DSP_CUDA(cudaMemcpyAsync(out, p->out[0].p, out_bytes, cudaMemcpyDeviceToHost, p->s_exec));
-    DSP_CUDA(cudaStreamSynchronize(p->s_exec));
-    return DSPB200_OK;
+    return run_staged(p->s_exec, {{u, (size_t)(nu * ncols) * esz, &p->in[0]}}, {{out, (size_t)(nout * ncols) * esz, &p->out[0]}},
+                      [&] { return dspb200_os_exec_dev(plan, p->in[0].p, nu, ncols, p->out[0].p, nout, p->s_exec); });
 }
 
-// Host pointers: x and the state are staged through plan scratch (x in in[0], [si_in | si_out] in in[1]), so out may be x and
-// si_out may be si_in.
+// Host pointers: x and the state are staged apart (x in in[0], out in out[0], si_in in in[1], si_out in out[1]).
 int dspb200_os_exec_state(dspb200_os_plan* plan, const void* x, int64_t nx, int64_t ncols, const void* si_in, void* si_out,
                           void* out) {
     DSP_RANGE("dspb200_os_exec_state");
     DSP_REQUIRE(plan != nullptr, "plan is NULL");
-    DSP_REQUIRE(nx >= 0 && ncols >= 0, "negative size");
-    if (ncols == 0) return DSPB200_OK;
-    DSP_REQUIRE(nx == 0 || (x && out), "NULL argument");
     OsPlanImpl* p = &plan->impl;
-    const size_t es = dtype_size(p->dtype);
-    const size_t bytes = (size_t)(nx * ncols) * es, sbytes = (size_t)((p->nv - 1) * ncols) * es;
-    if (nx == 0) {                                                       // the state passes through unchanged
-        if (si_out && sbytes && si_out != si_in) {
-            if (si_in) memmove(si_out, si_in, sbytes);
-            else memset(si_out, 0, sbytes);
-        }
-        return DSPB200_OK;
-    }
-    DSP_CUDA(cudaSetDevice(p->device));
-    DSP_TRY(ensure_streams(p));
-    DSP_TRY(p->in[0].reserve(bytes));
-    DSP_TRY(p->out[0].reserve(bytes));
-    DSP_TRY(p->in[1].reserve(2 * sbytes + 16));
-    char* d_si_in = (char*)p->in[1].p;
-    char* d_si_out = d_si_in + sbytes;
-    DSP_CUDA(cudaMemcpyAsync(p->in[0].p, x, bytes, cudaMemcpyHostToDevice, p->s_exec));
-    if (si_in && sbytes) DSP_CUDA(cudaMemcpyAsync(d_si_in, si_in, sbytes, cudaMemcpyHostToDevice, p->s_exec));
-    DSP_TRY(dspb200_os_exec_state_dev(plan, p->in[0].p, nx, ncols, si_in ? d_si_in : nullptr, si_out ? d_si_out : nullptr,
-                                      p->out[0].p, p->s_exec));
-    DSP_CUDA(cudaMemcpyAsync(out, p->out[0].p, bytes, cudaMemcpyDeviceToHost, p->s_exec));
-    if (si_out && sbytes) DSP_CUDA(cudaMemcpyAsync(si_out, d_si_out, sbytes, cudaMemcpyDeviceToHost, p->s_exec));
-    DSP_CUDA(cudaStreamSynchronize(p->s_exec));
-    return DSPB200_OK;
+    return exec_state_host(p, x, nx, ncols, si_in, si_out, out, p->nv - 1, dtype_size(p->dtype), p->in[0], p->out[0], p->in[1],
+                           p->out[1], [&](const void* d_x, const void* d_si_in, void* d_si_out, void* d_out) {
+                               return dspb200_os_exec_state_dev(plan, d_x, nx, ncols, d_si_in, d_si_out, d_out, p->s_exec);
+                           });
 }
 
 int dspb200_os_plan_destroy(dspb200_os_plan* plan) {
@@ -1491,33 +1415,25 @@ int dspb200_hilbert_exec(int dtype, const void* x, int64_t n, int64_t ncols, voi
     DSP_RANGE("dspb200_hilbert_exec");
     DSP_REQUIRE(dtype == DSPB200_F32 || dtype == DSPB200_F64, "hilbert takes a real signal (dtype %d)", dtype);
     DSP_REQUIRE(x && out && n >= 1 && ncols >= 1, "empty or NULL input");
-    const size_t esz = dtype_size(dtype);
-    DevBuf dx, dout;
-    auto body = [&]() -> int {
-        DSP_TRY(dx.reserve((size_t)(n * ncols) * esz));
-        DSP_TRY(dout.reserve((size_t)(n * ncols) * 2 * esz));
-        DSP_CUDA(cudaMemcpy(dx.p, x, (size_t)(n * ncols) * esz, cudaMemcpyHostToDevice));
-        DSP_TRY(dspb200_hilbert_exec_dev(dtype, dx.p, n, ncols, dout.p, nullptr));
-        DSP_CUDA(cudaMemcpy(out, dout.p, (size_t)(n * ncols) * 2 * esz, cudaMemcpyDeviceToHost));
-        return DSPB200_OK;
-    };
-    const int rc = body();
-    dx.release(); dout.release();
+    const size_t bytes = (size_t)(n * ncols) * dtype_size(dtype);
+    ConvenienceLock lock;                                       // scratch arena (common.cuh)
+    DevBuf &dx = scratch_buf(0), &dout = scratch_buf(1);
+    const int rc = run_staged(0, {{x, bytes, &dx}}, {{out, 2 * bytes, &dout}},
+                              [&] { return dspb200_hilbert_exec_dev(dtype, dx.p, n, ncols, dout.p, nullptr); });
+    scratch_trim((size_t)256 << 20);
     return rc;
 }
 
-// _conv_td!, src/dspbase.jl:646-660 (host pointers)
+// _conv_td!, src/dspbase.jl:646-660 (host pointers, scratch arena)
 int dspb200_conv_direct_exec(int dtype, const void* u, int64_t nu, const void* v, int64_t nv, void* out) {
     DSP_RANGE("dspb200_conv_direct_exec");
     DSP_REQUIRE(dtype_valid(dtype), "invalid dtype %d", dtype);
     DSP_REQUIRE(u && v && out && nu >= 1 && nv >= 1, "empty or NULL input");
     const size_t esz = dtype_size(dtype);
     const int64_t nout = nu + nv - 1;
-    DevBuf du, dv, dout;
-    auto body = [&]() -> int {
-        DSP_TRY(du.reserve((size_t)nu * esz)); DSP_TRY(dv.reserve((size_t)nv * esz)); DSP_TRY(dout.reserve((size_t)nout * esz));
-        DSP_CUDA(cudaMemcpy(du.p, u, (size_t)nu * esz, cudaMemcpyHostToDevice));
-        DSP_CUDA(cudaMemcpy(dv.p, v, (size_t)nv * esz, cudaMemcpyHostToDevice));
+    ConvenienceLock lock;
+    DevBuf &du = scratch_buf(0), &dv = scratch_buf(1), &dout = scratch_buf(2);
+    auto launch = [&]() -> int {
         const int threads = 128, g = grid_for(nout, threads);
         switch (dtype) {
             case DSPB200_F32: conv_direct_kernel<float, false><<<g, threads>>>(du.p, nu, dv.p, nv, dout.p); break;
@@ -1526,11 +1442,10 @@ int dspb200_conv_direct_exec(int dtype, const void* u, int64_t nu, const void* v
             default: conv_direct_kernel<double, true><<<g, threads>>>(du.p, nu, dv.p, nv, dout.p); break;
         }
         DSP_LAUNCH_OK();
-        DSP_CUDA(cudaMemcpy(out, dout.p, (size_t)nout * esz, cudaMemcpyDeviceToHost));
         return DSPB200_OK;
     };
-    const int rc = body();
-    du.release(); dv.release(); dout.release();
+    const int rc = run_staged(0, {{u, (size_t)nu * esz, &du}, {v, (size_t)nv * esz, &dv}}, {{out, (size_t)nout * esz, &dout}}, launch);
+    scratch_trim((size_t)256 << 20);
     return rc;
 }
 

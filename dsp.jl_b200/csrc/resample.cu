@@ -650,8 +650,14 @@ struct RsPlanImpl {
     int64_t tpp8 = 0;
     size_t smem_optin = 0;
     DevBuf in, out;
-    cudaStream_t stream = nullptr;
+    cudaStream_t s_exec = nullptr;
 };
+
+// makes the plan's device current and creates its stream on first use
+static int ensure_streams(RsPlanImpl* p) {
+    DSP_CUDA(cudaSetDevice(p->device));
+    return ensure_stream(&p->s_exec);
+}
 
 struct RsArgs {
     const void* x; int64_t x_begin, nx_local, x_col_stride;
@@ -945,12 +951,10 @@ static int rs_stream_check(const RsPlanImpl* p, const void* hist_in, const void*
     const size_t hbytes = (size_t)(H * ncols) * sx, xbytes = (size_t)(nx * ncols) * sx;
     const size_t obytes = (ncols && nout) ? (size_t)((ncols - 1) * ldo + nout) * so : 0;
     // the kernels read the samples, history and outputs of other channels' threads: no written buffer may overlap another
-    auto overlap = [](const void* a, size_t na, const void* b, size_t nb_) {
-        return a && b && na && nb_ && (const char*)a < (const char*)b + nb_ && (const char*)b < (const char*)a + na;
-    };
-    DSP_REQUIRE(!overlap(hist_out, hbytes, hist_in, hbytes) && !overlap(hist_out, hbytes, x, xbytes) &&
-                !overlap(hist_out, hbytes, out, obytes), "hist_out overlaps hist_in, x or out");
-    DSP_REQUIRE(!overlap(out, obytes, x, xbytes) && !overlap(out, obytes, hist_in, hbytes), "out overlaps x or a history buffer");
+    DSP_REQUIRE(!ranges_overlap(hist_out, hbytes, hist_in, hbytes) && !ranges_overlap(hist_out, hbytes, x, xbytes) &&
+                !ranges_overlap(hist_out, hbytes, out, obytes), "hist_out overlaps hist_in, x or out");
+    DSP_REQUIRE(!ranges_overlap(out, obytes, x, xbytes) && !ranges_overlap(out, obytes, hist_in, hbytes),
+                "out overlaps x or a history buffer");
     if (nx == 0 || ncols == 0) return DSPB200_OK;
     DSP_REQUIRE(x != nullptr && (out != nullptr || nout == 0) && (hist_out != nullptr || H == 0), "NULL argument");
     return DSPB200_OK;
@@ -1003,11 +1007,10 @@ int dspb200_resample_plan_create(dspb200_resample_plan** plan, int dtype_x, int 
     int optin = 0;
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, p->device);
     p->smem_optin = (size_t)optin;
-    if (e == cudaSuccess) e = cudaMalloc(&p->d_pfb, bytes);
-    if (e == cudaSuccess) e = cudaMemcpy(p->d_pfb, o64 ? (const void*)bank64.data() : (const void*)bank32.data(), bytes, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMalloc(&p->d_pfb8, cnt8 * (o64 ? 8 : 4));
-    if (e == cudaSuccess) e = cudaMemcpy(p->d_pfb8, o64 ? (const void*)b8_64.data() : (const void*)b8_32.data(), cnt8 * (o64 ? 8 : 4), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { const int rc = cuda_fail(e, "tap upload", __FILE__, __LINE__); dspb200_resample_plan_destroy(hnd); return rc; }
+    int rc = e != cudaSuccess ? cuda_fail(e, "cudaGetDevice", __FILE__, __LINE__) : DSPB200_OK;
+    if (rc == DSPB200_OK) rc = upload(&p->d_pfb, o64 ? (const void*)bank64.data() : (const void*)bank32.data(), bytes);
+    if (rc == DSPB200_OK) rc = upload(&p->d_pfb8, o64 ? (const void*)b8_64.data() : (const void*)b8_32.data(), cnt8 * (o64 ? 8 : 4));
+    if (rc != DSPB200_OK) { dspb200_resample_plan_destroy(hnd); return rc; }
     p->h8_32 = b8_32;
     p->h8_64 = b8_64;
     *plan = hnd;
@@ -1055,17 +1058,10 @@ int dspb200_resample_exec(dspb200_resample_plan* plan, const void* x, int64_t nx
     if (nout == 0 || ncols == 0) return DSPB200_OK;
     DSP_REQUIRE(out != nullptr && (x != nullptr || nx == 0), "NULL argument");
     RsPlanImpl* p = &plan->impl;
-    DSP_CUDA(cudaSetDevice(p->device));
-    if (!p->stream) DSP_CUDA(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
-    const size_t in_bytes = (size_t)(nx * ncols) * dtype_size(p->dtype_x);
-    const size_t out_bytes = (size_t)(nout * ncols) * dtype_size(p->dtype_out);
-    DSP_TRY(p->in.reserve(in_bytes ? in_bytes : 16));
-    DSP_TRY(p->out.reserve(out_bytes));
-    if (in_bytes) DSP_CUDA(cudaMemcpyAsync(p->in.p, x, in_bytes, cudaMemcpyHostToDevice, p->stream));
-    DSP_TRY(dspb200_resample_exec_dev(plan, p->in.p, nx, ncols, n0, phi0, p->out.p, nout, p->stream));
-    DSP_CUDA(cudaMemcpyAsync(out, p->out.p, out_bytes, cudaMemcpyDeviceToHost, p->stream));
-    DSP_CUDA(cudaStreamSynchronize(p->stream));
-    return DSPB200_OK;
+    DSP_TRY(ensure_streams(p));
+    return run_staged(p->s_exec, {{x, (size_t)(nx * ncols) * dtype_size(p->dtype_x), &p->in}},
+                      {{out, (size_t)(nout * ncols) * dtype_size(p->dtype_out), &p->out}},
+                      [&] { return dspb200_resample_exec_dev(plan, p->in.p, nx, ncols, n0, phi0, p->out.p, nout, p->s_exec); });
 }
 
 // FIRArbitrary(h, rate, Nphi), src/Filters/stream_filt.jl:92-134: pfb = taps2pfb(h, Nphi), dpfb = taps2pfb([diff(h); 0], Nphi)
@@ -1093,10 +1089,8 @@ int dspb200_resample_arb_plan_create(dspb200_resample_plan** plan, int dtype_x, 
             }
             if (o64) bank64[(size_t)(phi * p->tpp + r)] = v; else bank32[(size_t)(phi * p->tpp + r)] = (float)v;
         }
-    const size_t bytes = cnt * (o64 ? 8 : 4);
-    cudaError_t e = cudaMalloc(&p->d_dpfb, bytes);
-    if (e == cudaSuccess) e = cudaMemcpy(p->d_dpfb, o64 ? (const void*)bank64.data() : (const void*)bank32.data(), bytes, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) { const int rc = cuda_fail(e, "derivative tap upload", __FILE__, __LINE__); dspb200_resample_plan_destroy(*plan); *plan = nullptr; return rc; }
+    const int rc = upload(&p->d_dpfb, o64 ? (const void*)bank64.data() : (const void*)bank32.data(), cnt * (o64 ? 8 : 4));
+    if (rc != DSPB200_OK) { dspb200_resample_plan_destroy(*plan); *plan = nullptr; return rc; }
     return DSPB200_OK;
 }
 
@@ -1128,17 +1122,12 @@ int dspb200_resample_arb_batch_exec(dspb200_resample_plan* plan, const void* x, 
     if (nout == 0 || ncols == 0) return DSPB200_OK;
     DSP_REQUIRE(out != nullptr && (x != nullptr || ldx == 0), "NULL argument");
     RsPlanImpl* p = &plan->impl;
-    DSP_CUDA(cudaSetDevice(p->device));
-    if (!p->stream) DSP_CUDA(cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking));
-    const size_t in_bytes = (size_t)(ldx * ncols) * dtype_size(p->dtype_x);
-    const size_t out_bytes = (size_t)(nout * ncols) * dtype_size(p->dtype_out);
-    DSP_TRY(p->in.reserve(in_bytes ? in_bytes : 16));
-    DSP_TRY(p->out.reserve(out_bytes));
-    if (in_bytes) DSP_CUDA(cudaMemcpyAsync(p->in.p, x, in_bytes, cudaMemcpyHostToDevice, p->stream));
-    DSP_TRY(dspb200_resample_arb_batch_exec_dev(plan, p->in.p, nx, ldx, ncols, n0, acc0, delta, p->out.p, nout, p->stream));
-    DSP_CUDA(cudaMemcpyAsync(out, p->out.p, out_bytes, cudaMemcpyDeviceToHost, p->stream));
-    DSP_CUDA(cudaStreamSynchronize(p->stream));
-    return DSPB200_OK;
+    DSP_TRY(ensure_streams(p));
+    return run_staged(p->s_exec, {{x, (size_t)(ldx * ncols) * dtype_size(p->dtype_x), &p->in}},
+                      {{out, (size_t)(nout * ncols) * dtype_size(p->dtype_out), &p->out}}, [&] {
+                          return dspb200_resample_arb_batch_exec_dev(plan, p->in.p, nx, ldx, ncols, n0, acc0, delta, p->out.p, nout,
+                                                                     p->s_exec);
+                      });
 }
 
 int dspb200_resample_arb_exec(dspb200_resample_plan* plan, const void* x, int64_t nx, int64_t n0, double acc0, double delta,
@@ -1204,7 +1193,7 @@ int dspb200_resample_plan_destroy(dspb200_resample_plan* plan) {
     if (p->d_pfb8) cudaFree(p->d_pfb8);
     if (p->d_dpfb) cudaFree(p->d_dpfb);
     p->in.release(); p->out.release();
-    if (p->stream) cudaStreamDestroy(p->stream);
+    if (p->s_exec) cudaStreamDestroy(p->s_exec);
     delete plan;
     return DSPB200_OK;
 }

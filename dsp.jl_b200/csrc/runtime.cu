@@ -1,5 +1,6 @@
 // dspb200 -- runtime entry points: errors, device selection, memory helpers.
 #include "common.cuh"
+#include "fft_core.cuh"
 #include <atomic>
 #include <cufft.h>
 #include <mutex>
@@ -31,6 +32,55 @@ int device_sm_count() {
 }
 
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
+
+int upload(void** d, const void* h, size_t bytes) {
+    DSP_CUDA(cudaMalloc(d, bytes));
+    DSP_CUDA(cudaMemcpy(*d, h, bytes, cudaMemcpyHostToDevice));
+    return DSPB200_OK;
+}
+
+template <typename T>
+static int upload_fft_tables(int64_t nfft, void** d_tw, void** d_t16, void** d_t256) {
+    std::vector<cx<T>> tw((size_t)fft_tl_len_rt(nfft) + 1), t16((size_t)fft_tw16_len(nfft)), t256((size_t)fft_tw256_len(nfft));
+    fft_fill_tl<T>(tw.data(), nfft);
+    fft_fill_tables<T>(t16.data(), t256.data(), nfft);
+    DSP_TRY(upload(d_tw, tw.data(), tw.size() * sizeof(cx<T>)));
+    DSP_TRY(upload(d_t16, t16.data(), t16.size() * sizeof(cx<T>)));
+    return upload(d_t256, t256.data(), t256.size() * sizeof(cx<T>));
+}
+int upload_fft_tables(int64_t nfft, bool f64, void** d_tw, void** d_t16, void** d_t256) {
+    return f64 ? upload_fft_tables<double>(nfft, d_tw, d_t16, d_t256) : upload_fft_tables<float>(nfft, d_tw, d_t16, d_t256);
+}
+
+int settle(cudaStream_t st, int rc) {
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (rc != DSPB200_OK) {
+        cudaGetLastError();                             // the first error is the one reported
+        return rc;
+    }
+    return e == cudaSuccess ? DSPB200_OK : cuda_fail(e, "cudaStreamSynchronize", __FILE__, __LINE__);
+}
+
+int state_prologue_dev(const void* x, int64_t nx, int64_t ncols, const void* si_in, void* si_out, void* out, int64_t ns,
+                       size_t esz, cudaStream_t st) {
+    DSP_REQUIRE(nx >= 0 && ncols >= 0, "negative size");
+    const size_t sbytes = (size_t)(ns * ncols) * esz, xbytes = (size_t)(nx * ncols) * esz;
+    DSP_REQUIRE(!ranges_overlap(si_in, sbytes, si_out, sbytes), "si_in and si_out overlap");
+    DSP_REQUIRE(!ranges_overlap(x, xbytes, out, xbytes), "x and out overlap (filtering in place needs the host form)");
+    DSP_REQUIRE(!ranges_overlap(x, xbytes, si_out, sbytes) && !ranges_overlap(si_in, sbytes, out, xbytes) &&
+                    !ranges_overlap(out, xbytes, si_out, sbytes),
+                "a state buffer overlaps x or out");
+    if (ncols == 0) return DSPB200_OK;
+    if (nx == 0) {                                                       // the state passes through unchanged
+        if (si_out && sbytes) {
+            if (si_in) DSP_CUDA(cudaMemcpyAsync(si_out, si_in, sbytes, cudaMemcpyDeviceToDevice, st));
+            else DSP_CUDA(cudaMemsetAsync(si_out, 0, sbytes, st));
+        }
+        return DSPB200_OK;
+    }
+    DSP_REQUIRE(x && out, "NULL argument");
+    return DSPB200_OK;
+}
 
 // ---- plan cache / scratch arena of the plan-less entry points
 static std::recursive_mutex g_conv_mutex;

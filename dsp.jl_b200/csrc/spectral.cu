@@ -1613,15 +1613,16 @@ static int64_t nsegments(const SpecPlanImpl* p, int64_t len) {
     return len >= p->n ? (len - p->n) / p->hop + 1 : 0;   // src/periodograms.jl:49-50
 }
 
+// makes the plan's device current and creates its streams and events on first use (s_exec last: it marks the set complete)
 static int ensure_streams(SpecPlanImpl* p) {
+    DSP_CUDA(cudaSetDevice(p->device));
     if (p->s_exec) return DSPB200_OK;
-    DSP_CUDA(cudaStreamCreateWithFlags(&p->s_copy, cudaStreamNonBlocking));
-    DSP_CUDA(cudaStreamCreateWithFlags(&p->s_exec, cudaStreamNonBlocking));
+    DSP_TRY(ensure_stream(&p->s_copy));
     for (int i = 0; i < 2; ++i) {
-        DSP_CUDA(cudaEventCreateWithFlags(&p->ev_in[i], cudaEventDisableTiming));
-        DSP_CUDA(cudaEventCreateWithFlags(&p->ev_done[i], cudaEventDisableTiming));
+        if (!p->ev_in[i]) DSP_CUDA(cudaEventCreateWithFlags(&p->ev_in[i], cudaEventDisableTiming));
+        if (!p->ev_done[i]) DSP_CUDA(cudaEventCreateWithFlags(&p->ev_done[i], cudaEventDisableTiming));
     }
-    return DSPB200_OK;
+    return ensure_stream(&p->s_exec);
 }
 
 }  // namespace dspb200
@@ -1634,12 +1635,12 @@ struct dspb200_spec_plan {
 
 static size_t win_row_bytes(const SpecPlanImpl* p) { return (size_t)p->n * sizeof(double); }   // float2 pairs are 8 B too
 
-// mt_cross_power_spectra! / mt_coherence!, src/multitaper.jl:553-603, 722-790 (host pointers)
+// mt_cross_power_spectra! / mt_coherence!, src/multitaper.jl:553-603, 722-790; queues the work on st (the caller waits for it:
+// the plan's scratch is reused by the next call)
 template <typename T>
 static int mt_cross_run(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int demean, int64_t f_lo, int64_t nf,
-                        int coherence, void* out, bool dev = false, cudaStream_t user_stream = 0) {
+                        int coherence, void* out, bool dev, cudaStream_t st) {
     SpecPlanImpl* p = &plan->impl;
-    cudaStream_t st = dev ? user_stream : p->s_exec;
     const int64_t n = p->n, cnt = nchan * nchan * nf;
     const size_t cs_bytes = (size_t)cnt * sizeof(cx<T>), out_bytes = coherence ? (size_t)cnt * sizeof(T) : cs_bytes;
     if (!dev) DSP_TRY(p->in[0].reserve((size_t)(n * nchan) * sizeof(T)));
@@ -1671,7 +1672,6 @@ static int mt_cross_run(dspb200_spec_plan* plan, const void* signal, int64_t nch
         DSP_LAUNCH_OK();
     }
     DSP_CUDA(cudaMemcpyAsync(out, res, out_bytes, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-    DSP_CUDA(cudaStreamSynchronize(st));                 // the plan's scratch is reused by the next call
     return DSPB200_OK;
 }
 
@@ -1691,7 +1691,7 @@ static int periodogram2_run(const void* s, int64_t n1, int64_t n2, int64_t f1, i
         DSP_TRY(dX.reserve((size_t)(h * f2) * sizeof(cx<T>)));
         if (!dev) {
             DSP_TRY(dout.reserve((size_t)nout * sizeof(T)));
-            DSP_CUDA(cudaMemcpy(ds.p, s, (size_t)(n1 * n2) * sizeof(T), cudaMemcpyHostToDevice));
+            DSP_CUDA(cudaMemcpyAsync(ds.p, s, (size_t)(n1 * n2) * sizeof(T), cudaMemcpyHostToDevice, st));
         }
         const T* src = dev ? (const T*)s : (const T*)ds.p;
         T* dst = dev ? (T*)out : (T*)dout.p;
@@ -1721,11 +1721,10 @@ static int periodogram2_run(const void* s, int64_t n1, int64_t n2, int64_t f1, i
             per2_radial_finish_kernel<T><<<(unsigned)cdiv(kmax, threads), threads, 0, st>>>(acc, wc, kmax, ptype == 2, dst);
             DSP_LAUNCH_OK();
         }
-        if (dev) DSP_CUDA(cudaStreamSynchronize(st));      // the cached plan and the arena are reused by the next call
-        else DSP_CUDA(cudaMemcpy(out, dout.p, (size_t)nout * sizeof(T), cudaMemcpyDeviceToHost));
+        if (!dev) DSP_CUDA(cudaMemcpyAsync(out, dout.p, (size_t)nout * sizeof(T), cudaMemcpyDeviceToHost, st));
         return DSPB200_OK;
     };
-    const int rc = body();
+    const int rc = settle(st, body());                          // the cached plan and the arena are reused by the next call
     scratch_trim((size_t)256 << 20);
     return rc;
 }
@@ -1757,48 +1756,32 @@ static int spec_plan_create_impl(dspb200_spec_plan** plan, int dtype, int64_t n,
         if (window_host) {
             const int64_t nw = n * (nrows < 1 ? 1 : nrows);
             p->ntapers = nrows;
-            cudaError_t e = cudaMalloc(&p->d_window, (size_t)nw * sizeof(double));
-            if (e == cudaSuccess) {
-                if (p->f64) {
-                    e = cudaMemcpy(p->d_window, window_host, (size_t)nw * sizeof(double), cudaMemcpyHostToDevice);
-                } else {                                   // hi/lo float pairs (same 8 bytes per value)
-                    std::vector<float> pairs((size_t)nw * 2);
-                    for (int64_t j = 0; j < nw; ++j) {
-                        const float hi = (float)window_host[j];
-                        pairs[2 * j] = hi;
-                        pairs[2 * j + 1] = (float)(window_host[j] - (double)hi);
-                    }
-                    e = cudaMemcpy(p->d_window, pairs.data(), pairs.size() * sizeof(float), cudaMemcpyHostToDevice);
+            if (p->f64) {
+                rc = upload(&p->d_window, window_host, (size_t)nw * sizeof(double));
+            } else {                                       // hi/lo float pairs (same 8 bytes per value)
+                std::vector<float> pairs((size_t)nw * 2);
+                for (int64_t j = 0; j < nw; ++j) {
+                    const float hi = (float)window_host[j];
+                    pairs[2 * j] = hi;
+                    pairs[2 * j + 1] = (float)(window_host[j] - (double)hi);
                 }
+                rc = upload(&p->d_window, pairs.data(), pairs.size() * sizeof(float));
             }
-            if (e != cudaSuccess) { rc = cuda_fail(e, "window upload", __FILE__, __LINE__); break; }
+            if (rc != DSPB200_OK) break;
         }
         if (p->fused) {
             const size_t csz = p->f64 ? 16 : 8;
-            std::vector<unsigned char> tw((size_t)(fft_tl_len_rt(nfft) + 1) * csz), t16((size_t)fft_tw16_len(nfft) * csz), t256((size_t)fft_tw256_len(nfft) * csz);
-            if (p->f64) {
-                fft_fill_tl<double>((cx<double>*)tw.data(), nfft);
-                fft_fill_tables<double>((cx<double>*)t16.data(), (cx<double>*)t256.data(), nfft);
-            } else {
-                fft_fill_tl<float>((cx<float>*)tw.data(), nfft);
-                fft_fill_tables<float>((cx<float>*)t16.data(), (cx<float>*)t256.data(), nfft);
-            }
-            cudaError_t e = cudaMalloc(&p->d_tw, tw.size());
-            if (e == cudaSuccess) e = cudaMemcpy(p->d_tw, tw.data(), tw.size(), cudaMemcpyHostToDevice);
-            if (e == cudaSuccess) e = cudaMalloc(&p->d_t16, t16.size());
-            if (e == cudaSuccess) e = cudaMemcpy(p->d_t16, t16.data(), t16.size(), cudaMemcpyHostToDevice);
-            if (e == cudaSuccess) e = cudaMalloc(&p->d_t256, t256.size());
-            if (e == cudaSuccess) e = cudaMemcpy(p->d_t256, t256.data(), t256.size(), cudaMemcpyHostToDevice);
-            if (e == cudaSuccess && !p->f64 && nfft == 1024) {                 // table of the warp-per-unit STFT kernel
+            rc = upload_fft_tables(nfft, p->f64, &p->d_tw, &p->d_t16, &p->d_t256);
+            if (rc == DSPB200_OK && !p->f64 && nfft == 1024) {                 // table of the warp-per-unit STFT kernel
                 std::vector<cx<float>> t32(w1k::T32_LEN);
                 w1k::fill_t32(t32.data());
-                e = cudaMalloc(&p->d_t32, t32.size() * sizeof(cx<float>));
-                if (e == cudaSuccess) e = cudaMemcpy(p->d_t32, t32.data(), t32.size() * sizeof(cx<float>), cudaMemcpyHostToDevice);
+                rc = upload(&p->d_t32, t32.data(), t32.size() * sizeof(cx<float>));
             }
+            if (rc != DSPB200_OK) break;
             int optin = 0;
-            if (e == cudaSuccess) e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, p->device);
+            const cudaError_t e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, p->device);
+            if (e != cudaSuccess) { rc = cuda_fail(e, "cudaDeviceGetAttribute", __FILE__, __LINE__); break; }
             p->smem_optin = (size_t)optin;
-            if (e != cudaSuccess) { rc = cuda_fail(e, "twiddle upload", __FILE__, __LINE__); break; }
             // persistent Welch grid: CTAs per SM bounded by shared memory (228 KB/SM on H100) and 2048 threads
             // (data + tables + TMA staging for 50 % overlap) per CTA
             const size_t smem = (size_t)(p->f64 ? padded_len<double>((int)nfft) : padded_len<float>((int)nfft)) * csz + (size_t)(fft_tw16_len(nfft) + fft_tw256_len(nfft)) * csz +
@@ -1970,21 +1953,12 @@ int dspb200_welch_batch_exec(dspb200_spec_plan* plan, const void* s, int64_t len
     SpecPlanImpl* p = &plan->impl;
     if (nchan == 0) return DSPB200_OK;
     DSP_REQUIRE(out != nullptr, "out is NULL");
-    DSP_CUDA(cudaSetDevice(p->device));
+    const bool any = nsegments(p, len) > 0;                // otherwise out is zeroed and s is not read
+    DSP_REQUIRE(!any || s != nullptr, "s is NULL");
     DSP_TRY(ensure_streams(p));
-    const size_t esz = dtype_size(p->dtype);
-    const size_t out_bytes = (size_t)(p->nout * nchan) * (p->f64 ? 8 : 4);
-    const bool any = nsegments(p, len) > 0;
-    if (any) {
-        DSP_REQUIRE(s != nullptr, "s is NULL");
-        DSP_TRY(p->in[0].reserve((size_t)(len * nchan) * esz));
-    }
-    DSP_TRY(p->out.reserve(out_bytes));
-    if (any) DSP_CUDA(cudaMemcpyAsync(p->in[0].p, s, (size_t)(len * nchan) * esz, cudaMemcpyHostToDevice, p->s_exec));
-    DSP_TRY(dspb200_welch_batch_exec_dev(plan, any ? p->in[0].p : nullptr, len, nchan, r, p->out.p, p->s_exec));
-    DSP_CUDA(cudaMemcpyAsync(out, p->out.p, out_bytes, cudaMemcpyDeviceToHost, p->s_exec));
-    DSP_CUDA(cudaStreamSynchronize(p->s_exec));
-    return DSPB200_OK;
+    const size_t in_bytes = any ? (size_t)(len * nchan) * dtype_size(p->dtype) : 0;
+    return run_staged(p->s_exec, {{s, in_bytes, &p->in[0]}}, {{out, (size_t)(p->nout * nchan) * (p->f64 ? 8 : 4), &p->out}},
+                      [&] { return dspb200_welch_batch_exec_dev(plan, p->in[0].p, len, nchan, r, p->out.p, p->s_exec); });
 }
 
 // Host-pointer Welch: the signal is streamed through two device buffers in segment-aligned chunks so the
@@ -1994,7 +1968,6 @@ int dspb200_welch_exec(dspb200_spec_plan* plan, const void* s, int64_t len, doub
     DSP_REQUIRE(plan && out, "NULL argument");
     DSP_REQUIRE(r != 0.0, "r must be nonzero");
     SpecPlanImpl* p = &plan->impl;
-    DSP_CUDA(cudaSetDevice(p->device));
     DSP_TRY(ensure_streams(p));
     const size_t esz = dtype_size(p->dtype);
     const int64_t k = nsegments(p, len);
@@ -2037,28 +2010,23 @@ int dspb200_arraysplit_exec(dspb200_spec_plan* plan, const void* s, int64_t len,
     DSP_RANGE("dspb200_arraysplit_exec");
     DSP_REQUIRE(plan != nullptr, "plan is NULL");
     SpecPlanImpl* p = &plan->impl;
-    DSP_CUDA(cudaSetDevice(p->device));
-    DSP_TRY(ensure_streams(p));
     const int64_t k = nsegments(p, len);
     if (k == 0) return DSPB200_OK;
     DSP_REQUIRE(s && out, "NULL argument");
+    DSP_TRY(ensure_streams(p));
     const size_t esz = dtype_size(p->dtype);
-    const size_t in_bytes = (size_t)len * esz, out_bytes = (size_t)(k * p->nfft) * esz;
-    DSP_TRY(p->in[0].reserve(in_bytes));
-    DSP_TRY(p->out.reserve(out_bytes));
-    DSP_CUDA(cudaMemcpyAsync(p->in[0].p, s, in_bytes, cudaMemcpyHostToDevice, p->s_exec));
-    const int64_t total = k * p->nfft;
-    const int threads = 256;
-    const int grid = (int)(cdiv(total, threads) < 65535 * 8 ? cdiv(total, threads) : 65535 * 8);
+    return run_staged(p->s_exec, {{s, (size_t)len * esz, &p->in[0]}}, {{out, (size_t)(k * p->nfft) * esz, &p->out}}, [&]() -> int {
+        const int64_t total = k * p->nfft;
+        const int threads = 256;
+        const int grid = (int)(cdiv(total, threads) < 65535 * 8 ? cdiv(total, threads) : 65535 * 8);
 #define SEGK(T_, C_) seg_window_kernel<T_, C_><<<grid, threads, 0, p->s_exec>>>(p->in[0].p, 0, p->hop, p->n, p->nfft, k, k, \
         reinterpret_cast<const typename win_t<T_>::type*>(p->d_window), p->out.p)
-    if (p->f64) { if (p->cplx) SEGK(double, true); else SEGK(double, false); }
-    else { if (p->cplx) SEGK(float, true); else SEGK(float, false); }
+        if (p->f64) { if (p->cplx) SEGK(double, true); else SEGK(double, false); }
+        else { if (p->cplx) SEGK(float, true); else SEGK(float, false); }
 #undef SEGK
-    DSP_LAUNCH_OK();
-    DSP_CUDA(cudaMemcpyAsync(out, p->out.p, out_bytes, cudaMemcpyDeviceToHost, p->s_exec));
-    DSP_CUDA(cudaStreamSynchronize(p->s_exec));
-    return DSPB200_OK;
+        DSP_LAUNCH_OK();
+        return DSPB200_OK;
+    });
 }
 
 int dspb200_stft_exec_dev(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, double r, int psd_only,
@@ -2086,45 +2054,31 @@ int dspb200_stft_exec(dspb200_spec_plan* plan, const void* s, int64_t len, int64
     DSP_RANGE("dspb200_stft_exec");
     DSP_REQUIRE(plan != nullptr, "plan is NULL");
     SpecPlanImpl* p = &plan->impl;
-    DSP_CUDA(cudaSetDevice(p->device));
-    DSP_TRY(ensure_streams(p));
     const int64_t k = nsegments(p, len);
     if (k == 0 || nchan == 0) return DSPB200_OK;
     DSP_REQUIRE(s && out, "NULL argument");
-    const size_t esz = dtype_size(p->dtype);
-    const size_t in_bytes = (size_t)len * nchan * esz;
+    DSP_TRY(ensure_streams(p));
     const size_t oel = psd_only ? (p->f64 ? 8 : 4) : (p->f64 ? 16 : 8);
-    const size_t out_bytes = (size_t)p->nout * k * nchan * oel;
-    DSP_TRY(p->in[0].reserve(in_bytes));
-    DSP_TRY(p->out.reserve(out_bytes));
-    DSP_CUDA(cudaMemcpyAsync(p->in[0].p, s, in_bytes, cudaMemcpyHostToDevice, p->s_exec));
-    DSP_TRY(dspb200_stft_exec_dev(plan, p->in[0].p, len, nchan, r, psd_only, p->out.p, p->s_exec));
-    DSP_CUDA(cudaMemcpyAsync(out, p->out.p, out_bytes, cudaMemcpyDeviceToHost, p->s_exec));
-    DSP_CUDA(cudaStreamSynchronize(p->s_exec));
-    return DSPB200_OK;
+    return run_staged(p->s_exec, {{s, (size_t)len * nchan * dtype_size(p->dtype), &p->in[0]}}, {{out, (size_t)p->nout * k * nchan * oel, &p->out}},
+                      [&] { return dspb200_stft_exec_dev(plan, p->in[0].p, len, nchan, r, psd_only, p->out.p, p->s_exec); });
 }
 
 // Multitaper (SURVEY.md 8f rank 1; src/multitaper.jl:117-242, 262-404).  The plan's window holds `ntapers` rows of n
 // samples, each PRE-SCALED by 1/sqrt(r_t) (r_t = fs * sum|w_t|^2 / weight_t, :135-139), so that
 //   mt_pgram       = sum_t fft2pow!(FFT(w_t .* s), 1)         (one Welch-style accumulation per taper into one spectrum)
 //   mt_spectrogram = sum_t spectrogram(s; window = w_t, r = 1) (one STFT launch per taper + an accumulate kernel)
-static int mt_pgram_entry(dspb200_spec_plan* plan, const void* s, int64_t len, void* out, bool dev, cudaStream_t user_stream) {
+static int mt_pgram_check(dspb200_spec_plan* plan, const void* s, int64_t len, void* out) {
     DSP_REQUIRE(plan && s && out, "NULL argument");
+    DSP_REQUIRE(plan->impl.ntapers >= 1, "not a multitaper plan");
+    DSP_REQUIRE(len == plan->impl.n, "Expected `signal` to be of length `config.n_samples`");    // DimensionMismatch :226
+    return DSPB200_OK;
+}
+int dspb200_mt_pgram_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t len, void* d_out, void* stream) {
+    DSP_RANGE("dspb200_mt_pgram_exec_dev");
+    DSP_TRY(mt_pgram_check(plan, d_s, len, d_out));
     SpecPlanImpl* p = &plan->impl;
-    DSP_REQUIRE(p->ntapers >= 1, "not a multitaper plan");
-    DSP_REQUIRE(len == p->n, "Expected `signal` to be of length `config.n_samples`");          // DimensionMismatch :226
     DSP_CUDA(cudaSetDevice(p->device));
-    DSP_TRY(ensure_streams(p));
-    cudaStream_t st = dev ? user_stream : p->s_exec;
-    const size_t esz = dtype_size(p->dtype);
-    const size_t out_bytes = (size_t)p->nout * (p->f64 ? 8 : 4);
-    const void* d_s = s;
-    if (!dev) {
-        DSP_TRY(p->in[0].reserve((size_t)len * esz));
-        DSP_TRY(p->out.reserve(out_bytes));
-        DSP_CUDA(cudaMemcpyAsync(p->in[0].p, s, (size_t)len * esz, cudaMemcpyHostToDevice, st));
-        d_s = p->in[0].p;
-    }
+    cudaStream_t st = (cudaStream_t)stream;
     DSP_TRY(welch_begin(p, st));
     void* const base = p->d_window;
     int rc = DSPB200_OK;
@@ -2134,41 +2088,31 @@ static int mt_pgram_entry(dspb200_spec_plan* plan, const void* s, int64_t len, v
     }
     p->d_window = base;
     DSP_TRY(rc);
-    DSP_TRY(welch_finalize(p, 1.0, dev ? out : p->out.p, st));
-    if (!dev) DSP_CUDA(cudaMemcpyAsync(out, p->out.p, out_bytes, cudaMemcpyDeviceToHost, st));
+    DSP_TRY(welch_finalize(p, 1.0, d_out, st));
     DSP_CUDA(cudaStreamSynchronize(st));
     return DSPB200_OK;
 }
 int dspb200_mt_pgram_exec(dspb200_spec_plan* plan, const void* s, int64_t len, void* out) {
     DSP_RANGE("dspb200_mt_pgram_exec");
-    return mt_pgram_entry(plan, s, len, out, false, 0);
-}
-int dspb200_mt_pgram_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t len, void* d_out, void* stream) {
-    DSP_RANGE("dspb200_mt_pgram_exec_dev");
-    return mt_pgram_entry(plan, d_s, len, d_out, true, (cudaStream_t)stream);
+    DSP_TRY(mt_pgram_check(plan, s, len, out));
+    SpecPlanImpl* p = &plan->impl;
+    DSP_TRY(ensure_streams(p));
+    return run_staged(p->s_exec, {{s, (size_t)len * dtype_size(p->dtype), &p->in[0]}}, {{out, (size_t)p->nout * (p->f64 ? 8 : 4), &p->out}},
+                      [&] { return dspb200_mt_pgram_exec_dev(plan, p->in[0].p, len, p->out.p, p->s_exec); });
 }
 
-static int mt_spectrogram_entry(dspb200_spec_plan* plan, const void* s, int64_t len, void* out, bool dev, cudaStream_t user_stream) {
+int dspb200_mt_spectrogram_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t len, void* d_out, void* stream) {
+    DSP_RANGE("dspb200_mt_spectrogram_exec_dev");
     DSP_REQUIRE(plan != nullptr, "plan is NULL");
     SpecPlanImpl* p = &plan->impl;
     DSP_REQUIRE(p->ntapers >= 1, "not a multitaper plan");
     DSP_CUDA(cudaSetDevice(p->device));
-    DSP_TRY(ensure_streams(p));
     const int64_t k = nsegments(p, len);
     if (k == 0) return DSPB200_OK;
-    DSP_REQUIRE(s && out, "NULL argument");
-    cudaStream_t st = dev ? user_stream : p->s_exec;
-    const size_t esz = dtype_size(p->dtype), oel = p->f64 ? 8 : 4;
+    DSP_REQUIRE(d_s && d_out, "NULL argument");
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t oel = p->f64 ? 8 : 4;
     const int64_t cnt = p->nout * k;
-    const void* d_s = s;
-    void* d_out = out;
-    if (!dev) {
-        DSP_TRY(p->in[0].reserve((size_t)len * esz));
-        DSP_TRY(p->out.reserve((size_t)cnt * oel));
-        DSP_CUDA(cudaMemcpyAsync(p->in[0].p, s, (size_t)len * esz, cudaMemcpyHostToDevice, st));
-        d_s = p->in[0].p;
-        d_out = p->out.p;
-    }
     if (!p->fused) DSP_TRY(p->tmp.reserve((size_t)cnt * oel));
     void* const base = p->d_window;
     int rc = DSPB200_OK;
@@ -2189,17 +2133,20 @@ static int mt_spectrogram_entry(dspb200_spec_plan* plan, const void* s, int64_t 
     }
     p->d_window = base;
     DSP_TRY(rc);
-    if (!dev) DSP_CUDA(cudaMemcpyAsync(out, p->out.p, (size_t)cnt * oel, cudaMemcpyDeviceToHost, st));
     DSP_CUDA(cudaStreamSynchronize(st));
     return DSPB200_OK;
 }
 int dspb200_mt_spectrogram_exec(dspb200_spec_plan* plan, const void* s, int64_t len, void* out) {
     DSP_RANGE("dspb200_mt_spectrogram_exec");
-    return mt_spectrogram_entry(plan, s, len, out, false, 0);
-}
-int dspb200_mt_spectrogram_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t len, void* d_out, void* stream) {
-    DSP_RANGE("dspb200_mt_spectrogram_exec_dev");
-    return mt_spectrogram_entry(plan, d_s, len, d_out, true, (cudaStream_t)stream);
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    SpecPlanImpl* p = &plan->impl;
+    DSP_REQUIRE(p->ntapers >= 1, "not a multitaper plan");
+    const int64_t k = nsegments(p, len);
+    if (k == 0) return DSPB200_OK;
+    DSP_REQUIRE(s && out, "NULL argument");
+    DSP_TRY(ensure_streams(p));
+    return run_staged(p->s_exec, {{s, (size_t)len * dtype_size(p->dtype), &p->in[0]}}, {{out, (size_t)(p->nout * k) * (p->f64 ? 8 : 4), &p->out}},
+                      [&] { return dspb200_mt_spectrogram_exec_dev(plan, p->in[0].p, len, p->out.p, p->s_exec); });
 }
 
 static int mt_cross_entry(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int demean, int64_t f_lo, int64_t nf,
@@ -2213,10 +2160,10 @@ static int mt_cross_entry(dspb200_spec_plan* plan, const void* signal, int64_t n
     DSP_REQUIRE(f_lo >= 0 && nf >= 0 && f_lo + nf <= p->nout, "frequency range outside the spectrum");
     if (nf == 0) return DSPB200_OK;
     DSP_REQUIRE(signal && out, "NULL argument");
-    DSP_CUDA(cudaSetDevice(p->device));
     DSP_TRY(ensure_streams(p));
-    return p->f64 ? mt_cross_run<double>(plan, signal, nchan, demean, f_lo, nf, coherence, out, dev, st)
-                  : mt_cross_run<float>(plan, signal, nchan, demean, f_lo, nf, coherence, out, dev, st);
+    if (!dev) st = p->s_exec;
+    return settle(st, p->f64 ? mt_cross_run<double>(plan, signal, nchan, demean, f_lo, nf, coherence, out, dev, st)
+                             : mt_cross_run<float>(plan, signal, nchan, demean, f_lo, nf, coherence, out, dev, st));
 }
 int dspb200_mt_cross_spectra_exec(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int demean, int64_t f_lo,
                                   int64_t nf, int coherence, void* out) {

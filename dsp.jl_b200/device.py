@@ -78,6 +78,11 @@ class DeviceArray:
         b = max(a, b)
         return DeviceArray((b - a,), self.dtype, _base=self, _ptr=self.ptr + a * self.dtype.itemsize)
 
+    def overlaps(self, other):
+        """True when `other` (a DeviceArray, or None) shares at least one byte of device memory with this array."""
+        return (other is not None and self.nbytes > 0 and other.nbytes > 0 and self.ptr < other.ptr + other.nbytes
+                and other.ptr < self.ptr + self.nbytes)
+
     def to_host(self, out=None):
         """Copy back to a (Fortran-ordered for 2-D) numpy array."""
         if out is None:

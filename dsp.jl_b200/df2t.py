@@ -241,12 +241,8 @@ class DF2TFilter:
         if x.dtype != S:
             raise ArgumentError(f"device chunks must have the state's eltype {S} (got {x.dtype})")
         cur, nxt = self._si
-
-        def overlap(a, b):
-            return a.nbytes and b.nbytes and a.ptr < b.ptr + b.nbytes and b.ptr < a.ptr + a.nbytes
-
         # the kernel's CTAs read the samples and state behind their neighbours' outputs: in place would race
-        if overlap(out, x) or overlap(out, cur) or overlap(out, nxt) or overlap(x, nxt):
+        if out.overlaps(x) or out.overlaps(cur) or out.overlaps(nxt) or x.overlaps(nxt):
             raise ArgumentError("a device DF2TFilter cannot filter in place: out must not overlap x or the filter state")
         nx = x.shape[0]
         if nx == 0 or x.size == 0:

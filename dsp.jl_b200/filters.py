@@ -423,9 +423,6 @@ class FIRFilter:
         hshape = (self.history_len,) + x.shape[1:]
         hist = self._hist or [None, DeviceArray(hshape, x.dtype)]
 
-        def overlap(a, b):
-            return a is not None and a.nbytes and b.nbytes and a.ptr < b.ptr + b.nbytes and b.ptr < a.ptr + a.nbytes
-
         if buffer is None:
             out = DeviceArray((st.nout,) + x.shape[1:], plan.out_dtype)
         else:
@@ -435,7 +432,7 @@ class FIRFilter:
                 raise ArgumentError(f"buffer must be a {plan.out_dtype} DeviceArray of channel shape {x.shape[1:]}")
             if buffer.shape[0] < st.nout:
                 raise ArgumentError(f"buffer is too small: the call produces {st.nout} outputs, buffer holds {buffer.shape[0]}")
-            if overlap(buffer, x) or overlap(hist[0], buffer) or overlap(hist[1], buffer):
+            if buffer.overlaps(x) or buffer.overlaps(hist[0]) or buffer.overlaps(hist[1]):
                 raise ArgumentError("a device FIRFilter cannot filter in place: buffer must not overlap x")
             out = buffer
         if self._hist is None:
