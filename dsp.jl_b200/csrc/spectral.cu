@@ -8,6 +8,9 @@
 //   * Welch: |Z|^2 accumulated in registers across all segments a CTA owns; real signals ride two
 //     segments per complex FFT (z = a + i b), and because |A_k|^2 + |B_k|^2 = (|Z_k|^2 + |Z_{N-k}|^2)/2
 //     the split is deferred to the finalize kernel -- the inner loop never un-mixes the two spectra.
+//     One kernel body with two work assignments: one signal (a unit range per CTA, one partial row each, added to
+//     across streaming calls) or the columns of a matrix (a range of (channel, slice) items, one row per item); one
+//     finalize kernel reduces the rows of each channel.
 //   * STFT / spectrogram: the spectrum is parked in shared memory (natural order), un-mixed per bin and
 //     stored column by column, coalesced along frequency.
 // Generic path (any other nfft): segment/window kernel -> batched cuFFT -> power / store kernels.
@@ -85,7 +88,7 @@ template <typename T, bool CPLX> struct in_type { using type = T; };
 template <typename T> struct in_type<T, true> { using type = cx<T>; };
 
 // ---------------------------------------------------------------------------------------------- fused Welch
-// Persistent CTAs; CTA c owns a contiguous range of units (unit = one complex segment, or two consecutive real
+// Persistent CTAs; a virtual CTA (below) runs a sequence of units (unit = one complex segment, or two consecutive real
 // segments packed as re/im).  TMA variant: the raw samples of the NEXT unit (one contiguous hop+n range) are
 // fetched by a single cp.async.bulk into a staging buffer while the current unit's FFT passes run, so the HBM
 // latency of the segment loads is off the critical path; the first FFT pass reads the staged samples from
@@ -97,7 +100,7 @@ template <typename T> struct in_type<T, true> { using type = cx<T>; };
 // window values never change -- they are loaded once (32 registers for the Float32 hi/lo pairs), which removes the window
 // reads (13 % of the kernel's shared-memory wavefronts at nfft = 4096) and the 32 KB table.
 // G > 1: G independent thread groups per CTA, each a "virtual CTA" with its own data buffer, staging buffer and mbarrier
-// and its own range of units, synchronising among themselves only (named barriers); the groups share ONE copy of the
+// and its own work, synchronising among themselves only (named barriers); the groups share ONE copy of the
 // twiddle tables and of the window table, so three 4096-point transforms fit one SM where two single-group CTAs with
 // private tables did (ncu on the two-CTA configuration: 4 warps per scheduler, issue slots 60 % busy, the stalls that
 // remain -- wait, short scoreboard -- are latency a third warp set hides).
@@ -120,11 +123,27 @@ template <typename T, int N, int G> struct welch_bounds {
     static constexpr int minblocks = G == 1 ? fft_minblocks<T, N>::value : 1;
 };
 
-template <typename T, int N, bool CPLX, int MODE, int G>
+// The two work assignments of welch_fused_kernel; virtual CTA v of nv takes the v-th of nv equal contiguous shares of the
+// work.  One signal (BATCH = false: welch_exec*, range, streaming, multitaper, filt_welch): the work is the units of segments
+// seg0 .. seg0 + nseg - 1 (`sample_offset`: the signal index of the buffer's first sample), and v writes partial row v
+// once, at the end.  Many channels (BATCH = true: welch_batch_exec*): the columns of a len x nchan matrix, `chan_stride`
+// samples apart, nseg segments (upc units) each.  The work is nitems (channel, slice) items: slice j of a channel owns its
+// units [j per, min((j+1) per, upc)), so units never cross a channel and a real unit's two segments always belong to one
+// channel (the finalize pass un-mixes bins k and N-k of one row).  v writes ONE partial row per item (row = item index);
+// the TMA prefetch of the next unit runs across item and channel boundaries.  No atomics: the result is deterministic.
+// Each work assignment's parameters are Nil in the other's instances, and each keeps the parameter order it had as a kernel
+// of its own: ptxas assigns the parameters' uniform registers by offset, and a struct of them compiles to different code.
+struct Nil {};
+template <bool USED, typename X> using welch_arg = typename std::conditional<USED, X, Nil>::type;
+
+template <typename T, int N, bool CPLX, int MODE, int G, bool BATCH>
 __global__ void __launch_bounds__((welch_bounds<T, N, G>::NTG * G), (welch_bounds<T, N, G>::minblocks))
-welch_fused_kernel(const void* __restrict__ s_, int64_t seg0, int64_t nseg, int64_t hop, int n,
-                   int64_t sample_offset, const typename win_t<T>::type* __restrict__ win, const cx<T>* __restrict__ tw,
-                   const cx<T>* __restrict__ g16, const cx<T>* __restrict__ g256, T* __restrict__ partial, int fresh_from) {
+welch_fused_kernel(const void* __restrict__ s_, welch_arg<BATCH, int64_t> chan_stride, welch_arg<!BATCH, int64_t> seg0,
+                   int64_t nseg, welch_arg<BATCH, int64_t> upc, welch_arg<BATCH, int64_t> per, welch_arg<BATCH, int> slices,
+                   welch_arg<BATCH, int64_t> nitems, int64_t hop, int n, welch_arg<!BATCH, int64_t> sample_offset,
+                   const typename win_t<T>::type* __restrict__ win, const cx<T>* __restrict__ tw,
+                   const cx<T>* __restrict__ g16, const cx<T>* __restrict__ g256, T* __restrict__ partial,
+                   welch_arg<!BATCH, int> fresh_from) {
     constexpr int NT = fft_threads<N>::value;                 // threads of one group
     constexpr int NB16 = N / 16;
     constexpr int ITL = (NB16 + NT - 1) / NT;
@@ -170,16 +189,31 @@ welch_fused_kernel(const void* __restrict__ s_, int64_t seg0, int64_t nseg, int6
 #pragma unroll
         for (int r = 0; r < 16; ++r) acc[i][r] = T(0);
 
-    const int64_t units = CPLX ? nseg : (nseg + 1) / 2;
+    // this virtual CTA's share [w0, w1) of the units (one signal) or of the items (batch)
+    int64_t work;
+    if constexpr (BATCH) work = nitems;
+    else work = CPLX ? nseg : (nseg + 1) / 2;
     const int64_t vcta = (int64_t)blockIdx.x * G + gid, nvcta = (int64_t)gridDim.x * G;     // (CTA, group) = virtual CTA
-    const int64_t per = (units + nvcta - 1) / nvcta;
-    const int64_t u0 = vcta * per < units ? vcta * per : units;
-    const int64_t u1 = u0 + per < units ? u0 + per : units;
+    const int64_t share = (work + nvcta - 1) / nvcta;
+    const int64_t w0 = vcta * share < work ? vcta * share : work;
+    const int64_t w1 = w0 + share < work ? w0 + share : work;
 
-    auto unit_src = [&](int64_t u) -> const In* { return s + ((seg0 + (CPLX ? u : 2 * u)) * hop - sample_offset); };
+    // unit u (of channel c in a batch)
+    auto unit_src = [&](int64_t c, int64_t u) -> const In* {
+        if constexpr (BATCH) return s + c * chan_stride + (CPLX ? u : 2 * u) * hop;
+        else return s + ((seg0 + (CPLX ? u : 2 * u)) * hop - sample_offset);
+    };
     auto unit_bytes = [&](int64_t u) -> uint32_t {
         const bool hasB = !CPLX && (2 * u + 1 < nseg);
         return (uint32_t)((hasB ? hop + n : n) * sizeof(In));
+    };
+    // batch: item i -> (channel c, units [ua, ub))
+    auto item_range = [&](int64_t i, int64_t& c, int64_t& ua, int64_t& ub) {
+        if constexpr (BATCH) {
+            c = i / slices;
+            ua = (i - c * slices) * per;
+            ub = ua + per < upc ? ua + per : upc;
+        }
     };
     if constexpr (TMA) {
         if (tid == 0) {
@@ -189,206 +223,20 @@ welch_fused_kernel(const void* __restrict__ s_, int64_t seg0, int64_t nseg, int6
     }
     pdl_wait();                                       // constants staged; the samples and `partial` come from preceding kernels
     __syncthreads();                                  // twiddle tables staged, barrier initialised
+    // the current item: channel c, units [ua, ub); one signal is one item, its whole range
+    int64_t c = 0, ua = BATCH ? 0 : w0, ub = BATCH ? 0 : w1;
+    if constexpr (BATCH) {
+        if (w0 < w1) item_range(w0, c, ua, ub);
+    }
     if constexpr (TMA) {
-        if (tid == 0 && u0 < u1) {
-            mbar_expect_tx(bar, unit_bytes(u0));
-            tma_load_1d(stage, unit_src(u0), unit_bytes(u0), bar);
-        }
-    }
-    uint32_t parity = 0;
-
-    for (int64_t u = u0; u < u1; ++u) {
-        const bool hasB = !CPLX && (2 * u + 1 < nseg);
-        const In* pa = TMA ? stage : unit_src(u);
-        const In* pb = pa + hop;
-        if constexpr (TMA) {
-            mbar_wait(bar, parity);
-            parity ^= 1;
-        }
-        auto ld0 = [&](int j, int it, int r) -> cx<T> {
-            if (j >= n) return mkc<T>(T(0), T(0));
-            if constexpr (CPLX) {
-                cx<T> v = pa[j];
-                if (WREG || WSM || win) { const W w = WREG ? wreg[WREG ? it : 0][WREG ? r : 0] : (WSM ? wsm[j] : win[j]); v = mkc<T>(win_mul(v.x, w), win_mul(v.y, w)); }
-                return v;
-            } else {
-                T a = pa[j];
-                T b = hasB ? pb[j] : T(0);
-                if (WREG || WSM || win) { const W w = WREG ? wreg[WREG ? it : 0][WREG ? r : 0] : (WSM ? wsm[j] : win[j]); a = win_mul(a, w); b = win_mul(b, w); }
-                return mkc<T>(a, b);
-            }
-        };
-        // first pass: the staged samples are read and transformed, then -- one barrier later, which also ends the
-        // previous unit's last pass -- stored; once every thread is past its reads (the barrier after the pass: with two
-        // first-pass iterations, N = 16384, the second one reads after the pass's own barrier) the staging buffer is
-        // refilled with the next unit while the remaining passes run -- behind a proxy fence, which orders those
-        // generic-proxy reads before the bulk copy's async-proxy writes
-        fft_first_pass<T, N, NT, true>(ctx, tid, ld0, scope);
-        scope.sync();
-        if constexpr (TMA) {
-            if (tid == 0 && u + 1 < u1) {
-                fence_proxy_async_shared();
-                mbar_expect_tx(bar, unit_bytes(u + 1));
-                tma_load_1d(stage, unit_src(u + 1), unit_bytes(u + 1), bar);
-            }
-        }
-        fft_middle<T, N, NT>(ctx, tid, scope);
-#pragma unroll
-        for (int it = 0; it < ITL; ++it) {
-            const int tp = tid + it * NT;
-            if (NB16 % NT != 0 && tp >= NB16) break;
-            cx<T> v[16];
-            fft_last_pass<T, N>(ctx, tp, v);
-#pragma unroll
-            for (int r = 0; r < 16; ++r) acc[it][r] += cabs2(v[r]);
-        }
-    }
-
-    // rows below `fresh_from` hold the sums of earlier launches since welch_begin and are added to; the others are
-    // written for the first time (no memset of the partial rows, and the finalize pass reads only rows that were written)
-    T* dst = partial + vcta * N;
-    const bool add = vcta < fresh_from;
-#pragma unroll
-    for (int it = 0; it < ITL; ++it) {
-        const int tp = tid + it * NT;
-        if (tp < NB16) {
-#pragma unroll
-            for (int r = 0; r < 16; ++r) {                                       // natural order, coalesced along tp
-                T* q = dst + tp + r * NB16;
-                *q = add ? *q + acc[it][r] : acc[it][r];
-            }
-        }
-    }
-}
-
-// Reduce the partial spectra that were written since welch_begin (rows < nparts) in Float64, fold the two-for-one mixing
-// for real input, apply the fft2pow! scale (m1 = 1/r, m2 = 2/r; :142-172).  A CTA owns 32 consecutive bins; warp s sums
-// rows s, s+32, ... (a warp reads 128 contiguous bytes of a row -- the earlier one-warp-per-bin form read a 32-byte sector
-// per element and took 14 us for 592 rows, 5 % of the whole C3 Welch), then the 32 slices are added in a fixed order.
-template <typename T, int N>
-__global__ void __launch_bounds__(1024) welch_finalize_kernel(const T* __restrict__ partial, int nparts, T* __restrict__ out,
-                                                              int nout, int real_in, int onesided, double m1, double m2) {
-    __shared__ double red[32][33];
-    pdl_launch_dependents();
-    pdl_wait();
-    const int b = threadIdx.x & 31, sl = threadIdx.x >> 5;
-    const int k = blockIdx.x * 32 + b;
-    double sum = 0.0;
-    if (k < nout) {
-        const T* c0 = partial + k;                          // the partial spectra are in natural order
-        const T* c1 = partial + ((N - k) & (N - 1));
-        if (real_in) {
-#pragma unroll 4
-            for (int c = sl; c < nparts; c += 32) sum += (double)c0[(int64_t)c * N] + (double)c1[(int64_t)c * N];
-        } else {
-#pragma unroll 4
-            for (int c = sl; c < nparts; c += 32) sum += (double)c0[(int64_t)c * N];
-        }
-    }
-    red[sl][b] = sum;
-    __syncthreads();
-    if (sl == 0 && k < nout) {
-#pragma unroll
-        for (int i = 1; i < 32; ++i) sum += red[i][b];
-        double m = m1;
-        if (real_in) {
-            sum *= 0.5;
-            if (onesided && !(k == 0 || k == N / 2)) m = m2;
-        }
-        out[k] = (T)(sum * m);
-    }
-}
-
-// ---------------------------------------------------------------------------------------------- batched fused Welch
-// Many channels (the columns of a len x nchan matrix, `chan_stride` samples apart), one launch.  A work item is a
-// (channel, slice) pair: slice j of a channel owns its units [j per, min((j+1) per, upc)), so units never cross a channel and
-// a real unit's two segments always belong to one channel (the finalize pass un-mixes bins k and N-k of one row).  Virtual
-// CTA v takes the contiguous item range [v ipv, (v+1) ipv); it accumulates |Z|^2 in registers over an item's units and writes
-// ONE partial row per item (row = item index).  Same front end, FFT and shared-memory layout as welch_fused_kernel; the TMA
-// prefetch of the next unit runs across item and channel boundaries.  No atomics: the result is deterministic.
-template <typename T, int N, bool CPLX, int MODE, int G>
-__global__ void __launch_bounds__((welch_bounds<T, N, G>::NTG * G), (welch_bounds<T, N, G>::minblocks))
-welch_batch_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t nseg, int64_t upc, int64_t per, int slices,
-                   int64_t nitems, int64_t hop, int n, const typename win_t<T>::type* __restrict__ win,
-                   const cx<T>* __restrict__ tw, const cx<T>* __restrict__ g16, const cx<T>* __restrict__ g256,
-                   T* __restrict__ partial) {
-    constexpr int NT = fft_threads<N>::value;
-    constexpr int NB16 = N / 16;
-    constexpr int ITL = (NB16 + NT - 1) / NT;
-    using L = welch_layout<T, N, CPLX, MODE>;
-    using Scope = typename std::conditional<G == 1, FftCtaScope, FftGroupScope<NT>>::type;
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    using In = typename in_type<T, CPLX>::type;
-    const In* s = reinterpret_cast<const In*>(s_);
-    const int gid = G == 1 ? 0 : threadIdx.x / NT;
-    const int tid = G == 1 ? threadIdx.x : threadIdx.x - gid * NT;
-    constexpr bool TMA = MODE >= 1;
-    constexpr bool WSM = MODE == 2;
-    constexpr bool WREG = MODE == 3;
-    using W = typename win_t<T>::type;
-    cx<T>* tabs = reinterpret_cast<cx<T>*>(smem_raw);
-    W* wsm = reinterpret_cast<W*>(smem_raw + L::table_bytes());
-    unsigned char* gbase = smem_raw + L::table_bytes() + L::window_bytes(n) + (size_t)gid * L::group_bytes(n, hop);
-    cx<T>* sm = reinterpret_cast<cx<T>*>(gbase);
-    In* stage = reinterpret_cast<In*>(sm + padded_len<T>(N));
-    uint64_t* bar = reinterpret_cast<uint64_t*>(gbase + L::group_bytes(n, hop) - 16);
-    pdl_launch_dependents();
-    const FftCtx<T> ctx = fft_make_ctx_at<T, N, NT * G>(sm, tabs, g16, g256, tw, threadIdx.x);
-    if constexpr (WSM) {
-        for (int i = threadIdx.x; i < n; i += NT * G) wsm[i] = win[i];
-    }
-    Scope scope;
-    if constexpr (G > 1) scope.id = 8 + gid;
-    W wreg[WREG ? ITL : 1][WREG ? 16 : 1];
-    if constexpr (WREG) {
-#pragma unroll
-        for (int it = 0; it < ITL; ++it)
-#pragma unroll
-            for (int r = 0; r < 16; ++r) {
-                const int j = tid + it * NT + r * NB16;
-                wreg[it][r] = (j < n && tid + it * NT < NB16) ? win[j] : W{};
-            }
-    }
-    T acc[ITL][16];
-#pragma unroll
-    for (int i = 0; i < ITL; ++i)
-#pragma unroll
-        for (int r = 0; r < 16; ++r) acc[i][r] = T(0);
-
-    const int64_t vcta = (int64_t)blockIdx.x * G + gid, nvcta = (int64_t)gridDim.x * G;
-    const int64_t ipv = (nitems + nvcta - 1) / nvcta;
-    const int64_t i0 = vcta * ipv < nitems ? vcta * ipv : nitems;
-    const int64_t i1 = i0 + ipv < nitems ? i0 + ipv : nitems;
-    // item -> (channel, first unit, end unit)
-    auto item_range = [&](int64_t i, int64_t& c, int64_t& ua, int64_t& ub) {
-        c = i / slices;
-        ua = (i - c * slices) * per;
-        ub = ua + per < upc ? ua + per : upc;
-    };
-    auto unit_src = [&](int64_t c, int64_t u) -> const In* { return s + c * chan_stride + (CPLX ? u : 2 * u) * hop; };
-    auto unit_bytes = [&](int64_t u) -> uint32_t {
-        const bool hasB = !CPLX && (2 * u + 1 < nseg);
-        return (uint32_t)((hasB ? hop + n : n) * sizeof(In));
-    };
-    if constexpr (TMA) {
-        if (tid == 0) {
-            mbar_init(bar, 1);
-            mbar_fence_init();
-        }
-    }
-    pdl_wait();
-    __syncthreads();
-    int64_t c = 0, ua = 0, ub = 0;
-    if (i0 < i1) item_range(i0, c, ua, ub);
-    if constexpr (TMA) {
-        if (tid == 0 && i0 < i1) {
+        if (tid == 0 && w0 < w1) {
             mbar_expect_tx(bar, unit_bytes(ua));
             tma_load_1d(stage, unit_src(c, ua), unit_bytes(ua), bar);
         }
     }
     uint32_t parity = 0;
 
-    for (int64_t item = i0; item < i1; ++item) {
+    for (int64_t item = w0; !BATCH || item < w1; ++item) {
         for (int64_t u = ua; u < ub; ++u) {
             const bool hasB = !CPLX && (2 * u + 1 < nseg);
             const In* pa = TMA ? stage : unit_src(c, u);
@@ -410,13 +258,25 @@ welch_batch_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t nse
                     return mkc<T>(a, b);
                 }
             };
+            // first pass: the staged samples are read and transformed, then -- one barrier later, which also ends the
+            // previous unit's last pass -- stored; once every thread is past its reads (the barrier after the pass: with two
+            // first-pass iterations, N = 16384, the second one reads after the pass's own barrier) the staging buffer is
+            // refilled with the next unit while the remaining passes run -- behind a proxy fence, which orders those
+            // generic-proxy reads before the bulk copy's async-proxy writes
             fft_first_pass<T, N, NT, true>(ctx, tid, ld0, scope);
-            scope.sync();                               // every read of the staging buffer is done (welch_fused_kernel)
-            if constexpr (TMA) {
+            scope.sync();
+            if constexpr (TMA && !BATCH) {
+                if (tid == 0 && u + 1 < ub) {
+                    fence_proxy_async_shared();
+                    mbar_expect_tx(bar, unit_bytes(u + 1));
+                    tma_load_1d(stage, unit_src(c, u + 1), unit_bytes(u + 1), bar);
+                }
+            }
+            if constexpr (TMA && BATCH) {
                 // the next unit: the following one of this item, else the first one of the next item
                 if (tid == 0) {
                     int64_t nc = c, nu = u + 1, nub = ub;
-                    if (nu == ub && item + 1 < i1) item_range(item + 1, nc, nu, nub);
+                    if (nu == ub && item + 1 < w1) item_range(item + 1, nc, nu, nub);
                     if (nu < nub) {
                         fence_proxy_async_shared();
                         mbar_expect_tx(bar, unit_bytes(nu));
@@ -435,42 +295,59 @@ welch_batch_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t nse
                 for (int r = 0; r < 16; ++r) acc[it][r] += cabs2(v[r]);
             }
         }
-        T* dst = partial + item * N;
+
+        // one signal: rows below `fresh_from` hold the sums of earlier launches since welch_begin and are added to; the
+        // others are written for the first time (no memset of the partial rows, and the finalize pass reads only rows that
+        // were written).  Batch: row `item`, and the next item starts from zero.
+        T* dst = partial + (BATCH ? item : vcta) * N;
+        bool add = false;
+        if constexpr (!BATCH) add = vcta < fresh_from;
 #pragma unroll
         for (int it = 0; it < ITL; ++it) {
             const int tp = tid + it * NT;
             if (tp < NB16) {
 #pragma unroll
-                for (int r = 0; r < 16; ++r) {
-                    dst[tp + r * NB16] = acc[it][r];
-                    acc[it][r] = T(0);
+                for (int r = 0; r < 16; ++r) {                                   // natural order, coalesced along tp
+                    if constexpr (BATCH) {
+                        dst[tp + r * NB16] = acc[it][r];
+                        acc[it][r] = T(0);
+                    } else {
+                        T* q = dst + tp + r * NB16;
+                        *q = add ? *q + acc[it][r] : acc[it][r];
+                    }
                 }
             }
         }
-        if (item + 1 < i1) item_range(item + 1, c, ua, ub);
+        if constexpr (BATCH) {
+            if (item + 1 < w1) item_range(item + 1, c, ua, ub);
+        } else {
+            break;                                    // one signal: one pass
+        }
     }
 }
 
-// Channel c of the batch: rows c*slices .. c*slices + slices - 1 of `partial`, reduced in Float64 in a fixed order (warp sl
-// sums rows sl, sl + nw, ...; then the nw warp sums in order), un-mixed and scaled as in welch_finalize_kernel, written to
-// column c of the nout x nchan result.  blockIdx.y = channel; blockDim.x = 32 nw with nw = min(32, slices).
+// Reduce the partial spectra of channel blockIdx.y -- its `rows` rows, written since welch_begin (one signal) or one per slice
+// (batch) -- in Float64, fold the two-for-one mixing for real input, apply the fft2pow! scale (m1 = 1/r, m2 = 2/r; :142-172)
+// and write column blockIdx.y of the nout x nchan result.  A CTA owns 32 consecutive bins; warp sl of the nw = blockDim.x / 32
+// sums rows sl, sl + nw, ... (a warp reads 128 contiguous bytes of a row -- the earlier one-warp-per-bin form read a 32-byte
+// sector per element and took 14 us for 592 rows, 5 % of the whole C3 Welch), then the nw slices are added in a fixed order.
 template <typename T, int N>
-__global__ void __launch_bounds__(1024) welch_batch_finalize_kernel(const T* __restrict__ partial, int slices, T* __restrict__ out,
-                                                                    int nout, int real_in, int onesided, double m1, double m2) {
+__global__ void __launch_bounds__(1024) welch_finalize_kernel(const T* __restrict__ partial, int rows, T* __restrict__ out,
+                                                              int nout, int real_in, int onesided, double m1, double m2) {
     __shared__ double red[32][33];
     pdl_launch_dependents();
     pdl_wait();
     const int b = threadIdx.x & 31, sl = threadIdx.x >> 5, nw = blockDim.x >> 5;
     const int k = blockIdx.x * 32 + b;
-    const T* rows = partial + (int64_t)blockIdx.y * slices * N;
+    const T* chan = partial + (int64_t)blockIdx.y * rows * N;
     double sum = 0.0;
     if (k < nout) {
-        const T* c0 = rows + k;
-        const T* c1 = rows + ((N - k) & (N - 1));
+        const T* c0 = chan + k;                             // the partial spectra are in natural order
+        const T* c1 = chan + ((N - k) & (N - 1));
         if (real_in) {
-            for (int c = sl; c < slices; c += nw) sum += (double)c0[(int64_t)c * N] + (double)c1[(int64_t)c * N];
+            for (int c = sl; c < rows; c += nw) sum += (double)c0[(int64_t)c * N] + (double)c1[(int64_t)c * N];
         } else {
-            for (int c = sl; c < slices; c += nw) sum += (double)c0[(int64_t)c * N];
+            for (int c = sl; c < rows; c += nw) sum += (double)c0[(int64_t)c * N];
         }
     }
     red[sl][b] = sum;
@@ -1040,11 +917,27 @@ __global__ void per2_pad_kernel(const T* __restrict__ s, int64_t n1, int64_t n2,
 }
 
 // ---------------------------------------------------------------------------------------------- dispatch
-#define DSP_FUSED_SIZES(X) X(256) X(512) X(1024) X(2048) X(4096) X(8192) X(16384)
-
 static bool fused_size_ok(int64_t nfft, bool f64) {
     if (nfft < 256 || (nfft & (nfft - 1))) return false;
     return nfft <= (f64 ? 8192 : 16384);
+}
+
+// Calls f(T(), std::integral_constant<int, N>()) with T the plan's real eltype and N = nfft, for the sizes that have fused
+// kernels (fused_size_ok); otherwise sets the "no fused <what> kernel" error
+template <typename T, typename F> static int fused_size_dispatch(const SpecPlanImpl* p, const char* what, F&& f) {
+    switch (p->nfft) {
+#define X(NN)                                                                                               \
+    case NN:                                                                                                \
+        if constexpr (sizeof(T) == 8 && NN > 8192) break;                                                   \
+        else return f(T(0), std::integral_constant<int, NN>());
+        X(256) X(512) X(1024) X(2048) X(4096) X(8192) X(16384)
+#undef X
+    }
+    set_error("no fused %s kernel for nfft=%lld", what, (long long)p->nfft);
+    return DSPB200_EUNSUPPORTED;
+}
+template <typename F> static int fused_dispatch(const SpecPlanImpl* p, const char* what, F&& f) {
+    return p->f64 ? fused_size_dispatch<double>(p, what, f) : fused_size_dispatch<float>(p, what, f);
 }
 
 template <typename K> static int set_smem(K kernel, size_t bytes) {
@@ -1052,60 +945,25 @@ template <typename K> static int set_smem(K kernel, size_t bytes) {
     return DSPB200_OK;
 }
 
-// Launch configuration of the fused Welch kernel: MODE (staging / window placement) x G (thread groups per CTA).  Every
-// candidate that fits is rated by the warps it keeps resident per SM (occupancy calculator x G); ties go to the window
-// in shared memory, then to fewer groups.
-template <typename T, int N, bool CPLX>
-static int launch_welch_fused(SpecPlanImpl* p, const void* s, int64_t seg0, int64_t nseg, int64_t sample_offset,
-                              cudaStream_t st) {
-    constexpr int NT = fft_threads<N>::value;
-    using In = typename in_type<T, CPLX>::type;
-    using W = typename win_t<T>::type;
-    using Kern = void (*)(const void*, int64_t, int64_t, int64_t, int, int64_t, const W*, const cx<T>*, const cx<T>*, const cx<T>*, T*, int);
+template <typename T, bool BATCH>
+using welch_kern_t = void (*)(const void*, welch_arg<BATCH, int64_t>, welch_arg<!BATCH, int64_t>, int64_t,
+                              welch_arg<BATCH, int64_t>, welch_arg<BATCH, int64_t>, welch_arg<BATCH, int>,
+                              welch_arg<BATCH, int64_t>, int64_t, int, welch_arg<!BATCH, int64_t>,
+                              const typename win_t<T>::type*, const cx<T>*, const cx<T>*, const cx<T>*, T*,
+                              welch_arg<!BATCH, int>);
+
+// The fused Welch instances (MODE: staging / window placement, G: thread groups per CTA) in order of preference (measured
+// sweep): f(kernel, shared-memory bytes, MODE, G) for each one that may run on TMA-`aligned` segments with(out) a window, the
+// direct-load instance last.  These are all the instances there are; dspb200_spec_plan_pin_welch names them from this list.
+template <typename T, int N, bool CPLX, bool BATCH, typename F>
+static int welch_candidates(const SpecPlanImpl* p, bool aligned, bool windowed, F&& f) {
     constexpr bool MULTI = sizeof(T) == 4 && N >= 1024 && N <= 4096;       // sizes that get multi-group variants
-    // TMA staging needs 16-byte aligned segment starts and sizes
-    const uintptr_t first = (uintptr_t)s + (uintptr_t)((seg0 * p->hop - sample_offset) * (int64_t)sizeof(In));
-    const bool aligned = (first % 16 == 0) && ((p->hop * sizeof(In)) % 16 == 0) && ((p->n * sizeof(In)) % 16 == 0);
-    const int64_t units = CPLX ? nseg : (nseg + 1) / 2;
-    if (units < 1) return DSPB200_OK;
-    const W* win = reinterpret_cast<const W*>(p->d_window);
-    struct Cand { Kern k; size_t smem; int mode, g, warps, per_sm; };
-    Cand best{nullptr, 0, 0, 0, -1, 0};
-    SpecPlanImpl::WelchCfg& cached = p->welch_cfg[aligned ? 1 : 0];
-    if (cached.kern != nullptr) {
-        const int64_t cap = (int64_t)p->sm_count * cached.per_sm;
-        const int64_t want = cdiv(units, cached.g);
-        const int grid = cached.vctas ? (int)(cached.vctas / cached.g) : (int)(want < cap ? want : cap);
-        DSP_CUDA(launch_pdl(reinterpret_cast<Kern>(cached.kern), (unsigned)grid, (unsigned)cached.threads, cached.smem, st,
-                            s, seg0, nseg, p->hop, (int)p->n, sample_offset, win, reinterpret_cast<const cx<T>*>(p->d_tw),
-                            reinterpret_cast<const cx<T>*>(p->d_t16), reinterpret_cast<const cx<T>*>(p->d_t256),
-                            reinterpret_cast<T*>(p->partial.p), p->rows_used));
-        DSP_LAUNCH_OK();
-        if (grid * cached.g > p->rows_used) p->rows_used = grid * cached.g;
-        cached.used = (int64_t)grid * cached.g;
-        return DSPB200_OK;
-    }
-    // candidates are offered in order of preference (measured sweep); the first one that
-    // keeps at least 12 warps resident per SM is taken, otherwise the one with the most resident warps
-    auto consider = [&](Kern k, size_t smem, int mode, int g) -> int {
-        if (best.warps >= 12) return DSPB200_OK;
-        if (smem > p->smem_optin) return DSPB200_OK;
-        DSP_TRY(set_smem(k, smem));
-        int per_sm = 0;
-        DSP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, NT * g, smem));
-        if (per_sm < 1) return DSPB200_OK;
-        if ((int64_t)per_sm * g * p->sm_count > p->nparts) per_sm = (int)(p->nparts / ((int64_t)g * p->sm_count));
-        if (per_sm < 1) return DSPB200_OK;
-        const int warps = per_sm * g * NT / 32;
-        if (warps > best.warps) best = Cand{k, smem, mode, g, warps, per_sm};
-        return DSPB200_OK;
-    };
-#define DSP_WELCH_CAND(MODE_, G_)                                                                        \
-    DSP_TRY(consider(welch_fused_kernel<T, N, CPLX, MODE_, G_>,                                          \
-                     welch_layout<T, N, CPLX, MODE_>::total(p->n, p->hop, G_), MODE_, G_))
-    constexpr bool WREGOK = sizeof(T) == 4 && N <= 4096;           // window in registers: 32 extra registers per thread
+    constexpr bool WREGOK = sizeof(T) == 4 && N <= 4096;                   // window in registers: 32 extra registers per thread
+#define DSP_WELCH_CAND(MODE_, G_)                                                                                   \
+    DSP_TRY(f(welch_kern_t<T, BATCH>(welch_fused_kernel<T, N, CPLX, MODE_, G_, BATCH>),                             \
+              welch_layout<T, N, CPLX, MODE_>::total(p->n, p->hop, G_), MODE_, G_))
     if (aligned) {
-        if (win) {
+        if (windowed) {
             if constexpr (CPLX) {
                 // complex: two CTAs per SM with the window in registers, then in shared memory
                 if constexpr (WREGOK) DSP_WELCH_CAND(3, 1);
@@ -1122,30 +980,98 @@ static int launch_welch_fused(SpecPlanImpl* p, const void* s, int64_t seg0, int6
         DSP_WELCH_CAND(1, 1);
         if constexpr (MULTI) DSP_WELCH_CAND(1, 2);
     }
-    if (best.k == nullptr) DSP_WELCH_CAND(0, 1);
+    DSP_WELCH_CAND(0, 1);
 #undef DSP_WELCH_CAND
-    DSP_REQUIRE(best.k != nullptr, "no Welch kernel configuration fits (nfft=%lld)", (long long)p->nfft);
+    return DSPB200_OK;
+}
+
+// Resident CTAs per SM of a G-group instance; row_cap > 0 bounds one wave to that many virtual CTAs
+template <typename K>
+static int welch_per_sm(const SpecPlanImpl* p, K k, int threads, int g, size_t smem, int64_t row_cap, int* per_sm) {
+    DSP_TRY(set_smem(k, smem));
+    DSP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(per_sm, k, threads, smem));
+    if (row_cap > 0 && (int64_t)*per_sm * g * p->sm_count > row_cap) *per_sm = (int)(row_cap / ((int64_t)g * p->sm_count));
+    return DSPB200_OK;
+}
+
+// Launch configuration of the fused Welch kernel, chosen once per (plan, path, alignment class) into `cfg`: every candidate
+// that fits is rated by the warps it keeps resident per SM (occupancy calculator x G); the first one that keeps at least 12
+// is taken, otherwise the one with the most, and the direct-load instance only when no other fits.  The selection walks up
+// to nine instances through cudaFuncSetAttribute + the occupancy calculator (tens of microseconds), hence the cache.
+// row_cap: the single-signal path's `nparts` (one wave never has more virtual CTAs than `partial` has rows), 0 for a batch.
+template <typename T, int N, bool CPLX, bool BATCH>
+static int welch_select(SpecPlanImpl* p, SpecPlanImpl::WelchCfg& cfg, bool aligned, int64_t row_cap) {
+    if (cfg.kern != nullptr) return DSPB200_OK;
+    constexpr int NT = fft_threads<N>::value;
+    using Kern = welch_kern_t<T, BATCH>;
+    struct Cand { Kern k; size_t smem; int mode, g, warps, per_sm; };
+    Cand best{nullptr, 0, 0, 0, -1, 0};
+    auto consider = [&](Kern k, size_t smem, int mode, int g) -> int {
+        if (best.warps >= 12 || (mode == 0 && best.k != nullptr)) return DSPB200_OK;
+        if (smem > p->smem_optin) return DSPB200_OK;
+        int per_sm = 0;
+        DSP_TRY(welch_per_sm(p, k, NT * g, g, smem, row_cap, &per_sm));
+        if (per_sm < 1) return DSPB200_OK;
+        const int warps = per_sm * g * NT / 32;
+        if (warps > best.warps) best = Cand{k, smem, mode, g, warps, per_sm};
+        return DSPB200_OK;
+    };
+    DSP_TRY((welch_candidates<T, N, CPLX, BATCH>(p, aligned, p->d_window != nullptr, consider)));
+    DSP_REQUIRE(best.k != nullptr, "no %sWelch kernel configuration fits (nfft=%lld)", BATCH ? "batched " : "", (long long)p->nfft);
     DSP_TRY(set_smem(best.k, best.smem));              // (the last candidate examined may have left a different limit)
-    cached.kern = reinterpret_cast<void*>(best.k); cached.smem = best.smem; cached.g = best.g; cached.per_sm = best.per_sm;
-    cached.threads = NT * best.g; cached.mode = best.mode;
-    // one wave of persistent CTAs: exactly the number that is co-resident; (CTAs x groups) never exceeds the rows of `partial`
-    const int64_t cap = (int64_t)p->sm_count * best.per_sm;
-    const int64_t want = cdiv(units, best.g);
-    const int grid = (int)(want < cap ? want : cap);
-    DSP_CUDA(launch_pdl(best.k, (unsigned)grid, (unsigned)(NT * best.g), best.smem, st, s, seg0, nseg, p->hop, (int)p->n,
-                        sample_offset, win, reinterpret_cast<const cx<T>*>(p->d_tw), reinterpret_cast<const cx<T>*>(p->d_t16),
-                        reinterpret_cast<const cx<T>*>(p->d_t256), reinterpret_cast<T*>(p->partial.p), p->rows_used));
+    cfg.kern = reinterpret_cast<void*>(best.k); cfg.smem = best.smem; cfg.g = best.g; cfg.per_sm = best.per_sm;
+    cfg.threads = NT * best.g; cfg.mode = best.mode;
+    return DSPB200_OK;
+}
+
+// CTAs of one resident wave of the chosen instance, or the pinned number of virtual CTAs / G
+static int64_t welch_wave(const SpecPlanImpl* p, const SpecPlanImpl::WelchCfg& cfg) {
+    return cfg.vctas ? cfg.vctas / cfg.g : (int64_t)p->sm_count * cfg.per_sm;
+}
+
+// Launch the chosen instance on the CTAs that `work` units (one signal) or items (batch) need at G per CTA, at most one wave
+template <typename T, bool BATCH>
+static int welch_launch(SpecPlanImpl* p, SpecPlanImpl::WelchCfg& cfg, int64_t work, const void* s,
+                        welch_arg<BATCH, int64_t> chan_stride, welch_arg<!BATCH, int64_t> seg0, int64_t nseg,
+                        welch_arg<BATCH, int64_t> upc, welch_arg<BATCH, int64_t> per, welch_arg<BATCH, int> slices,
+                        welch_arg<BATCH, int64_t> nitems, welch_arg<!BATCH, int64_t> sample_offset, void* partial,
+                        welch_arg<!BATCH, int> fresh_from, cudaStream_t st) {
+    const int64_t wave = welch_wave(p, cfg), want = cdiv(work, cfg.g);
+    const int grid = (int)(want < wave ? want : wave);
+    DSP_CUDA(launch_pdl(reinterpret_cast<welch_kern_t<T, BATCH>>(cfg.kern), (unsigned)grid, (unsigned)cfg.threads, cfg.smem, st,
+                        s, chan_stride, seg0, nseg, upc, per, slices, nitems, p->hop, (int)p->n, sample_offset,
+                        reinterpret_cast<const typename win_t<T>::type*>(p->d_window), reinterpret_cast<const cx<T>*>(p->d_tw),
+                        reinterpret_cast<const cx<T>*>(p->d_t16), reinterpret_cast<const cx<T>*>(p->d_t256),
+                        reinterpret_cast<T*>(partial), fresh_from));
     DSP_LAUNCH_OK();
-    if (grid * best.g > p->rows_used) p->rows_used = grid * best.g;
-    cached.used = (int64_t)grid * best.g;
+    cfg.used = (int64_t)grid * cfg.g;
+    return DSPB200_OK;
+}
+
+// One signal: segments seg0 .. seg0 + nseg - 1 of the buffer s (whose first sample is the signal's sample_offset), added to
+// the partial rows of the accumulation open since welch_begin
+template <typename T, int N, bool CPLX>
+static int launch_welch_fused(SpecPlanImpl* p, const void* s, int64_t seg0, int64_t nseg, int64_t sample_offset,
+                              cudaStream_t st) {
+    using In = typename in_type<T, CPLX>::type;
+    // TMA staging needs 16-byte aligned segment starts and sizes
+    const uintptr_t first = (uintptr_t)s + (uintptr_t)((seg0 * p->hop - sample_offset) * (int64_t)sizeof(In));
+    const bool aligned = (first % 16 == 0) && ((p->hop * sizeof(In)) % 16 == 0) && ((p->n * sizeof(In)) % 16 == 0);
+    const int64_t units = CPLX ? nseg : (nseg + 1) / 2;
+    if (units < 1) return DSPB200_OK;
+    SpecPlanImpl::WelchCfg& cfg = p->welch_cfg[aligned ? 1 : 0];
+    DSP_TRY((welch_select<T, N, CPLX, false>(p, cfg, aligned, p->nparts)));
+    // a pinned number of virtual CTAs runs in full, past the units if need be
+    DSP_TRY((welch_launch<T, false>(p, cfg, cfg.vctas ? cfg.vctas : units, s, Nil(), seg0, nseg, Nil(), Nil(), Nil(), Nil(),
+                                    sample_offset, p->partial.p, p->rows_used, st)));
+    if (cfg.used > p->rows_used) p->rows_used = (int)cfg.used;
     return DSPB200_OK;
 }
 
 template <typename T, int N>
 static int launch_welch_finalize(SpecPlanImpl* p, double r, void* out, cudaStream_t st) {
-    const int threads = 1024;
-    const int grid = (int)cdiv(p->nout, 32);
-    DSP_CUDA(launch_pdl(welch_finalize_kernel<T, N>, (unsigned)grid, (unsigned)threads, (size_t)0, st,
+    // one channel, 32 warps
+    DSP_CUDA(launch_pdl(welch_finalize_kernel<T, N>, (unsigned)cdiv(p->nout, 32), 1024u, (size_t)0, st,
                         reinterpret_cast<const T*>(p->partial.p), p->rows_used, reinterpret_cast<T*>(out), (int)p->nout,
                         p->cplx ? 0 : 1, (int)p->onesided, 1.0 / r, 2.0 / r));
     DSP_LAUNCH_OK();
@@ -1171,86 +1097,31 @@ static int64_t welch_batch_slices(int64_t gc, int64_t upc, int64_t nv, int64_t m
     return best;
 }
 
-// Batched Welch over the nchan columns of a len x nchan matrix (k segments each).  The kernel configuration (MODE x G) is
-// chosen by the same preference list as launch_welch_fused, cached separately.
+// Batched Welch over the nchan columns of a len x nchan matrix (k segments each): one kernel and one finalize launch per
+// channel group
 template <typename T, int N, bool CPLX>
 static int launch_welch_batch(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan, int64_t k, double r, void* out,
                               cudaStream_t st) {
-    constexpr int NT = fft_threads<N>::value;
     using In = typename in_type<T, CPLX>::type;
-    using W = typename win_t<T>::type;
-    using Kern = void (*)(const void*, int64_t, int64_t, int64_t, int64_t, int, int64_t, int64_t, int, const W*, const cx<T>*,
-                          const cx<T>*, const cx<T>*, T*);
-    constexpr bool MULTI = sizeof(T) == 4 && N >= 1024 && N <= 4096;
     // TMA staging needs every unit start 16-byte aligned: the base, the channel stride (launch_stft_fused's rule), hop and n
     const bool aligned = ((uintptr_t)s % 16 == 0) && ((len * sizeof(In)) % 16 == 0 || nchan == 1) &&
                          ((p->hop * sizeof(In)) % 16 == 0) && ((p->n * sizeof(In)) % 16 == 0);
-    const W* win = reinterpret_cast<const W*>(p->d_window);
     SpecPlanImpl::WelchCfg& cfg = p->welch_batch_cfg[aligned ? 1 : 0];
-    if (cfg.kern == nullptr) {
-        struct Cand { Kern k; size_t smem; int mode, g, warps, per_sm; };
-        Cand best{nullptr, 0, 0, 0, -1, 0};
-        auto consider = [&](Kern kn, size_t smem, int mode, int g) -> int {
-            if (best.warps >= 12) return DSPB200_OK;
-            if (smem > p->smem_optin) return DSPB200_OK;
-            DSP_TRY(set_smem(kn, smem));
-            int per_sm = 0;
-            DSP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kn, NT * g, smem));
-            if (per_sm < 1) return DSPB200_OK;
-            const int warps = per_sm * g * NT / 32;
-            if (warps > best.warps) best = Cand{kn, smem, mode, g, warps, per_sm};
-            return DSPB200_OK;
-        };
-#define DSP_WELCH_CAND(MODE_, G_)                                                                                    \
-    DSP_TRY(consider(welch_batch_kernel<T, N, CPLX, MODE_, G_>, welch_layout<T, N, CPLX, MODE_>::total(p->n, p->hop, G_), \
-                     MODE_, G_))
-        constexpr bool WREGOK = sizeof(T) == 4 && N <= 4096;
-        if (aligned) {
-            if (win) {
-                if constexpr (CPLX) {
-                    if constexpr (WREGOK) DSP_WELCH_CAND(3, 1);
-                    DSP_WELCH_CAND(2, 1);
-                    if constexpr (MULTI) { DSP_WELCH_CAND(3, 2); DSP_WELCH_CAND(2, 2); }
-                } else {
-                    if constexpr (MULTI) { DSP_WELCH_CAND(2, 3); DSP_WELCH_CAND(2, 2); }
-                    DSP_WELCH_CAND(2, 1);
-                    if constexpr (WREGOK) DSP_WELCH_CAND(3, 1);
-                }
-            }
-            if constexpr (MULTI && !CPLX) DSP_WELCH_CAND(1, 3);
-            DSP_WELCH_CAND(1, 1);
-            if constexpr (MULTI) DSP_WELCH_CAND(1, 2);
-        }
-        if (best.k == nullptr) DSP_WELCH_CAND(0, 1);
-#undef DSP_WELCH_CAND
-        DSP_REQUIRE(best.k != nullptr, "no batched Welch kernel configuration fits (nfft=%lld)", (long long)p->nfft);
-        DSP_TRY(set_smem(best.k, best.smem));
-        cfg.kern = reinterpret_cast<void*>(best.k); cfg.smem = best.smem; cfg.g = best.g; cfg.per_sm = best.per_sm;
-        cfg.threads = NT * best.g; cfg.mode = best.mode;
-    }
+    DSP_TRY((welch_select<T, N, CPLX, true>(p, cfg, aligned, 0)));
     const int64_t upc = CPLX ? k : (k + 1) / 2;
-    const int64_t cap = cfg.vctas ? cfg.vctas / cfg.g : (int64_t)p->sm_count * cfg.per_sm;   // resident CTAs: one wave
-    const int64_t nv = cap * cfg.g;                                   // resident virtual CTAs
+    const int64_t nv = welch_wave(p, cfg) * cfg.g;                   // resident virtual CTAs
     const int64_t rows_cap = (int64_t)(WELCH_BATCH_SCRATCH / ((size_t)N * sizeof(T)));
     const int64_t gc_max = nchan < rows_cap ? nchan : rows_cap;
-    const auto* tw = reinterpret_cast<const cx<T>*>(p->d_tw);
-    const auto* g16 = reinterpret_cast<const cx<T>*>(p->d_t16);
-    const auto* g256 = reinterpret_cast<const cx<T>*>(p->d_t256);
     for (int64_t c0 = 0; c0 < nchan; c0 += gc_max) {
         const int64_t gc = nchan - c0 < gc_max ? nchan - c0 : gc_max;
         const int64_t slices = welch_batch_slices(gc, upc, nv, rows_cap / gc);
         const int64_t per = cdiv(upc, slices);
         const int64_t nitems = gc * slices;
         DSP_TRY(p->bpartial.reserve((size_t)nitems * N * sizeof(T)));
-        const int64_t want = cdiv(nitems, cfg.g);
-        const int grid = (int)(want < cap ? want : cap);
-        DSP_CUDA(launch_pdl(reinterpret_cast<Kern>(cfg.kern), (unsigned)grid, (unsigned)cfg.threads, cfg.smem, st,
-                            (const void*)((const In*)s + c0 * len), len, k, upc, per, (int)slices, nitems, p->hop, (int)p->n,
-                            win, tw, g16, g256, reinterpret_cast<T*>(p->bpartial.p)));
-        DSP_LAUNCH_OK();
-        cfg.used = (int64_t)grid * cfg.g;
+        DSP_TRY((welch_launch<T, true>(p, cfg, nitems, (const In*)s + c0 * len, len, Nil(), k, upc, per, (int)slices, nitems,
+                                       Nil(), p->bpartial.p, Nil(), st)));
         const int nw = slices < 32 ? (int)slices : 32;
-        welch_batch_finalize_kernel<T, N><<<dim3((unsigned)cdiv(p->nout, 32), (unsigned)gc), 32 * nw, 0, st>>>(
+        welch_finalize_kernel<T, N><<<dim3((unsigned)cdiv(p->nout, 32), (unsigned)gc), 32 * nw, 0, st>>>(
             reinterpret_cast<const T*>(p->bpartial.p), (int)slices, reinterpret_cast<T*>(out) + c0 * p->nout, (int)p->nout,
             CPLX ? 0 : 1, (int)p->onesided, 1.0 / r, 2.0 / r);
         DSP_LAUNCH_OK();
@@ -1329,82 +1200,21 @@ static int launch_stft_fused(SpecPlanImpl* p, const void* s, int64_t len, int64_
     return DSPB200_OK;
 }
 
-template <typename T> static int welch_fused_dispatch(SpecPlanImpl* p, const void* s, int64_t seg0, int64_t nseg,
-                                                       int64_t sample_offset, cudaStream_t st) {
-    switch (p->nfft) {
-#define X(NN)                                                                                               \
-    case NN:                                                                                                \
-        if constexpr (sizeof(T) == 8 && NN > 8192) break;                                                   \
-        else return p->cplx ? launch_welch_fused<T, NN, true>(p, s, seg0, nseg, sample_offset, st)          \
-                            : launch_welch_fused<T, NN, false>(p, s, seg0, nseg, sample_offset, st);
-        DSP_FUSED_SIZES(X)
-#undef X
-    }
-    set_error("no fused Welch kernel for nfft=%lld", (long long)p->nfft);
-    return DSPB200_EUNSUPPORTED;
-}
-template <typename T> static int welch_finalize_dispatch(SpecPlanImpl* p, double r, void* out, cudaStream_t st) {
-    switch (p->nfft) {
-#define X(NN)                                                                                               \
-    case NN:                                                                                                \
-        if constexpr (sizeof(T) == 8 && NN > 8192) break;                                                   \
-        else return launch_welch_finalize<T, NN>(p, r, out, st);
-        DSP_FUSED_SIZES(X)
-#undef X
-    }
-    set_error("no fused Welch kernel for nfft=%lld", (long long)p->nfft);
-    return DSPB200_EUNSUPPORTED;
-}
-template <typename T> static int welch_batch_dispatch(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan, int64_t k,
-                                                       double r, void* out, cudaStream_t st) {
-    switch (p->nfft) {
-#define X(NN)                                                                                               \
-    case NN:                                                                                                \
-        if constexpr (sizeof(T) == 8 && NN > 8192) break;                                                   \
-        else return p->cplx ? launch_welch_batch<T, NN, true>(p, s, len, nchan, k, r, out, st)              \
-                            : launch_welch_batch<T, NN, false>(p, s, len, nchan, k, r, out, st);
-        DSP_FUSED_SIZES(X)
-#undef X
-    }
-    set_error("no fused Welch kernel for nfft=%lld", (long long)p->nfft);
-    return DSPB200_EUNSUPPORTED;
-}
-
-// Pinned Welch launch configuration (dspb200_spec_plan_pin_welch, a testing aid).  The instances are exactly the candidates
-// of the preference lists in launch_welch_fused / launch_welch_batch: nothing is compiled for the hook alone.
-template <typename T, int N, bool CPLX, bool BATCH> static void* welch_instance(int mode, int g) {
-    constexpr bool MULTI = sizeof(T) == 4 && N >= 1024 && N <= 4096;
-    constexpr bool WREGOK = sizeof(T) == 4 && N <= 4096;
-#define DSP_WELCH_INST(MODE_, G_)                                                                       \
-    if (mode == MODE_ && g == G_)                                                                       \
-        return BATCH ? reinterpret_cast<void*>(welch_batch_kernel<T, N, CPLX, MODE_, G_>)               \
-                     : reinterpret_cast<void*>(welch_fused_kernel<T, N, CPLX, MODE_, G_>);
-    DSP_WELCH_INST(0, 1) DSP_WELCH_INST(1, 1) DSP_WELCH_INST(2, 1)
-    if constexpr (WREGOK) { DSP_WELCH_INST(3, 1) }
-    if constexpr (MULTI) {
-        DSP_WELCH_INST(1, 2) DSP_WELCH_INST(2, 2)
-        if constexpr (CPLX) { DSP_WELCH_INST(3, 2) }
-        else { DSP_WELCH_INST(1, 3) DSP_WELCH_INST(2, 3) }
-    }
-#undef DSP_WELCH_INST
-    return nullptr;
-}
-template <typename T, int N, bool CPLX> static size_t welch_smem(int mode, int64_t n, int64_t hop, int g) {
-    switch (mode) {
-    case 0: return welch_layout<T, N, CPLX, 0>::total(n, hop, g);
-    case 1: return welch_layout<T, N, CPLX, 1>::total(n, hop, g);
-    case 2: return welch_layout<T, N, CPLX, 2>::total(n, hop, g);
-    default: return welch_layout<T, N, CPLX, 3>::total(n, hop, g);
-    }
-}
-// Fills both alignment classes of the cache: aligned calls get (mode, g), unaligned ones MODE 0, G = 1; both `vctas`.
-template <typename T, int N, bool CPLX>
-static int welch_pin(SpecPlanImpl* p, bool batched, int mode, int g, int64_t vctas) {
+// Pinned Welch launch configuration (dspb200_spec_plan_pin_welch, a testing aid): any instance of welch_candidates.  Fills
+// both alignment classes of the cache: aligned calls get (mode, g), unaligned ones MODE 0, G = 1; both `vctas`.
+template <typename T, int N, bool CPLX, bool BATCH>
+static int welch_pin(SpecPlanImpl* p, int mode, int g, int64_t vctas) {
     constexpr int NT = fft_threads<N>::value;
+    using Kern = welch_kern_t<T, BATCH>;
     SpecPlanImpl::WelchCfg pinned[2];
     for (int a = 0; a < 2; ++a) {
         const int m = a ? mode : 0, gg = a ? g : 1;
-        void* k = batched ? welch_instance<T, N, CPLX, true>(m, gg) : welch_instance<T, N, CPLX, false>(m, gg);
+        Kern k = nullptr;
+        size_t smem = 0;
+        DSP_TRY((welch_candidates<T, N, CPLX, BATCH>(p, true, true, [&](Kern kc, size_t sc, int mc, int gc) -> int {
+            if (mc == m && gc == gg) { k = kc; smem = sc; }
+            return DSPB200_OK;
+        })));
         if (k == nullptr) {
             set_error("no Welch kernel instance MODE %d, G %d for this plan (nfft=%lld)", m, gg, (long long)N);
             return DSPB200_EUNSUPPORTED;
@@ -1413,55 +1223,23 @@ static int welch_pin(SpecPlanImpl* p, bool batched, int mode, int g, int64_t vct
             set_error("Welch MODE %d needs a window", m);
             return DSPB200_EUNSUPPORTED;
         }
-        const size_t smem = welch_smem<T, N, CPLX>(m, p->n, p->hop, gg);
         if (smem > p->smem_optin) {
             set_error("Welch MODE %d, G %d needs %zu bytes of shared memory (limit %zu)", m, gg, smem, p->smem_optin);
             return DSPB200_EUNSUPPORTED;
         }
-        DSP_TRY(set_smem(k, smem));
         int per_sm = 0;
-        DSP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, NT * gg, smem));
-        // (one resident wave of the single-signal kernel never has more virtual CTAs than `partial` has rows)
-        if (!batched && vctas == 0 && (int64_t)per_sm * gg * p->sm_count > p->nparts)
-            per_sm = (int)(p->nparts / ((int64_t)gg * p->sm_count));
+        DSP_TRY(welch_per_sm(p, k, NT * gg, gg, smem, !BATCH && vctas == 0 ? p->nparts : 0, &per_sm));
         if (per_sm < 1) {
             set_error("Welch MODE %d, G %d does not fit an SM", m, gg);
             return DSPB200_EUNSUPPORTED;
         }
-        pinned[a].kern = k; pinned[a].smem = smem; pinned[a].g = gg; pinned[a].per_sm = per_sm; pinned[a].threads = NT * gg;
-        pinned[a].mode = m; pinned[a].vctas = vctas;
+        pinned[a].kern = reinterpret_cast<void*>(k); pinned[a].smem = smem; pinned[a].g = gg; pinned[a].per_sm = per_sm;
+        pinned[a].threads = NT * gg; pinned[a].mode = m; pinned[a].vctas = vctas;
     }
-    SpecPlanImpl::WelchCfg* cfg = batched ? p->welch_batch_cfg : p->welch_cfg;
+    SpecPlanImpl::WelchCfg* cfg = BATCH ? p->welch_batch_cfg : p->welch_cfg;
     cfg[0] = pinned[0];
     cfg[1] = pinned[1];
     return DSPB200_OK;
-}
-template <typename T> static int welch_pin_dispatch(SpecPlanImpl* p, bool batched, int mode, int g, int64_t vctas) {
-    switch (p->nfft) {
-#define X(NN)                                                                                               \
-    case NN:                                                                                                \
-        if constexpr (sizeof(T) == 8 && NN > 8192) break;                                                   \
-        else return p->cplx ? welch_pin<T, NN, true>(p, batched, mode, g, vctas)                            \
-                            : welch_pin<T, NN, false>(p, batched, mode, g, vctas);
-        DSP_FUSED_SIZES(X)
-#undef X
-    }
-    set_error("no fused Welch kernel for nfft=%lld", (long long)p->nfft);
-    return DSPB200_EUNSUPPORTED;
-}
-template <typename T> static int stft_fused_dispatch(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan,
-                                                      int64_t k, double r, int psd_only, void* out, cudaStream_t st) {
-    switch (p->nfft) {
-#define X(NN)                                                                                               \
-    case NN:                                                                                                \
-        if constexpr (sizeof(T) == 8 && NN > 8192) break;                                                   \
-        else return p->cplx ? launch_stft_fused<T, NN, true>(p, s, len, nchan, k, r, psd_only, out, st)     \
-                            : launch_stft_fused<T, NN, false>(p, s, len, nchan, k, r, psd_only, out, st);
-        DSP_FUSED_SIZES(X)
-#undef X
-    }
-    set_error("no fused STFT kernel for nfft=%lld", (long long)p->nfft);
-    return DSPB200_EUNSUPPORTED;
 }
 
 // ---------------------------------------------------------------------------------------------- generic path
@@ -1590,15 +1368,20 @@ static int welch_accumulate(SpecPlanImpl* p, const void* s, int64_t sample_offse
                             cudaStream_t st) {
     if (seg_end <= seg_begin) return DSPB200_OK;
     if (p->fused) {
-        return p->f64 ? welch_fused_dispatch<double>(p, s, seg_begin, seg_end - seg_begin, sample_offset, st)
-                      : welch_fused_dispatch<float>(p, s, seg_begin, seg_end - seg_begin, sample_offset, st);
+        return fused_dispatch(p, "Welch", [&](auto t, auto nn) {
+            using T = decltype(t);
+            constexpr int N = decltype(nn)::value;
+            return p->cplx ? launch_welch_fused<T, N, true>(p, s, seg_begin, seg_end - seg_begin, sample_offset, st)
+                           : launch_welch_fused<T, N, false>(p, s, seg_begin, seg_end - seg_begin, sample_offset, st);
+        });
     }
     return p->f64 ? welch_generic_acc<double>(p, s, sample_offset, seg_begin, seg_end, st)
                   : welch_generic_acc<float>(p, s, sample_offset, seg_begin, seg_end, st);
 }
 
 static int welch_finalize(SpecPlanImpl* p, double r, void* out, cudaStream_t st) {
-    if (p->fused) return p->f64 ? welch_finalize_dispatch<double>(p, r, out, st) : welch_finalize_dispatch<float>(p, r, out, st);
+    if (p->fused)
+        return fused_dispatch(p, "Welch", [&](auto t, auto nn) { return launch_welch_finalize<decltype(t), decltype(nn)::value>(p, r, out, st); });
     const int threads = 128;
     const int grid = (int)cdiv(p->nout, threads);
     if (p->f64)
@@ -1897,8 +1680,12 @@ int dspb200_spec_plan_pin_welch(dspb200_spec_plan* plan, int batched, int mode, 
                 (long long)vctas, groups);
     DSP_REQUIRE(batched || vctas <= p->nparts, "vctas (%lld) exceeds the plan's %d partial rows", (long long)vctas, p->nparts);
     DSP_CUDA(cudaSetDevice(p->device));
-    return p->f64 ? welch_pin_dispatch<double>(p, batched != 0, mode, groups, vctas)
-                  : welch_pin_dispatch<float>(p, batched != 0, mode, groups, vctas);
+    return fused_dispatch(p, "Welch", [&](auto t, auto nn) {
+        using T = decltype(t);
+        constexpr int N = decltype(nn)::value;
+        if (batched) return p->cplx ? welch_pin<T, N, true, true>(p, mode, groups, vctas) : welch_pin<T, N, false, true>(p, mode, groups, vctas);
+        return p->cplx ? welch_pin<T, N, true, false>(p, mode, groups, vctas) : welch_pin<T, N, false, false>(p, mode, groups, vctas);
+    });
 }
 
 int dspb200_spec_plan_welch_config(const dspb200_spec_plan* plan, int batched, int aligned, int* mode, int* groups,
@@ -1921,7 +1708,7 @@ int dspb200_welch_exec_dev(dspb200_spec_plan* plan, const void* s, int64_t len, 
 
 // Batched welch_pgram: the nchan columns of the column-major len x nchan matrix `s` are independent signals, each Welch-averaged
 // with the plan's configuration; out is nout x nchan.  Fused sizes: one launch over (channel, slice) work items plus one
-// finalize launch per channel group (welch_batch_kernel); cuFFT sizes: channel by channel.
+// finalize launch per channel group (welch_fused_kernel<..., BATCH = true>); cuFFT sizes: channel by channel.
 int dspb200_welch_batch_exec_dev(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, double r, void* out,
                                  void* stream) {
     DSP_RANGE("dspb200_welch_batch_exec_dev");
@@ -1939,8 +1726,12 @@ int dspb200_welch_batch_exec_dev(dspb200_spec_plan* plan, const void* s, int64_t
     DSP_REQUIRE(s != nullptr, "s is NULL");
     DSP_REQUIRE(r != 0.0, "r must be nonzero");
     if (p->fused)
-        return p->f64 ? welch_batch_dispatch<double>(p, s, len, nchan, k, r, out, st)
-                      : welch_batch_dispatch<float>(p, s, len, nchan, k, r, out, st);
+        return fused_dispatch(p, "Welch", [&](auto t, auto nn) {
+            using T = decltype(t);
+            constexpr int N = decltype(nn)::value;
+            return p->cplx ? launch_welch_batch<T, N, true>(p, s, len, nchan, k, r, out, st)
+                           : launch_welch_batch<T, N, false>(p, s, len, nchan, k, r, out, st);
+        });
     DSP_TRY(generic_prepare(p));
     return p->f64 ? welch_batch_generic<double>(p, s, len, nchan, k, r, out, st)
                   : welch_batch_generic<float>(p, s, len, nchan, k, r, out, st);
@@ -2042,8 +1833,12 @@ int dspb200_stft_exec_dev(dspb200_spec_plan* plan, const void* s, int64_t len, i
     DSP_REQUIRE(s && out, "NULL argument");
     if (r == 0.0) r = 1.0;
     if (p->fused)
-        return p->f64 ? stft_fused_dispatch<double>(p, s, len, nchan, k, r, psd_only, out, st)
-                      : stft_fused_dispatch<float>(p, s, len, nchan, k, r, psd_only, out, st);
+        return fused_dispatch(p, "STFT", [&](auto t, auto nn) {
+            using T = decltype(t);
+            constexpr int N = decltype(nn)::value;
+            return p->cplx ? launch_stft_fused<T, N, true>(p, s, len, nchan, k, r, psd_only, out, st)
+                           : launch_stft_fused<T, N, false>(p, s, len, nchan, k, r, psd_only, out, st);
+        });
     DSP_TRY(generic_prepare(p));
     return p->f64 ? stft_generic<double>(p, s, len, nchan, k, r, psd_only, out, st)
                   : stft_generic<float>(p, s, len, nchan, k, r, psd_only, out, st);

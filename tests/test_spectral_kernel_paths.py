@@ -1,7 +1,7 @@
 """Every Welch and STFT kernel instance and entry point (csrc/spectral.cu) bin by bin against a float64 reference.
 
 A plan with a power-of-two nfft = N in 256 .. 16384 (Float32) or 256 .. 8192 (Float64) is fused.  Welch runs
-`welch_fused_kernel<T, N, CPLX, MODE, G>` (one signal) or `welch_batch_kernel<...>` (the columns of a matrix): MODE 0
+`welch_fused_kernel<T, N, CPLX, MODE, G, BATCH>` on one signal or, BATCH, on the columns of a matrix: MODE 0
 loads the segments directly, 1 stages them by TMA, 2 also keeps the window in shared memory, 3 in registers; G thread
 groups share one CTA.  Which instance runs is chosen on the device from a preference list and the occupancy calculator,
 so `dspb200_spec_plan_pin_welch` pins it: every instance runs on the same data, on the same virtual-CTA count, and must
@@ -125,7 +125,7 @@ def welch_smem(dt, N, mode, n, hop, g):
 
 
 def welch_candidates(dt, N, aligned, windowed):
-    """The preference list of launch_welch_fused / launch_welch_batch, in order: (MODE, G)."""
+    """The preference list of welch_candidates in csrc/spectral.cu, in order: (MODE, G)."""
     f32, cplx = not _f64(dt), _cplx(dt)
     multi = f32 and 1024 <= N <= 4096
     wreg = f32 and N <= 4096
