@@ -90,6 +90,8 @@ SIGNATURES = {
     "dspb200_spec_plan_geometry": (_int, [_vp, C.POINTER(_int), C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_i64)]),
     "dspb200_stft_exec": (_int, [_vp, _vp, _i64, _i64, _dbl, _int, _vp]),
     "dspb200_stft_exec_dev": (_int, [_vp, _vp, _i64, _i64, _dbl, _int, _vp, _vp]),
+    "dspb200_stft_stream_exec": (_int, [_vp, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _i64, _dbl, _int, _vp, _i64]),
+    "dspb200_stft_stream_exec_dev": (_int, [_vp, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _i64, _dbl, _int, _vp, _i64, _vp]),
     "dspb200_arraysplit_exec": (_int, [_vp, _vp, _i64, _vp]),
     "dspb200_periodogram2_exec": (_int, [_int, _vp, _i64, _i64, _i64, _i64, _dbl, _int, _vp]),
     "dspb200_periodogram2_exec_dev": (_int, [_int, _vp, _i64, _i64, _i64, _i64, _dbl, _int, _vp, _vp]),
@@ -304,6 +306,17 @@ class SpecPlan(_Plan):
 
     def stft_dev(self, s_ptr, length, nchan, r, psd_only, out_ptr, stream=0):
         check(lib.dspb200_stft_exec_dev(self.handle, s_ptr, length, nchan, float(r), 1 if psd_only else 0, out_ptr, stream))
+
+    def stft_stream(self, hist_in, nhist, hist_out, ldh, x, nx, nchan, nseg, r, psd_only, out, ldo):
+        """One chunk of a host STFTStream: Fortran-ordered host arrays, histories ldh x nchan (hist_in None: empty)."""
+        check(lib.dspb200_stft_stream_exec(self.handle, None if hist_in is None else ptr(hist_in), int(nhist), ptr(hist_out),
+                                           int(ldh), ptr(x), int(nx), int(nchan), int(nseg), float(r), 1 if psd_only else 0,
+                                           ptr(out), int(ldo)))
+
+    def stft_stream_dev(self, hist_in_ptr, nhist, hist_out_ptr, ldh, x_ptr, nx, nchan, nseg, r, psd_only, out_ptr, ldo, stream=0):
+        """One chunk of a device STFTStream (dspb200_stft_stream_exec_dev): device pointers."""
+        check(lib.dspb200_stft_stream_exec_dev(self.handle, hist_in_ptr, int(nhist), hist_out_ptr, int(ldh), x_ptr, int(nx),
+                                               int(nchan), int(nseg), float(r), 1 if psd_only else 0, out_ptr, int(ldo), stream))
 
 
 class MtPlan(SpecPlan):

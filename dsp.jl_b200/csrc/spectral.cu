@@ -14,6 +14,9 @@
 //   * STFT / spectrogram: the spectrum is parked in shared memory (natural order), un-mixed per bin and
 //     stored column by column, coalesced along frequency.
 // Generic path (any other nfft): segment/window kernel -> batched cuFFT -> power / store kernels.
+// Streaming STFT (dspb200_stft_stream_exec(_dev)): the STREAM instances of the two STFT kernels read each channel's virtual
+// column [history; chunk] (StftStream) after stft_stream_edge_kernel has copied the seam samples and written the new history;
+// cuFFT sizes run the (channel, segment) pairs of a call through stft_stream_seg_kernel -> cuFFT -> stft_stream_store_kernel.
 #include "fft_core.cuh"
 #include "async_copy.cuh"
 #include <cufft.h>
@@ -63,6 +66,8 @@ struct SpecPlanImpl {
     DevBuf segbuf, specbuf, acc;  // acc: double[nbins_fft]
     // host-pointer path
     DevBuf in[2], out;
+    DevBuf hin, hout;             // dspb200_stft_stream_exec: the staged histories
+    DevBuf seam;                  // streaming STFT, fused sizes: the seam samples of the last call (stft_stream_edge_kernel)
     cudaStream_t s_copy = nullptr, s_exec = nullptr;
     cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr};
 };
@@ -436,6 +441,23 @@ __device__ __forceinline__ void stft_emit(const cx<T>* __restrict__ sm, void* __
     }
 }
 
+// Streaming STFT (dspb200_stft_stream_exec_dev): a call transforms segments 0 .. k - 1 of every channel's virtual column
+// v = [history (h samples); x].  A unit that starts in the history (a seam unit) reads the copy of v's first samples that the
+// call's edge kernel wrote to `seam` (stft_stream_edge_kernel); every other unit reads x + start - h.  Either way a unit's
+// samples are one contiguous range, staged by TMA or loaded directly exactly as in the one-shot call, so the same values
+// enter the same butterflies.  The one-shot instances take the empty struct, so their parameters and code are those of before.
+template <typename In, bool STREAM> struct StftStream {};
+template <typename In> struct StftStream<In, true> {
+    const In* seam;             // lds x nchan: v[0, lds) of every channel (the samples of its seam units)
+    int64_t lds, h;             // column stride of `seam`, samples of history
+    int64_t ldo;                // output columns per channel (replaces k as the column stride)
+    int tma;                    // the call meets the TMA alignment conditions (stft_w1k_kernel: stage every unit)
+    // first sample of the unit that starts at v[start] of channel c (x: the chunk, chan_stride = nx)
+    __device__ __forceinline__ const In* src(const In* x, int64_t chan_stride, int64_t c, int64_t start) const {
+        return start < h ? seam + c * lds + start : x + c * chan_stride + (start - h);
+    }
+};
+
 // One unit of the STFT kernel.  FAST: n == N (no zero padding) and, for real input, both segments present -- no per-sample
 // predicates; WIN: 1 window table present, 0 none (compile time), -1 run time.
 template <typename T, int N, bool CPLX, bool TMA, int WIN, bool FAST, class IssueNext>
@@ -493,12 +515,14 @@ __device__ __forceinline__ void stft_unit(const FftCtx<T>& ctx, cx<T>* sm, int t
 // (tried: compiling the Float32 STFT kernels for 768 resident threads per SM -- the 1024-point kernel fits 64 registers and
 //  gets 11 CTAs per SM instead of 8 -- but the spectrogram got slower and the windowed variants spill; kept at 512 threads /
 //  128 registers)
-template <typename T, int N, bool CPLX, bool TMA, int WIN>
+// STREAM: a streaming call (StftStream): s_ is the chunk x (chan_stride = nx), k the call's segments per channel; a
+// unit's samples come from StftStream::src and its columns are ldo apart.
+template <typename T, int N, bool CPLX, bool TMA, int WIN, bool STREAM>
 __global__ void __launch_bounds__(fft_threads<N>::value, fft_minblocks<T, N>::value)
 stft_fused_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int64_t units_per_chan, int64_t total_units,
                   int64_t hop, int n, const typename win_t<T>::type* __restrict__ win, const cx<T>* __restrict__ tw,
                   const cx<T>* __restrict__ g16, const cx<T>* __restrict__ g256, void* __restrict__ out_, int nout,
-                  int psd_only, int onesided, T m1, T m2) {
+                  int psd_only, int onesided, T m1, T m2, const StftStream<typename in_type<T, CPLX>::type, STREAM> ss) {
     constexpr int NT = fft_threads<N>::value;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
@@ -515,7 +539,10 @@ stft_fused_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, i
     // (channel, unit inside the channel) of the current unit, advanced incrementally: no 64-bit division in the loop
     int64_t chan = u0 < u1 ? u0 / units_per_chan : 0;
     int64_t uin = u0 < u1 ? u0 - chan * units_per_chan : 0;
-    auto src_of = [&](int64_t c, int64_t u) -> const In* { return s + c * chan_stride + (CPLX ? u : 2 * u) * hop; };
+    auto src_of = [&](int64_t c, int64_t u) -> const In* {
+        if constexpr (STREAM) return ss.src(s, chan_stride, c, (CPLX ? u : 2 * u) * hop);
+        else return s + c * chan_stride + (CPLX ? u : 2 * u) * hop;
+    };
     auto bytes_of = [&](int64_t u) -> uint32_t {
         const bool hb = !CPLX && (2 * u + 1 < k);
         return (uint32_t)((hb ? hop + n : n) * sizeof(In));
@@ -556,7 +583,9 @@ stft_fused_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, i
                 }
             }
         };
-        const int64_t colA = (chan * k + segA) * (int64_t)nout;
+        int64_t colA;
+        if constexpr (!STREAM) colA = (chan * k + segA) * (int64_t)nout;
+        else colA = (chan * ss.ldo + segA) * (int64_t)nout;     // the caller's output stride
         if (full && (CPLX || hasB))
             stft_unit<T, N, CPLX, TMA, WIN, true>(ctx, sm, tid, pa, hop, n, hasB, win, out_, colA, nout, psd_only, onesided, m1, m2, issue_next);
         else
@@ -588,11 +617,14 @@ inline void fill_t32(cx<float>* t32) {
 __host__ __device__ inline size_t warp_bytes(int64_t stage_elems, size_t elt) { return (((size_t)DATA_LEN * 8 + (size_t)stage_elems * elt + 15) & ~(size_t)15) + 16; }
 }  // namespace w1k
 
-template <bool CPLX, int WIN, int WARPS>
+// STREAM: a streaming call (StftStream, as stft_fused_kernel).  A stream keeps this plan whatever the alignment of the call:
+// ss.tma = 0 (unaligned) reads every unit directly from global memory in the first pass instead of staging it.
+template <bool CPLX, int WIN, int WARPS, bool STREAM>
 __global__ void __launch_bounds__(32 * WARPS)
 stft_w1k_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int64_t units_per_chan, int64_t total_units,
                 int64_t hop, int n, const float2* __restrict__ win, const cx<float>* __restrict__ g32, void* __restrict__ out_,
-                int nout, int psd_only, int onesided, float m1, float m2) {
+                int nout, int psd_only, int onesided, float m1, float m2,
+                const StftStream<typename in_type<float, CPLX>::type, STREAM> ss) {
     using T = float;
     using In = typename in_type<T, CPLX>::type;
     constexpr int N = w1k::N;
@@ -624,14 +656,24 @@ stft_w1k_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int
     const int64_t u1 = u0 + per < total_units ? u0 + per : total_units;
     int64_t chan = u0 < u1 ? u0 / units_per_chan : 0;
     int64_t uin = u0 < u1 ? u0 - chan * units_per_chan : 0;
-    auto src_of = [&](int64_t c, int64_t u) -> const In* { return s + c * chan_stride + (CPLX ? u : 2 * u) * hop; };
+    auto src_of = [&](int64_t c, int64_t u) -> const In* {
+        if constexpr (STREAM) return ss.src(s, chan_stride, c, (CPLX ? u : 2 * u) * hop);
+        else return s + c * chan_stride + (CPLX ? u : 2 * u) * hop;
+    };
     auto bytes_of = [&](int64_t u) -> uint32_t {
         const bool hb = !CPLX && (2 * u + 1 < k);
         return (uint32_t)((hb ? hop + n : n) * sizeof(In));
     };
-    if (lane == 0 && u0 < u1) {
-        mbar_expect_tx(bar, bytes_of(uin));
-        tma_load_1d(stage, src_of(chan, uin), bytes_of(uin), bar);
+    if constexpr (!STREAM) {
+        if (lane == 0 && u0 < u1) {
+            mbar_expect_tx(bar, bytes_of(uin));
+            tma_load_1d(stage, src_of(chan, uin), bytes_of(uin), bar);
+        }
+    } else {
+        if (lane == 0 && u0 < u1 && ss.tma) {
+            mbar_expect_tx(bar, bytes_of(uin));
+            tma_load_1d(stage, src_of(chan, uin), bytes_of(uin), bar);
+        }
     }
     uint32_t parity = 0;
     const bool full = (n == N);
@@ -645,9 +687,19 @@ stft_w1k_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int
         const bool hasB = !CPLX && (segA + 1 < k);
         int64_t nchan = chan, nuin = uin + 1;
         if (nuin == units_per_chan) { nuin = 0; ++nchan; }
-        mbar_wait(bar, parity);
-        parity ^= 1;
+        if constexpr (!STREAM) {
+            mbar_wait(bar, parity);
+            parity ^= 1;
+        } else {
+            if (ss.tma) {
+                mbar_wait(bar, parity);
+                parity ^= 1;
+            }
+        }
         const In* pa = stage;
+        if constexpr (STREAM) {
+            if (!ss.tma) pa = src_of(chan, uin);       // an unaligned streaming call reads its units directly
+        }
         const In* pb = pa + hop;
         // first pass: plain 32-point DFT of x[lane + 32 m] (window applied), 32 contiguous slots at block `lane`
         cx<T> v[32];
@@ -667,10 +719,18 @@ stft_w1k_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int
             }
         }
         __syncwarp();                                   // every lane has read the staging buffer (and the previous unit's spectrum)
-        if (lane == 0 && gu + 1 < u1) {                 // refill it with the next unit while this one is transformed
-            fence_proxy_async_shared();
-            mbar_expect_tx(bar, bytes_of(nuin));
-            tma_load_1d(stage, src_of(nchan, nuin), bytes_of(nuin), bar);
+        if constexpr (!STREAM) {
+            if (lane == 0 && gu + 1 < u1) {             // refill it with the next unit while this one is transformed
+                fence_proxy_async_shared();
+                mbar_expect_tx(bar, bytes_of(nuin));
+                tma_load_1d(stage, src_of(nchan, nuin), bytes_of(nuin), bar);
+            }
+        } else {
+            if (lane == 0 && gu + 1 < u1 && ss.tma) {
+                fence_proxy_async_shared();
+                mbar_expect_tx(bar, bytes_of(nuin));
+                tma_load_1d(stage, src_of(nchan, nuin), bytes_of(nuin), bar);
+            }
         }
         fft_bfly<T, 32, true>(v, nullptr);
         {
@@ -690,7 +750,9 @@ stft_w1k_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int
         }
         __syncwarp();
         // emit: bins kk = lane + 32 i; N - kk = (32 - lane) + 32 (31 - i) for lane > 0
-        const int64_t colA = (chan * k + segA) * (int64_t)nout;
+        int64_t colA;
+        if constexpr (!STREAM) colA = (chan * k + segA) * (int64_t)nout;
+        else colA = (chan * ss.ldo + segA) * (int64_t)nout;     // the caller's output stride
         const cx<T>* pk = sm + w1k::pad(lane);
         const cx<T>* pm = lane ? sm + w1k::pad(32 - lane) : sm;
         const bool half = !CPLX && onesided;
@@ -805,6 +867,72 @@ __global__ void stft_store_kernel(const cx<T>* __restrict__ X, int64_t nbins_fft
             reinterpret_cast<T*>(out_)[(col0 + b) * nout + k] = cabs2(z) * m;
         } else {
             reinterpret_cast<cx<T>*>(out_)[(col0 + b) * nout + k] = mirrored ? cconj(z) : z;
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------- streaming STFT, small kernels
+// Launch 1 of a streaming call, one grid-stride pass over nchan x (ls + hn) items: (a) seam[c lds + i] = v_c[i], i < ls --
+// the samples of the units that start in the history, contiguous, so that the transform reads every unit from one range;
+// (b) the new history hist_out[c ldh + i] = v_c[skip + i], i < hn.  v_c = [hist_in (h samples, column stride ldh); x_c].
+template <typename E>
+__global__ void stft_stream_edge_kernel(const E* __restrict__ hist_in, int64_t h, int64_t ldh, const E* __restrict__ x,
+                                        int64_t nx, int64_t nchan, E* __restrict__ seam, int64_t ls, int64_t lds, int64_t skip,
+                                        int64_t hn, E* __restrict__ hist_out) {
+    const int64_t per = ls + hn, total = nchan * per;
+    for (int64_t w = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; w < total; w += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t c = w / per, i = w - c * per;
+        const int64_t t = (i < ls ? i : skip + i - ls) - h;                     // index in x (negative: history)
+        const E v = t < 0 ? hist_in[c * ldh + h + t] : x[c * nx + t];
+        if (i < ls) seam[c * lds + i] = v;
+        else hist_out[c * ldh + i - ls] = v;
+    }
+}
+
+// Streaming calls, cuFFT sizes: the call's nchan x k (channel c, segment j) pairs, f = c k + j, fill the cuFFT batch in
+// order.  Slot b = blockIdx.y holds pair f0 + b: buf[b][i] = window[i] * v_c[j hop + i] (i < n), 0 for n <= i < nfft and
+// for slots past the list -- seg_window_kernel's values, read from the virtual column.  One slot per grid row: the pair is
+// resolved once per block, not per element.
+template <typename T, bool CPLX>
+__global__ void stft_stream_seg_kernel(const void* __restrict__ hist_, int64_t h, int64_t ldh, const void* __restrict__ x_,
+                                       int64_t nx, int64_t f0, int64_t nf, int64_t k, int64_t hop, int64_t n, int64_t nfft,
+                                       const typename win_t<T>::type* __restrict__ win, void* __restrict__ buf_) {
+    using In = typename in_type<T, CPLX>::type;
+    const In* hist = reinterpret_cast<const In*>(hist_);
+    const In* x = reinterpret_cast<const In*>(x_);
+    const int64_t b = blockIdx.y;
+    In* buf = reinterpret_cast<In*>(buf_) + b * nfft;
+    const int64_t f = f0 + b, c = f / k, t0 = (f - c * k) * hop - h;        // index in x of the segment's first sample
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nfft; i += (int64_t)gridDim.x * blockDim.x) {
+        In v;
+        if constexpr (CPLX) v = mkc<T>(T(0), T(0)); else v = T(0);
+        if (b < nf && i < n) {
+            const int64_t t = t0 + i;
+            v = t < 0 ? hist[c * ldh + h + t] : x[c * nx + t];
+            if (win) {
+                const auto w = win[i];
+                if constexpr (CPLX) v = mkc<T>(win_mul(v.x, w), win_mul(v.y, w)); else v = win_mul(v, w);
+            }
+        }
+        buf[i] = v;
+    }
+}
+
+// stft_store_kernel's values for the spectra of pairs f0 .. f0 + nf - 1 (slot b = blockIdx.y), into column (c ldo + j) of out
+template <typename T>
+__global__ void stft_stream_store_kernel(const cx<T>* __restrict__ X, int64_t nbins_fft, int64_t nfft, int64_t nout, int64_t f0,
+                                         int64_t k, int64_t ldo, int psd_only, int onesided, T m1, T m2, void* __restrict__ out_) {
+    const int64_t b = blockIdx.y, f = f0 + b, c = f / k, col = c * ldo + (f - c * k);
+    const cx<T>* Xb = X + b * nbins_fft;
+    for (int64_t kk = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; kk < nout; kk += (int64_t)gridDim.x * blockDim.x) {
+        const bool mirrored = kk >= nbins_fft;
+        const cx<T> z = Xb[mirrored ? nfft - kk : kk];
+        if (psd_only) {
+            T m = m1;
+            if (onesided && kk != 0 && !(kk == nbins_fft - 1 && (nfft % 2 == 0))) m = m2;
+            reinterpret_cast<T*>(out_)[col * nout + kk] = cabs2(z) * m;
+        } else {
+            reinterpret_cast<cx<T>*>(out_)[col * nout + kk] = mirrored ? cconj(z) : z;
         }
     }
 }
@@ -1129,35 +1257,47 @@ static int launch_welch_batch(SpecPlanImpl* p, const void* s, int64_t len, int64
     return DSPB200_OK;
 }
 
-template <typename T, int N, bool CPLX>
+// The history side of a streaming call (dspb200_stft_stream_exec_dev); the one-shot call passes none
+// (seam, lds: the copy of every channel's first virtual-column samples that the edge kernel wrote; fused sizes only)
+struct StftStreamArgs { const void* hist = nullptr; int64_t h = 0, ldh = 0, ldo = 0; const void* seam = nullptr; int64_t lds = 0; };
+
+// One-shot call (STREAM = false): k segments of each of the nchan columns of the len x nchan matrix s.  Streaming call: k
+// segments of each channel's virtual column [history; s], s being the nx = len x nchan chunk.  A stream runs the instance an
+// aligned one-shot call of the same plan runs, whatever the alignment of its history or chunk: stft_w1k_kernel rounds
+// differently from stft_fused_kernel, and the two TMA / direct instances of stft_fused_kernel round alike.
+template <typename T, int N, bool CPLX, bool STREAM = false>
 static int launch_stft_fused(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan, int64_t k, double r,
-                             int psd_only, void* out, cudaStream_t st) {
+                             int psd_only, void* out, cudaStream_t st, const StftStreamArgs& sa = StftStreamArgs()) {
     constexpr int NT = fft_threads<N>::value;
     using In = typename in_type<T, CPLX>::type;
+    using SS = StftStream<In, STREAM>;
+    SS ss{};
     const size_t base = (size_t)fft_smem_elems<T, N>() * sizeof(cx<T>);
     const size_t stage = (size_t)(CPLX ? p->n : p->hop + p->n) * sizeof(In) + 16;
     // Float32, N = 1024: every call that meets the TMA alignment conditions runs stft_w1k_kernel (its shared memory is at
     // most about 84 KB), so the fallback below is the direct-load instance alone
     constexpr bool W1K = sizeof(T) == 4 && N == 1024;
-    const bool tma = !W1K && ((uintptr_t)s % 16 == 0) && ((len * sizeof(In)) % 16 == 0 || nchan == 1) &&
-                     ((p->hop * sizeof(In)) % 16 == 0) && ((p->n * sizeof(In)) % 16 == 0) &&
+    const bool plan_aligned = ((p->hop * sizeof(In)) % 16 == 0) && ((p->n * sizeof(In)) % 16 == 0);
+    // the TMA alignment conditions: 16-byte aligned unit starts (streaming: x + start - h) and sizes
+    const bool aligned = plan_aligned && ((uintptr_t)s % 16 == 0) && ((len * sizeof(In)) % 16 == 0 || nchan == 1) &&
+                         (!STREAM || (sa.h * sizeof(In)) % 16 == 0);
+    const bool tma = !W1K && aligned &&
                      (base + stage <= p->smem_optin) && (base + stage <= 100 * 1024 || N >= 8192);   // N >= 8192: one CTA per SM anyway
     const size_t smem = tma ? base + stage : base;
     const int64_t upc = CPLX ? k : (k + 1) / 2;
     const int64_t units = upc * nchan;
     if (units < 1) return DSPB200_OK;
+    if constexpr (STREAM) ss = SS{reinterpret_cast<const In*>(sa.seam), sa.lds, sa.h, sa.ldo, (W1K ? aligned : tma) ? 1 : 0};
     const auto* w = reinterpret_cast<const typename win_t<T>::type*>(p->d_window);
     if constexpr (W1K) {
-        // one warp per unit (stft_w1k_kernel): needs the TMA alignment conditions
-        const bool aligned = ((uintptr_t)s % 16 == 0) && ((len * sizeof(In)) % 16 == 0 || nchan == 1) &&
-                             ((p->hop * sizeof(In)) % 16 == 0) && ((p->n * sizeof(In)) % 16 == 0);
-        if (aligned && p->d_t32 != nullptr) {
+        // one warp per unit (stft_w1k_kernel): a one-shot call needs the TMA alignment conditions, a stream those of its plan
+        if ((STREAM ? plan_aligned : aligned) && p->d_t32 != nullptr) {
             constexpr int WARPS = 4;
             const size_t smem1 = (size_t)w1k::T32_LEN * sizeof(cx<float>) + (w ? (size_t)p->n * sizeof(float2) : 0) +
                                  (size_t)WARPS * w1k::warp_bytes(CPLX ? p->n : p->hop + p->n, sizeof(In));
             using K1 = void (*)(const void*, int64_t, int64_t, int64_t, int64_t, int64_t, int, const float2*, const cx<float>*, void*, int,
-                                int, int, float, float);
-            K1 k1 = w ? (K1)stft_w1k_kernel<CPLX, 1, WARPS> : (K1)stft_w1k_kernel<CPLX, 0, WARPS>;
+                                int, int, float, float, SS);
+            K1 k1 = w ? (K1)stft_w1k_kernel<CPLX, 1, WARPS, STREAM> : (K1)stft_w1k_kernel<CPLX, 0, WARPS, STREAM>;
             if (smem1 <= p->smem_optin) {
                 DSP_TRY(set_smem(k1, smem1));
                 int per = 1;
@@ -1167,7 +1307,7 @@ static int launch_stft_fused(SpecPlanImpl* p, const void* s, int64_t len, int64_
                 const unsigned grid1 = (unsigned)(want < cap1 ? want : cap1);
                 k1<<<grid1, 32 * WARPS, smem1, st>>>(s, len, k, upc, units, p->hop, (int)p->n, reinterpret_cast<const float2*>(w),
                                                       reinterpret_cast<const cx<float>*>(p->d_t32), out, (int)p->nout, psd_only,
-                                                      p->onesided, (float)(1.0 / r), (float)(2.0 / r));
+                                                      p->onesided, (float)(1.0 / r), (float)(2.0 / r), ss);
                 DSP_LAUNCH_OK();
                 return DSPB200_OK;
             }
@@ -1177,17 +1317,17 @@ static int launch_stft_fused(SpecPlanImpl* p, const void* s, int64_t len, int64_
     const auto* g16 = reinterpret_cast<const cx<T>*>(p->d_t16);
     const auto* g256 = reinterpret_cast<const cx<T>*>(p->d_t256);
     using Kern = void (*)(const void*, int64_t, int64_t, int64_t, int64_t, int64_t, int, const typename win_t<T>::type*, const cx<T>*,
-                          const cx<T>*, const cx<T>*, void*, int, int, int, T, T);
+                          const cx<T>*, const cx<T>*, void*, int, int, int, T, T, SS);
     // window presence is a compile-time property of the Float32 kernels (predicated-off window products still issue)
     constexpr bool SPEC = sizeof(T) == 4;
     Kern kern;
     if constexpr (W1K) {
-        kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, false, 1> : (Kern)stft_fused_kernel<T, N, CPLX, false, 0>;
+        kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, false, 1, STREAM> : (Kern)stft_fused_kernel<T, N, CPLX, false, 0, STREAM>;
     } else if constexpr (SPEC) {
-        if (tma) kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, true, 1> : (Kern)stft_fused_kernel<T, N, CPLX, true, 0>;
-        else kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, false, 1> : (Kern)stft_fused_kernel<T, N, CPLX, false, 0>;
+        if (tma) kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, true, 1, STREAM> : (Kern)stft_fused_kernel<T, N, CPLX, true, 0, STREAM>;
+        else kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, false, 1, STREAM> : (Kern)stft_fused_kernel<T, N, CPLX, false, 0, STREAM>;
     } else {
-        kern = tma ? (Kern)stft_fused_kernel<T, N, CPLX, true, -1> : (Kern)stft_fused_kernel<T, N, CPLX, false, -1>;
+        kern = tma ? (Kern)stft_fused_kernel<T, N, CPLX, true, -1, STREAM> : (Kern)stft_fused_kernel<T, N, CPLX, false, -1, STREAM>;
     }
     DSP_TRY(set_smem(kern, smem));
     int per_sm = 1;
@@ -1195,7 +1335,7 @@ static int launch_stft_fused(SpecPlanImpl* p, const void* s, int64_t len, int64_
     const int64_t cap = (int64_t)p->sm_count * (per_sm < 1 ? 1 : per_sm);
     const unsigned grid = (unsigned)(units < cap ? units : cap);
     kern<<<grid, NT, smem, st>>>(s, len, k, upc, units, p->hop, (int)p->n, w, tw, g16, g256, out, (int)p->nout, psd_only,
-                                 p->onesided, (T)(1.0 / r), (T)(2.0 / r));
+                                 p->onesided, (T)(1.0 / r), (T)(2.0 / r), ss);
     DSP_LAUNCH_OK();
     return DSPB200_OK;
 }
@@ -1325,6 +1465,38 @@ template <typename T> static int stft_generic(SpecPlanImpl* p, const void* s, in
                                                            (T)(2.0 / r), out, c * k + b0);
             DSP_LAUNCH_OK();
         }
+    }
+    return DSPB200_OK;
+}
+
+// Streaming call, cuFFT sizes: the nchan x k (channel, segment) pairs fill the plan's batch in order, three launches per batch
+template <typename T> static int stft_stream_generic(SpecPlanImpl* p, const StftStreamArgs& sa, const void* x, int64_t nx,
+                                                      int64_t nchan, int64_t k, double r, int psd_only, void* out,
+                                                      cudaStream_t st) {
+    const int64_t pairs = nchan * k;
+    const int threads = 256;
+    const auto* w = reinterpret_cast<const typename win_t<T>::type*>(p->d_window);
+    // one grid row per batch slot, enough blocks along it for about 16 waves of the whole batch
+    auto cols = [&](int64_t len) {
+        const int64_t want = cdiv(len, threads), cap = cdiv((int64_t)p->sm_count * 16, p->batch);
+        return (unsigned)(want < cap ? want : cap);
+    };
+    for (int64_t f0 = 0; f0 < pairs; f0 += p->batch) {
+        const int64_t nf = pairs - f0 < p->batch ? pairs - f0 : p->batch;
+        const dim3 gseg(cols(p->nfft), (unsigned)p->batch);
+        if (p->cplx)
+            stft_stream_seg_kernel<T, true><<<gseg, threads, 0, st>>>(sa.hist, sa.h, sa.ldh, x, nx, f0, nf, k, p->hop, p->n, p->nfft,
+                                                                     w, p->segbuf.p);
+        else
+            stft_stream_seg_kernel<T, false><<<gseg, threads, 0, st>>>(sa.hist, sa.h, sa.ldh, x, nx, f0, nf, k, p->hop, p->n, p->nfft,
+                                                                      w, p->segbuf.p);
+        DSP_LAUNCH_OK();
+        DSP_TRY(generic_fft(p, st));
+        const dim3 gout(cols(p->nout), (unsigned)nf);
+        stft_stream_store_kernel<T><<<gout, threads, 0, st>>>(reinterpret_cast<const cx<T>*>(p->specbuf.p), p->nbins_fft, p->nfft,
+                                                              p->nout, f0, k, sa.ldo, psd_only, p->onesided, (T)(1.0 / r),
+                                                              (T)(2.0 / r), out);
+        DSP_LAUNCH_OK();
     }
     return DSPB200_OK;
 }
@@ -1858,6 +2030,119 @@ int dspb200_stft_exec(dspb200_spec_plan* plan, const void* s, int64_t len, int64
                       [&] { return dspb200_stft_exec_dev(plan, p->in[0].p, len, nchan, r, psd_only, p->out.p, p->s_exec); });
 }
 
+// Streaming stft / spectrogram.  Checks shared by both forms; *newh = samples of the new history.  Returns with *launch = false
+// when the call has nothing to do (no channel, or no sample and no segment: the history stays in hist_in).
+static int stft_stream_check(const SpecPlanImpl* p, const void* hist_in, int64_t nhist, const void* hist_out, int64_t ldh,
+                             const void* x, int64_t nx, int64_t nchan, int64_t nseg, double r, int psd_only, const void* out,
+                             int64_t ldo, bool dev, int64_t* newh, bool* launch) {
+    *launch = false;
+    DSP_REQUIRE(nhist >= 0 && nx >= 0 && nchan >= 0 && nseg >= 0 && ldh >= 0, "negative size");
+    DSP_REQUIRE(psd_only == 0 || psd_only == 1, "psd_only must be 0 (raw spectra) or 1 (PSD columns)");
+    DSP_REQUIRE(r != 0.0 || !psd_only, "r must be nonzero");
+    DSP_REQUIRE(hist_in != nullptr || nhist == 0, "hist_in is NULL but nhist = %lld", (long long)nhist);
+    DSP_REQUIRE(nhist <= ldh, "nhist (%lld) exceeds ldh (%lld)", (long long)nhist, (long long)ldh);
+    DSP_REQUIRE(ldo >= nseg, "output column stride ldo < nseg");
+    DSP_REQUIRE(nseg == 0 || (nseg - 1) * p->hop + p->n <= nhist + nx, "segment %lld runs past the virtual column (%lld samples)",
+                (long long)(nseg - 1), (long long)(nhist + nx));
+    *newh = nhist + nx - nseg * p->hop;
+    DSP_REQUIRE(*newh <= ldh, "the new history (%lld samples) exceeds ldh (%lld)", (long long)*newh, (long long)ldh);
+    if (dev) {
+        const size_t esz = dtype_size(p->dtype), oel = (psd_only ? 1 : 2) * (p->f64 ? 8 : 4);
+        const size_t hbytes = (size_t)(ldh * nchan) * esz, xbytes = (size_t)(nx * nchan) * esz;
+        const size_t obytes = (nchan && nseg) ? (size_t)(((nchan - 1) * ldo + nseg) * p->nout) * oel : 0;
+        // the kernels read the samples and history of other channels' CTAs: no written buffer may overlap another buffer
+        DSP_REQUIRE(!ranges_overlap(hist_out, hbytes, hist_in, hbytes) && !ranges_overlap(hist_out, hbytes, x, xbytes) &&
+                    !ranges_overlap(hist_out, hbytes, out, obytes), "hist_out overlaps hist_in, x or out");
+        DSP_REQUIRE(!ranges_overlap(out, obytes, x, xbytes) && !ranges_overlap(out, obytes, hist_in, hbytes),
+                    "out overlaps x or a history buffer");
+    }
+    if (nchan == 0 || (nx == 0 && nseg == 0)) return DSPB200_OK;
+    DSP_REQUIRE((x != nullptr || nx == 0) && (out != nullptr || nseg == 0) && (hist_out != nullptr || *newh == 0), "NULL argument");
+    *launch = true;
+    return DSPB200_OK;
+}
+
+// Segments 0 .. nseg - 1 of every channel's virtual column [hist_in (nhist); x (nx)] into out (column s of channel c at
+// out + (c ldo + s) nout), then the new history v[nseg hop, nhist + nx) into hist_out.  Fused sizes: at most two launches.
+int dspb200_stft_stream_exec_dev(dspb200_spec_plan* plan, const void* hist_in, int64_t nhist, void* hist_out, int64_t ldh,
+                                 const void* x, int64_t nx, int64_t nchan, int64_t nseg, double r, int psd_only, void* out,
+                                 int64_t ldo, void* stream) {
+    DSP_RANGE("dspb200_stft_stream_exec_dev");
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    SpecPlanImpl* p = &plan->impl;
+    int64_t newh = 0;
+    bool launch = false;
+    DSP_TRY(stft_stream_check(p, hist_in, nhist, hist_out, ldh, x, nx, nchan, nseg, r, psd_only, out, ldo, true, &newh, &launch));
+    if (!launch) return DSPB200_OK;
+    if (r == 0.0) r = 1.0;
+    cudaStream_t st = (cudaStream_t)stream;
+    StftStreamArgs sa{hist_in, nhist, ldh, ldo};
+    // launch 1: the seam copy (fused sizes: v[0, ls) of every channel, the samples of the units that start in the history)
+    // and the new history
+    int64_t ls = 0;
+    if (p->fused && nseg > 0 && nhist > 0) {
+        const int64_t us = p->cplx ? p->hop : 2 * p->hop, upc = p->cplx ? nseg : (nseg + 1) / 2;
+        const int64_t nsu = cdiv(nhist, us) < upc ? cdiv(nhist, us) : upc;            // seam units per channel
+        const int64_t end = (nsu - 1) * us + (p->cplx ? p->n : p->hop + p->n);
+        ls = end < nhist + nx ? end : nhist + nx;
+    }
+    const size_t esz = dtype_size(p->dtype);
+    const int64_t lds = cdiv(ls * (int64_t)esz, 16) * 16 / (int64_t)esz;              // 16-byte aligned columns (TMA)
+    if (ls > 0) DSP_TRY(p->seam.reserve((size_t)(lds * nchan) * esz));
+    sa.seam = p->seam.p;
+    sa.lds = lds;
+    if (ls + newh > 0) {
+        const int64_t total = nchan * (ls + newh);
+        const int threads = 256;
+        const unsigned grid = (unsigned)(cdiv(total, threads) < (int64_t)p->sm_count * 8 ? cdiv(total, threads) : (int64_t)p->sm_count * 8);
+        const int64_t skip = nseg * p->hop;
+#define DSP_EDGE(E) stft_stream_edge_kernel<E><<<grid, threads, 0, st>>>((const E*)hist_in, nhist, ldh, (const E*)x, nx, nchan, \
+                                                                         (E*)p->seam.p, ls, lds, skip, newh, (E*)hist_out)
+        switch (esz) {
+            case 4: DSP_EDGE(float); break;
+            case 8: DSP_EDGE(double); break;
+            default: DSP_EDGE(cx<double>); break;
+        }
+#undef DSP_EDGE
+        DSP_LAUNCH_OK();
+    }
+    if (nseg == 0) return DSPB200_OK;
+    // launch 2 (fused sizes): the transforms
+    if (p->fused)
+        return fused_dispatch(p, "STFT", [&](auto t, auto nn) {
+            using T = decltype(t);
+            constexpr int N = decltype(nn)::value;
+            return p->cplx ? launch_stft_fused<T, N, true, true>(p, x, nx, nchan, nseg, r, psd_only, out, st, sa)
+                           : launch_stft_fused<T, N, false, true>(p, x, nx, nchan, nseg, r, psd_only, out, st, sa);
+        });
+    DSP_TRY(generic_prepare(p));
+    return p->f64 ? stft_stream_generic<double>(p, sa, x, nx, nchan, nseg, r, psd_only, out, st)
+                  : stft_stream_generic<float>(p, sa, x, nx, nchan, nseg, r, psd_only, out, st);
+}
+
+// Host twin (returns when the work is done): the chunk and the ldh x nchan histories are staged; the rows of hist_out past
+// the new history are unspecified
+int dspb200_stft_stream_exec(dspb200_spec_plan* plan, const void* hist_in, int64_t nhist, void* hist_out, int64_t ldh,
+                             const void* x, int64_t nx, int64_t nchan, int64_t nseg, double r, int psd_only, void* out,
+                             int64_t ldo) {
+    DSP_RANGE("dspb200_stft_stream_exec");
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    SpecPlanImpl* p = &plan->impl;
+    int64_t newh = 0;
+    bool launch = false;
+    DSP_TRY(stft_stream_check(p, hist_in, nhist, hist_out, ldh, x, nx, nchan, nseg, r, psd_only, out, ldo, false, &newh, &launch));
+    if (!launch) return DSPB200_OK;
+    DSP_TRY(ensure_streams(p));
+    const size_t esz = dtype_size(p->dtype), oel = (psd_only ? 1 : 2) * (p->f64 ? 8 : 4);
+    const size_t hbytes = (size_t)(ldh * nchan) * esz;
+    const size_t obytes = nseg ? (size_t)(((nchan - 1) * ldo + nseg) * p->nout) * oel : 0;
+    return run_staged(p->s_exec, {{x, (size_t)(nx * nchan) * esz, &p->in[0]}, {hist_in, hist_in ? hbytes : 0, &p->hin}},
+                      {{out, obytes, &p->out}, {hist_out, newh ? hbytes : 0, &p->hout}}, [&] {
+                          return dspb200_stft_stream_exec_dev(plan, hist_in ? p->hin.p : nullptr, nhist, p->hout.p, ldh, p->in[0].p,
+                                                              nx, nchan, nseg, r, psd_only, p->out.p, ldo, p->s_exec);
+                      });
+}
+
 // Multitaper (SURVEY.md 8f rank 1; src/multitaper.jl:117-242, 262-404).  The plan's window holds `ntapers` rows of n
 // samples, each PRE-SCALED by 1/sqrt(r_t) (r_t = fs * sum|w_t|^2 / weight_t, :135-139), so that
 //   mt_pgram       = sum_t fft2pow!(FFT(w_t .* s), 1)         (one Welch-style accumulation per taper into one spectrum)
@@ -2003,7 +2288,7 @@ int dspb200_spec_plan_destroy(dspb200_spec_plan* plan) {
     if (p->d_t32) cudaFree(p->d_t32);
     if (p->d_t256) cudaFree(p->d_t256);
     p->partial.release(); p->bpartial.release(); p->bacc.release(); p->segbuf.release(); p->specbuf.release(); p->acc.release();
-    p->in[0].release(); p->in[1].release(); p->out.release(); p->tmp.release();
+    p->in[0].release(); p->in[1].release(); p->out.release(); p->tmp.release(); p->hin.release(); p->hout.release(); p->seam.release();
     if (p->fft_ok) cufftDestroy(p->fft);
     for (int i = 0; i < 2; ++i) {
         if (p->ev_in[i]) cudaEventDestroy(p->ev_in[i]);

@@ -445,3 +445,200 @@ def spectrogram(s, n=None, noverlap=None, onesided=None, nfft=None, fs=1, window
     k = out.shape[1]
     t = (n / 2 + (n - noverlap) * np.arange(k, dtype=np.float64)) / fs               # :835
     return Spectrogram(out, rfftfreq(nfft, fs) if onesided else fftfreq(nfft, fs), t)
+
+
+# --------------------------------------------------------------------------------------------- streaming stft
+
+def stft_stream_step(h, nx, n, noverlap, paired, final=False):
+    """Bookkeeping of one STFTStream call, shared by the host and the device form: with h history samples and nx new
+    ones, the call emits the first `kc` complete segments of the virtual column [history; x] and keeps v[kc*hop, h+nx) as
+    the new history.  `paired` (real input): segments 2u and 2u+1 of the one-shot call share one complex FFT, so kc is
+    even and a complete segment whose partner is not complete yet stays in the history -- except in the `final` call
+    (finish()), which emits it unpaired.  Returns (kc, new h)."""
+    k = arraysplit_count(h + nx, n, noverlap)
+    kc = k - (k & 1) if paired and not final else k
+    return kc, h + nx - kc * (n - noverlap)
+
+
+class STFTStream:
+    """stft / spectrogram of a signal that arrives in chunks (an extension: the reference's stft takes one vector).
+
+    STFTStream(n, noverlap=n>>1, psdonly=False, onesided=None, nfft=nextfastfft(n), fs=1, window=None, device=False) takes
+    the parameters of `stft`.  Every chunk `x` is a vector (nx,) or a column-major (nx, nchan) matrix of channels that share
+    one sample count; `stft(x)` returns the columns the chunk completes -- (nout, kc) or (nout, kc, nchan) -- and for each
+    channel they are exactly (bit for bit) the columns of stft(concatenation of all chunks so far) at the global segment
+    indices nsegments .. nsegments + kc - 1.  For real input the one-shot call transforms segments 2u and 2u+1 as one complex
+    FFT, so a real stream emits segments in those pairs only; `finish()` emits the held-back last segment, if any.  After
+    finish(), further chunks raise ArgumentError until `reset()`.
+
+    device=True: chunks and results are DeviceArrays; a chunk costs at most two kernel launches for power-of-two nfft (the
+    cuFFT sizes take three per batch of segments plus one), no copy of the chunk and no host synchronisation.  `history` is
+    then the current history buffer -- (ldh,) or (ldh, nchan), the first `history_len` rows valid.  A host stream takes host
+    arrays (its `history` is the (history_len,) or (history_len, nchan) array).  A host stream refuses DeviceArrays and a
+    device stream host arrays.  The first chunk fixes the eltype and channel shape; reset() drops them."""
+
+    def __init__(self, n, noverlap=None, psdonly=False, onesided=None, nfft=None, fs=1, window=None, device=False):
+        self.n = int(n)
+        self.noverlap = self.n >> 1 if noverlap is None else int(noverlap)
+        if not (0 <= self.noverlap < self.n):
+            raise DomainError("noverlap must be between zero and n")                     # ArraySplit :44
+        self.nfft = nextfastfft(self.n) if nfft is None else int(nfft)
+        if self.nfft < self.n:
+            raise DomainError("nfft must be >= n")                                        # ArraySplit :45
+        self.hop = self.n - self.noverlap
+        self.psdonly, self.fs, self.device = bool(psdonly), fs, bool(device)
+        self._onesided_arg = onesided
+        self.window, norm2 = compute_window(window, self.n)
+        self.r = fs * norm2
+        self._plans = {}
+        self.reset()
+
+    def reset(self):
+        """Start a new stream: drops the history, the segment count, the eltype and the channel shape."""
+        self.nsegments = 0
+        self.history_len = 0
+        self.history = None
+        self._key = None             # (eltype, channel shape) fixed by the first chunk
+        self._hist = None            # [current, next] history buffers
+        self._finished = False
+        return self
+
+    # ---- first chunk: eltype, onesided, plan
+    def _setup(self, dt, chan_shape):
+        cplx = dt.kind == "c"
+        onesided = (not cplx) if self._onesided_arg is None else bool(self._onesided_arg)
+        if onesided and cplx:
+            raise ArgumentError("cannot compute one-sided FFT of a complex signal")      # :876
+        if dt not in self._plans:
+            self._plans[dt] = _lib.SpecPlan(dt, self.n, self.noverlap, self.nfft, onesided, self.window)
+        self.onesided, self.cplx = onesided, cplx
+        self.nout = self.nfft // 2 + 1 if onesided else self.nfft
+        self.odt = fftabs2type(dt) if self.psdonly else fftouttype(dt)
+        # history capacity: n + hop - 1 samples for real input (a held-back segment), n - 1 for complex
+        self.ldh = max(1, self.n - 1 + (0 if cplx else self.hop))
+        self._key = (dt, chan_shape)
+
+    def _check(self, x):
+        if self.device and not isinstance(x, DeviceArray):
+            raise ArgumentError("a device STFTStream takes DeviceArrays (construct it without device=True for host arrays)")
+        if not self.device and isinstance(x, DeviceArray):
+            raise ArgumentError("a host STFTStream takes host arrays (construct it with device=True for DeviceArrays)")
+        if self._finished:
+            raise ArgumentError("the stream is finished: reset() starts a new one")
+        if not self.device:
+            x = np.asarray(x)
+        if x.ndim not in (1, 2):
+            raise ArgumentError("an STFTStream chunk is a vector or a len x nchan matrix")
+        dt = x.dtype if self.device else fftintype(x.dtype)
+        if self.device and dt != fftintype(dt):
+            raise ArgumentError("device chunks must be Float32, Float64, ComplexF32 or ComplexF64")
+        key = (np.dtype(dt), tuple(x.shape[1:]))
+        if self._key is None:
+            self._setup(key[0], key[1])
+        elif key != self._key:
+            raise ArgumentError(f"this STFTStream streams {self._key[0]} chunks of channel shape {self._key[1]}; got "
+                                f"{key[0]} {key[1]} (reset() starts a new stream)")
+        if not self.device:
+            x = np.asfortranarray(x, dtype=dt)
+        return x
+
+    def _out_shape(self, cols):
+        return (self.nout, cols) + self._key[1]
+
+    def _run(self, x, nseg, out, ldo):
+        """One library call on chunk x (nx may be 0): nseg segments into out (ldo columns per channel), then the swap of the
+        history buffers."""
+        nx = x.shape[0] if x is not None else 0
+        nchan = int(np.prod(self._key[1])) if self._key[1] else 1
+        plan = self._plans[self._key[0]]
+        h = self.history_len
+        newh = h + nx - nseg * self.hop
+        if nchan and (nx or nseg):
+            if self._hist is None:
+                hshape = (self.ldh,) + self._key[1]
+                self._hist = ([None, DeviceArray(hshape, self._key[0])] if self.device
+                              else [None, np.zeros(hshape, dtype=self._key[0], order="F")])
+            cur, nxt = self._hist
+            if self.device:
+                plan.stft_stream_dev(cur.ptr if cur is not None else None, h, nxt.ptr, self.ldh,
+                                     x.ptr if x is not None else None, nx, nchan, nseg, self.r, self.psdonly,
+                                     out.ptr if out is not None else None, ldo, 0)
+            else:
+                xx = x if x is not None else np.zeros((1,) + self._key[1], dtype=self._key[0], order="F")
+                oo = out if out is not None else np.zeros(1, dtype=self.odt)
+                plan.stft_stream(cur, h, nxt, self.ldh, xx, nx, nchan, nseg, self.r, self.psdonly, oo, ldo)
+            if cur is None:                                 # the first call: an empty history in, none to reuse
+                cur = (DeviceArray(nxt.shape, nxt.dtype) if self.device
+                       else np.zeros(nxt.shape, dtype=nxt.dtype, order="F"))
+            self._hist = [nxt, cur]
+        self.history_len = newh
+        if self._hist is not None:
+            self.history = self._hist[0] if self.device else self._hist[0][:newh]
+        self.nsegments += nseg
+
+    def _chunk(self, x, out=None):
+        fresh = self._key is None
+        x = self._check(x)
+        try:
+            return self._emit(x, out)
+        except ArgumentError:
+            if fresh:                   # a refused first call leaves the stream as it was: no eltype or channel shape fixed
+                self._key = None
+            raise
+
+    def _emit(self, x, out):
+        kc, _ = stft_stream_step(self.history_len, x.shape[0], self.n, self.noverlap, not self.cplx)
+        if out is None:
+            out = (DeviceArray if self.device else (lambda s, d: np.zeros(s, dtype=d, order="F")))(self._out_shape(kc), self.odt)
+            ldo = kc
+        else:
+            if self.device != isinstance(out, DeviceArray):
+                raise ArgumentError("out must be a DeviceArray for a device STFTStream and a host array for a host one")
+            if out.dtype != self.odt or out.ndim != 2 + len(self._key[1]) or out.shape[0] != self.nout or \
+                    tuple(out.shape[2:]) != self._key[1]:
+                raise ArgumentError(f"out must be a {self.odt} array of shape (nout = {self.nout}, >= {kc}) + {self._key[1]}")
+            if out.shape[1] < kc:
+                raise ArgumentError(f"out is too small: the chunk completes {kc} columns per channel, out holds {out.shape[1]}")
+            if self.device:
+                if out.overlaps(x) or (self._hist is not None and (out.overlaps(self._hist[0]) or out.overlaps(self._hist[1]))):
+                    raise ArgumentError("out must not overlap the chunk or the stream's history")
+            elif not out.flags.f_contiguous:
+                raise ArgumentError("out must be Fortran-ordered (column-major)")
+            ldo = out.shape[1]
+        self._run(x if x.shape[0] else None, kc, out, ldo)
+        return out, kc
+
+    def stft(self, x):
+        """The columns chunk x completes: (nout, kc) for a vector chunk, (nout, kc, nchan) for a matrix chunk."""
+        return self._chunk(x)[0]
+
+    def stft_(self, out, x):
+        """stft(x) into `out`, whose second dimension holds at least kc columns; returns kc."""
+        return self._chunk(x, out)[1]
+
+    def spectrogram(self, x):
+        """Spectrogram(power, freq, time) of the columns chunk x completes (psdonly streams): time of global segment g is
+        (n/2 + g*hop)/fs, as in spectrogram (src/periodograms.jl:835)."""
+        if not self.psdonly:
+            raise ArgumentError("spectrogram() needs a psdonly STFTStream")
+        g0 = self.nsegments
+        p = self.stft(x)
+        return Spectrogram(p, rfftfreq(self.nfft, self.fs) if self.onesided else fftfreq(self.nfft, self.fs),
+                           self._times(g0, p.shape[1]))
+
+    def _times(self, g0, kc):
+        return (self.n / 2 + self.hop * np.arange(g0, g0 + kc, dtype=np.float64)) / self.fs
+
+    def finish(self):
+        """The held-back last segment of a real stream (0 or 1 column per channel, transformed unpaired as the one-shot call
+        does when it has an odd number of segments); None before the first chunk.  Ends the stream until reset()."""
+        if self._key is None:
+            return None
+        if self._finished:
+            raise ArgumentError("the stream is finished: reset() starts a new one")
+        kc, _ = stft_stream_step(self.history_len, 0, self.n, self.noverlap, not self.cplx, final=True)
+        out = (DeviceArray if self.device else (lambda s, d: np.zeros(s, dtype=d, order="F")))(self._out_shape(kc), self.odt)
+        if kc:
+            self._run(None, kc, out, kc)
+        self._finished = True
+        return out

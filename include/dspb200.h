@@ -246,6 +246,25 @@ DSPB200_API int dspb200_stft_exec(dspb200_spec_plan* plan, const void* s, int64_
                       void* out);
 DSPB200_API int dspb200_stft_exec_dev(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, double r, int psd_only,
                           void* out, void* stream);
+/* Streaming stft / spectrogram (an extension; the reference's stft takes one vector).  Every channel c has the virtual column
+ * v = [hist_in[:, c] (nhist samples); x[:, c] (nx samples)]; hist_in / hist_out are ldh x nchan, x is nx x nchan (all
+ * column-major).  The call emits segments 0 .. nseg-1 of each v (segment s starts at s*hop) -- column s of channel c at
+ * out + (c*ldo + s)*nout, ldo >= nseg -- then writes the new history v[nseg*hop, nhist + nx) to hist_out.  hist_in == NULL:
+ * an empty history.  psd_only: 0 raw spectra, 1 PSD columns scaled with r = fs*norm2 (no accumulate form).  Real input:
+ * segments 2u and 2u+1 are transformed together, as the one-shot call pairs them, and an odd nseg transforms the last one
+ * alone; so a stream whose calls start at even global segments reproduces stft of the concatenated signal bit for bit.  The
+ * plan is the one an aligned one-shot call runs, whatever the alignment of the history or chunk.  DSPB200_EINVALID, before
+ * any launch, when hist_out overlaps hist_in, x or out, when out overlaps x or a history buffer, when ldo < nseg, when
+ * (nseg-1)*hop + n > nhist + nx, or when the new history would exceed ldh.  nx == 0 with nseg == 0 launches nothing and
+ * leaves hist_out as it was (the history is still hist_in).  Fused sizes: at most two launches; cuFFT sizes: three per
+ * batch of (channel, segment) pairs plus the history. */
+DSPB200_API int dspb200_stft_stream_exec_dev(dspb200_spec_plan* plan, const void* hist_in, int64_t nhist, void* hist_out, int64_t ldh,
+                                             const void* x, int64_t nx, int64_t nchan, int64_t nseg, double r, int psd_only,
+                                             void* out, int64_t ldo, void* stream);
+/* host pointers; hist_in / hist_out hold ldh x nchan elements, the rows of hist_out past the new history are unspecified */
+DSPB200_API int dspb200_stft_stream_exec(dspb200_spec_plan* plan, const void* hist_in, int64_t nhist, void* hist_out, int64_t ldh,
+                                         const void* x, int64_t nx, int64_t nchan, int64_t nseg, double r, int psd_only,
+                                         void* out, int64_t ldo);
 /* arraysplit(s, n, noverlap, nfft, window) / ArraySplit: src/periodograms.jl:32-73, 134-137.  out = k x nfft matrix, row i =
  * [window .* s[i*hop .. i*hop+n) ; zeros(nfft-n)] (the reference yields the rows one at a time into one reused buffer). */
 DSPB200_API int dspb200_arraysplit_exec(dspb200_spec_plan* plan, const void* s, int64_t len, void* out);
