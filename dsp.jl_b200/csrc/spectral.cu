@@ -14,9 +14,10 @@
 //   * STFT / spectrogram: the spectrum is parked in shared memory (natural order), un-mixed per bin and
 //     stored column by column, coalesced along frequency.
 // Generic path (any other nfft): segment/window kernel -> batched cuFFT -> power / store kernels.
-// Streaming STFT (dspb200_stft_stream_exec(_dev)): the STREAM instances of the two STFT kernels read each channel's virtual
-// column [history; chunk] (StftStream) after stft_stream_edge_kernel has copied the seam samples and written the new history;
-// cuFFT sizes run the (channel, segment) pairs of a call through stft_stream_seg_kernel -> cuFFT -> stft_stream_store_kernel.
+// STFT: one-shot and streaming calls (dspb200_stft_stream_exec(_dev)) run the same kernels over each channel's virtual column
+// [history; chunk] (StftStream; a one-shot call has no history), a stream after stft_stream_edge_kernel has copied the seam
+// samples and written the new history; cuFFT sizes run a call's (channel, segment) pairs through stft_seg_kernel -> cuFFT ->
+// stft_store_kernel.
 #include "fft_core.cuh"
 #include "async_copy.cuh"
 #include <cufft.h>
@@ -441,13 +442,12 @@ __device__ __forceinline__ void stft_emit(const cx<T>* __restrict__ sm, void* __
     }
 }
 
-// Streaming STFT (dspb200_stft_stream_exec_dev): a call transforms segments 0 .. k - 1 of every channel's virtual column
-// v = [history (h samples); x].  A unit that starts in the history (a seam unit) reads the copy of v's first samples that the
-// call's edge kernel wrote to `seam` (stft_stream_edge_kernel); every other unit reads x + start - h.  Either way a unit's
-// samples are one contiguous range, staged by TMA or loaded directly exactly as in the one-shot call, so the same values
-// enter the same butterflies.  The one-shot instances take the empty struct, so their parameters and code are those of before.
-template <typename In, bool STREAM> struct StftStream {};
-template <typename In> struct StftStream<In, true> {
+// An STFT call transforms segments 0 .. k - 1 of every channel's virtual column v = [history (h samples); x]; a one-shot call
+// is one with h = 0 and ldo = k.  A unit that starts in the history (a seam unit) reads the copy of v's first samples that
+// the call's edge kernel wrote to `seam` (stft_stream_edge_kernel); every other unit reads x + start - h.  Either way a
+// unit's samples are one contiguous range, staged by TMA or loaded directly, so a stream puts the same values into the same
+// butterflies as one call over the concatenated signal.
+template <typename In> struct StftStream {
     const In* seam;             // lds x nchan: v[0, lds) of every channel (the samples of its seam units)
     int64_t lds, h;             // column stride of `seam`, samples of history
     int64_t ldo;                // output columns per channel (replaces k as the column stride)
@@ -515,14 +515,14 @@ __device__ __forceinline__ void stft_unit(const FftCtx<T>& ctx, cx<T>* sm, int t
 // (tried: compiling the Float32 STFT kernels for 768 resident threads per SM -- the 1024-point kernel fits 64 registers and
 //  gets 11 CTAs per SM instead of 8 -- but the spectrogram got slower and the windowed variants spill; kept at 512 threads /
 //  128 registers)
-// STREAM: a streaming call (StftStream): s_ is the chunk x (chan_stride = nx), k the call's segments per channel; a
-// unit's samples come from StftStream::src and its columns are ldo apart.
-template <typename T, int N, bool CPLX, bool TMA, int WIN, bool STREAM>
+// s_ is the chunk x (chan_stride = its column length), k the call's segments per channel; a unit's samples come from
+// StftStream::src and its columns are ldo apart.
+template <typename T, int N, bool CPLX, bool TMA, int WIN>
 __global__ void __launch_bounds__(fft_threads<N>::value, fft_minblocks<T, N>::value)
 stft_fused_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int64_t units_per_chan, int64_t total_units,
                   int64_t hop, int n, const typename win_t<T>::type* __restrict__ win, const cx<T>* __restrict__ tw,
                   const cx<T>* __restrict__ g16, const cx<T>* __restrict__ g256, void* __restrict__ out_, int nout,
-                  int psd_only, int onesided, T m1, T m2, const StftStream<typename in_type<T, CPLX>::type, STREAM> ss) {
+                  int psd_only, int onesided, T m1, T m2, const StftStream<typename in_type<T, CPLX>::type> ss) {
     constexpr int NT = fft_threads<N>::value;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     cx<T>* sm = reinterpret_cast<cx<T>*>(smem_raw);
@@ -539,10 +539,7 @@ stft_fused_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, i
     // (channel, unit inside the channel) of the current unit, advanced incrementally: no 64-bit division in the loop
     int64_t chan = u0 < u1 ? u0 / units_per_chan : 0;
     int64_t uin = u0 < u1 ? u0 - chan * units_per_chan : 0;
-    auto src_of = [&](int64_t c, int64_t u) -> const In* {
-        if constexpr (STREAM) return ss.src(s, chan_stride, c, (CPLX ? u : 2 * u) * hop);
-        else return s + c * chan_stride + (CPLX ? u : 2 * u) * hop;
-    };
+    auto src_of = [&](int64_t c, int64_t u) -> const In* { return ss.src(s, chan_stride, c, (CPLX ? u : 2 * u) * hop); };
     auto bytes_of = [&](int64_t u) -> uint32_t {
         const bool hb = !CPLX && (2 * u + 1 < k);
         return (uint32_t)((hb ? hop + n : n) * sizeof(In));
@@ -583,9 +580,7 @@ stft_fused_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, i
                 }
             }
         };
-        int64_t colA;
-        if constexpr (!STREAM) colA = (chan * k + segA) * (int64_t)nout;
-        else colA = (chan * ss.ldo + segA) * (int64_t)nout;     // the caller's output stride
+        const int64_t colA = (chan * ss.ldo + segA) * (int64_t)nout;
         if (full && (CPLX || hasB))
             stft_unit<T, N, CPLX, TMA, WIN, true>(ctx, sm, tid, pa, hop, n, hasB, win, out_, colA, nout, psd_only, onesided, m1, m2, issue_next);
         else
@@ -617,14 +612,14 @@ inline void fill_t32(cx<float>* t32) {
 __host__ __device__ inline size_t warp_bytes(int64_t stage_elems, size_t elt) { return (((size_t)DATA_LEN * 8 + (size_t)stage_elems * elt + 15) & ~(size_t)15) + 16; }
 }  // namespace w1k
 
-// STREAM: a streaming call (StftStream, as stft_fused_kernel).  A stream keeps this plan whatever the alignment of the call:
-// ss.tma = 0 (unaligned) reads every unit directly from global memory in the first pass instead of staging it.
-template <bool CPLX, int WIN, int WARPS, bool STREAM>
+// Arguments as stft_fused_kernel.  A stream keeps this plan whatever the alignment of the call: ss.tma = 0 (unaligned) reads
+// every unit directly from global memory in the first pass instead of staging it.
+template <bool CPLX, int WIN, int WARPS>
 __global__ void __launch_bounds__(32 * WARPS)
 stft_w1k_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int64_t units_per_chan, int64_t total_units,
                 int64_t hop, int n, const float2* __restrict__ win, const cx<float>* __restrict__ g32, void* __restrict__ out_,
                 int nout, int psd_only, int onesided, float m1, float m2,
-                const StftStream<typename in_type<float, CPLX>::type, STREAM> ss) {
+                const StftStream<typename in_type<float, CPLX>::type> ss) {
     using T = float;
     using In = typename in_type<T, CPLX>::type;
     constexpr int N = w1k::N;
@@ -656,24 +651,14 @@ stft_w1k_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int
     const int64_t u1 = u0 + per < total_units ? u0 + per : total_units;
     int64_t chan = u0 < u1 ? u0 / units_per_chan : 0;
     int64_t uin = u0 < u1 ? u0 - chan * units_per_chan : 0;
-    auto src_of = [&](int64_t c, int64_t u) -> const In* {
-        if constexpr (STREAM) return ss.src(s, chan_stride, c, (CPLX ? u : 2 * u) * hop);
-        else return s + c * chan_stride + (CPLX ? u : 2 * u) * hop;
-    };
+    auto src_of = [&](int64_t c, int64_t u) -> const In* { return ss.src(s, chan_stride, c, (CPLX ? u : 2 * u) * hop); };
     auto bytes_of = [&](int64_t u) -> uint32_t {
         const bool hb = !CPLX && (2 * u + 1 < k);
         return (uint32_t)((hb ? hop + n : n) * sizeof(In));
     };
-    if constexpr (!STREAM) {
-        if (lane == 0 && u0 < u1) {
-            mbar_expect_tx(bar, bytes_of(uin));
-            tma_load_1d(stage, src_of(chan, uin), bytes_of(uin), bar);
-        }
-    } else {
-        if (lane == 0 && u0 < u1 && ss.tma) {
-            mbar_expect_tx(bar, bytes_of(uin));
-            tma_load_1d(stage, src_of(chan, uin), bytes_of(uin), bar);
-        }
+    if (lane == 0 && u0 < u1 && ss.tma) {
+        mbar_expect_tx(bar, bytes_of(uin));
+        tma_load_1d(stage, src_of(chan, uin), bytes_of(uin), bar);
     }
     uint32_t parity = 0;
     const bool full = (n == N);
@@ -687,50 +672,39 @@ stft_w1k_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int
         const bool hasB = !CPLX && (segA + 1 < k);
         int64_t nchan = chan, nuin = uin + 1;
         if (nuin == units_per_chan) { nuin = 0; ++nchan; }
-        if constexpr (!STREAM) {
+        if (ss.tma) {
             mbar_wait(bar, parity);
             parity ^= 1;
-        } else {
-            if (ss.tma) {
-                mbar_wait(bar, parity);
-                parity ^= 1;
-            }
         }
-        const In* pa = stage;
-        if constexpr (STREAM) {
-            if (!ss.tma) pa = src_of(chan, uin);       // an unaligned streaming call reads its units directly
-        }
-        const In* pb = pa + hop;
-        // first pass: plain 32-point DFT of x[lane + 32 m] (window applied), 32 contiguous slots at block `lane`
+        // first pass: plain 32-point DFT of x[lane + 32 m] (window applied), 32 contiguous slots at block `lane`.  Written
+        // out once per source, so that a staged unit is read by shared-memory loads (through a pointer that may point to
+        // either space they become generic loads); an unaligned streaming call reads its units directly
         cx<T> v[32];
         const bool fast = full && (CPLX || hasB);
+        auto first_pass = [&](const In* pa) {
+            const In* pb = pa + hop;
 #pragma unroll
-        for (int m = 0; m < 32; ++m) {
-            const int j = lane + 32 * m;
-            if constexpr (CPLX) {
-                cx<T> x = (fast || j < n) ? pa[j] : mkc<T>(0.f, 0.f);
-                if constexpr (WIN != 0) { const float2 w = wsm[fast || j < n ? j : 0]; x = mkc<T>(win_mul(x.x, w), win_mul(x.y, w)); }
-                v[m] = x;
-            } else {
-                float a = (fast || j < n) ? pa[j] : 0.f;
-                float b = (fast || (hasB && j < n)) ? pb[j] : 0.f;
-                if constexpr (WIN != 0) { const float2 w = wsm[fast || j < n ? j : 0]; a = win_mul(a, w); b = win_mul(b, w); }
-                v[m] = mkc<T>(a, b);
+            for (int m = 0; m < 32; ++m) {
+                const int j = lane + 32 * m;
+                if constexpr (CPLX) {
+                    cx<T> x = (fast || j < n) ? pa[j] : mkc<T>(0.f, 0.f);
+                    if constexpr (WIN != 0) { const float2 w = wsm[fast || j < n ? j : 0]; x = mkc<T>(win_mul(x.x, w), win_mul(x.y, w)); }
+                    v[m] = x;
+                } else {
+                    float a = (fast || j < n) ? pa[j] : 0.f;
+                    float b = (fast || (hasB && j < n)) ? pb[j] : 0.f;
+                    if constexpr (WIN != 0) { const float2 w = wsm[fast || j < n ? j : 0]; a = win_mul(a, w); b = win_mul(b, w); }
+                    v[m] = mkc<T>(a, b);
+                }
             }
-        }
-        __syncwarp();                                   // every lane has read the staging buffer (and the previous unit's spectrum)
-        if constexpr (!STREAM) {
-            if (lane == 0 && gu + 1 < u1) {             // refill it with the next unit while this one is transformed
-                fence_proxy_async_shared();
-                mbar_expect_tx(bar, bytes_of(nuin));
-                tma_load_1d(stage, src_of(nchan, nuin), bytes_of(nuin), bar);
-            }
-        } else {
-            if (lane == 0 && gu + 1 < u1 && ss.tma) {
-                fence_proxy_async_shared();
-                mbar_expect_tx(bar, bytes_of(nuin));
-                tma_load_1d(stage, src_of(nchan, nuin), bytes_of(nuin), bar);
-            }
+        };
+        if (ss.tma) first_pass(stage);
+        else first_pass(src_of(chan, uin));
+        __syncwarp();                                  // every lane has read the staging buffer (and the previous unit's spectrum)
+        if (lane == 0 && gu + 1 < u1 && ss.tma) {       // refill it with the next unit while this one is transformed
+            fence_proxy_async_shared();
+            mbar_expect_tx(bar, bytes_of(nuin));
+            tma_load_1d(stage, src_of(nchan, nuin), bytes_of(nuin), bar);
         }
         fft_bfly<T, 32, true>(v, nullptr);
         {
@@ -750,9 +724,7 @@ stft_w1k_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int
         }
         __syncwarp();
         // emit: bins kk = lane + 32 i; N - kk = (32 - lane) + 32 (31 - i) for lane > 0
-        int64_t colA;
-        if constexpr (!STREAM) colA = (chan * k + segA) * (int64_t)nout;
-        else colA = (chan * ss.ldo + segA) * (int64_t)nout;     // the caller's output stride
+        const int64_t colA = (chan * ss.ldo + segA) * (int64_t)nout;
         const cx<T>* pk = sm + w1k::pad(lane);
         const cx<T>* pm = lane ? sm + w1k::pad(32 - lane) : sm;
         const bool half = !CPLX && onesided;
@@ -851,27 +823,7 @@ __global__ void pow_finalize_kernel(const double* __restrict__ acc, int64_t nbin
     out[k] = (T)(acc[src] * m);
 }
 
-// STFT store from a batch of spectra X[b][nbins_fft] into columns of out (nout x k)
-template <typename T>
-__global__ void stft_store_kernel(const cx<T>* __restrict__ X, int64_t nbins_fft, int64_t nfft, int64_t nout,
-                                  int64_t nseg, int psd_only, int onesided, T m1, T m2, void* __restrict__ out_,
-                                  int64_t col0) {
-    const int64_t total = nseg * nout;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t b = i / nout, k = i - b * nout;
-        const bool mirrored = k >= nbins_fft;
-        const cx<T> z = X[b * nbins_fft + (mirrored ? nfft - k : k)];
-        if (psd_only) {
-            T m = m1;
-            if (onesided && k != 0 && !(k == nbins_fft - 1 && (nfft % 2 == 0))) m = m2;
-            reinterpret_cast<T*>(out_)[(col0 + b) * nout + k] = cabs2(z) * m;
-        } else {
-            reinterpret_cast<cx<T>*>(out_)[(col0 + b) * nout + k] = mirrored ? cconj(z) : z;
-        }
-    }
-}
-
-// ---------------------------------------------------------------------------------------------- streaming STFT, small kernels
+// ---------------------------------------------------------------------------------------------- STFT, small kernels
 // Launch 1 of a streaming call, one grid-stride pass over nchan x (ls + hn) items: (a) seam[c lds + i] = v_c[i], i < ls --
 // the samples of the units that start in the history, contiguous, so that the transform reads every unit from one range;
 // (b) the new history hist_out[c ldh + i] = v_c[skip + i], i < hn.  v_c = [hist_in (h samples, column stride ldh); x_c].
@@ -889,14 +841,14 @@ __global__ void stft_stream_edge_kernel(const E* __restrict__ hist_in, int64_t h
     }
 }
 
-// Streaming calls, cuFFT sizes: the call's nchan x k (channel c, segment j) pairs, f = c k + j, fill the cuFFT batch in
+// STFT calls, cuFFT sizes: the call's nchan x k (channel c, segment j) pairs, f = c k + j, fill the cuFFT batch in
 // order.  Slot b = blockIdx.y holds pair f0 + b: buf[b][i] = window[i] * v_c[j hop + i] (i < n), 0 for n <= i < nfft and
 // for slots past the list -- seg_window_kernel's values, read from the virtual column.  One slot per grid row: the pair is
 // resolved once per block, not per element.
 template <typename T, bool CPLX>
-__global__ void stft_stream_seg_kernel(const void* __restrict__ hist_, int64_t h, int64_t ldh, const void* __restrict__ x_,
-                                       int64_t nx, int64_t f0, int64_t nf, int64_t k, int64_t hop, int64_t n, int64_t nfft,
-                                       const typename win_t<T>::type* __restrict__ win, void* __restrict__ buf_) {
+__global__ void stft_seg_kernel(const void* __restrict__ hist_, int64_t h, int64_t ldh, const void* __restrict__ x_,
+                                int64_t nx, int64_t f0, int64_t nf, int64_t k, int64_t hop, int64_t n, int64_t nfft,
+                                const typename win_t<T>::type* __restrict__ win, void* __restrict__ buf_) {
     using In = typename in_type<T, CPLX>::type;
     const In* hist = reinterpret_cast<const In*>(hist_);
     const In* x = reinterpret_cast<const In*>(x_);
@@ -918,10 +870,11 @@ __global__ void stft_stream_seg_kernel(const void* __restrict__ hist_, int64_t h
     }
 }
 
-// stft_store_kernel's values for the spectra of pairs f0 .. f0 + nf - 1 (slot b = blockIdx.y), into column (c ldo + j) of out
+// The spectra of pairs f0 .. f0 + nf - 1 (slot b = blockIdx.y) into column (c ldo + j) of out: raw (the real two-sided
+// mirror conjugated), or PSD (fft2pow! scaling, :142-172)
 template <typename T>
-__global__ void stft_stream_store_kernel(const cx<T>* __restrict__ X, int64_t nbins_fft, int64_t nfft, int64_t nout, int64_t f0,
-                                         int64_t k, int64_t ldo, int psd_only, int onesided, T m1, T m2, void* __restrict__ out_) {
+__global__ void stft_store_kernel(const cx<T>* __restrict__ X, int64_t nbins_fft, int64_t nfft, int64_t nout, int64_t f0,
+                                  int64_t k, int64_t ldo, int psd_only, int onesided, T m1, T m2, void* __restrict__ out_) {
     const int64_t b = blockIdx.y, f = f0 + b, c = f / k, col = c * ldo + (f - c * k);
     const cx<T>* Xb = X + b * nbins_fft;
     for (int64_t kk = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; kk < nout; kk += (int64_t)gridDim.x * blockDim.x) {
@@ -1257,21 +1210,24 @@ static int launch_welch_batch(SpecPlanImpl* p, const void* s, int64_t len, int64
     return DSPB200_OK;
 }
 
-// The history side of a streaming call (dspb200_stft_stream_exec_dev); the one-shot call passes none
-// (seam, lds: the copy of every channel's first virtual-column samples that the edge kernel wrote; fused sizes only)
-struct StftStreamArgs { const void* hist = nullptr; int64_t h = 0, ldh = 0, ldo = 0; const void* seam = nullptr; int64_t lds = 0; };
+// The history side of an STFT call (dspb200_stft_stream_exec_dev); a one-shot call has none and ldo = k
+// (seam, lds: the copy of every channel's first virtual-column samples that the edge kernel wrote; fused sizes only).
+// keep_plan: run the instance an aligned call of the plan runs, whatever the alignment of this call (streams)
+struct StftStreamArgs {
+    const void* hist = nullptr; int64_t h = 0, ldh = 0, ldo = 0; const void* seam = nullptr; int64_t lds = 0;
+    bool keep_plan = false;
+};
 
-// One-shot call (STREAM = false): k segments of each of the nchan columns of the len x nchan matrix s.  Streaming call: k
-// segments of each channel's virtual column [history; s], s being the nx = len x nchan chunk.  A stream runs the instance an
-// aligned one-shot call of the same plan runs, whatever the alignment of its history or chunk: stft_w1k_kernel rounds
-// differently from stft_fused_kernel, and the two TMA / direct instances of stft_fused_kernel round alike.
-template <typename T, int N, bool CPLX, bool STREAM = false>
+// k segments of each channel's virtual column [history; s], s being the len x nchan chunk (one-shot: the whole matrix).  A
+// stream keeps its plan's instance (sa.keep_plan): stft_w1k_kernel rounds differently from stft_fused_kernel, and the two
+// TMA / direct instances of stft_fused_kernel round alike.  A one-shot Float32 1024-point call runs stft_w1k_kernel only
+// when it meets the TMA alignment conditions.
+template <typename T, int N, bool CPLX>
 static int launch_stft_fused(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan, int64_t k, double r,
-                             int psd_only, void* out, cudaStream_t st, const StftStreamArgs& sa = StftStreamArgs()) {
+                             int psd_only, void* out, cudaStream_t st, const StftStreamArgs& sa) {
     constexpr int NT = fft_threads<N>::value;
     using In = typename in_type<T, CPLX>::type;
-    using SS = StftStream<In, STREAM>;
-    SS ss{};
+    using SS = StftStream<In>;
     const size_t base = (size_t)fft_smem_elems<T, N>() * sizeof(cx<T>);
     const size_t stage = (size_t)(CPLX ? p->n : p->hop + p->n) * sizeof(In) + 16;
     // Float32, N = 1024: every call that meets the TMA alignment conditions runs stft_w1k_kernel (its shared memory is at
@@ -1280,24 +1236,24 @@ static int launch_stft_fused(SpecPlanImpl* p, const void* s, int64_t len, int64_
     const bool plan_aligned = ((p->hop * sizeof(In)) % 16 == 0) && ((p->n * sizeof(In)) % 16 == 0);
     // the TMA alignment conditions: 16-byte aligned unit starts (streaming: x + start - h) and sizes
     const bool aligned = plan_aligned && ((uintptr_t)s % 16 == 0) && ((len * sizeof(In)) % 16 == 0 || nchan == 1) &&
-                         (!STREAM || (sa.h * sizeof(In)) % 16 == 0);
+                         (sa.h * sizeof(In)) % 16 == 0;
     const bool tma = !W1K && aligned &&
                      (base + stage <= p->smem_optin) && (base + stage <= 100 * 1024 || N >= 8192);   // N >= 8192: one CTA per SM anyway
     const size_t smem = tma ? base + stage : base;
     const int64_t upc = CPLX ? k : (k + 1) / 2;
     const int64_t units = upc * nchan;
     if (units < 1) return DSPB200_OK;
-    if constexpr (STREAM) ss = SS{reinterpret_cast<const In*>(sa.seam), sa.lds, sa.h, sa.ldo, (W1K ? aligned : tma) ? 1 : 0};
+    const SS ss{reinterpret_cast<const In*>(sa.seam), sa.lds, sa.h, sa.ldo, (W1K ? aligned : tma) ? 1 : 0};
     const auto* w = reinterpret_cast<const typename win_t<T>::type*>(p->d_window);
     if constexpr (W1K) {
         // one warp per unit (stft_w1k_kernel): a one-shot call needs the TMA alignment conditions, a stream those of its plan
-        if ((STREAM ? plan_aligned : aligned) && p->d_t32 != nullptr) {
+        if ((sa.keep_plan ? plan_aligned : aligned) && p->d_t32 != nullptr) {
             constexpr int WARPS = 4;
             const size_t smem1 = (size_t)w1k::T32_LEN * sizeof(cx<float>) + (w ? (size_t)p->n * sizeof(float2) : 0) +
                                  (size_t)WARPS * w1k::warp_bytes(CPLX ? p->n : p->hop + p->n, sizeof(In));
             using K1 = void (*)(const void*, int64_t, int64_t, int64_t, int64_t, int64_t, int, const float2*, const cx<float>*, void*, int,
                                 int, int, float, float, SS);
-            K1 k1 = w ? (K1)stft_w1k_kernel<CPLX, 1, WARPS, STREAM> : (K1)stft_w1k_kernel<CPLX, 0, WARPS, STREAM>;
+            K1 k1 = w ? (K1)stft_w1k_kernel<CPLX, 1, WARPS> : (K1)stft_w1k_kernel<CPLX, 0, WARPS>;
             if (smem1 <= p->smem_optin) {
                 DSP_TRY(set_smem(k1, smem1));
                 int per = 1;
@@ -1322,12 +1278,12 @@ static int launch_stft_fused(SpecPlanImpl* p, const void* s, int64_t len, int64_
     constexpr bool SPEC = sizeof(T) == 4;
     Kern kern;
     if constexpr (W1K) {
-        kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, false, 1, STREAM> : (Kern)stft_fused_kernel<T, N, CPLX, false, 0, STREAM>;
+        kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, false, 1> : (Kern)stft_fused_kernel<T, N, CPLX, false, 0>;
     } else if constexpr (SPEC) {
-        if (tma) kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, true, 1, STREAM> : (Kern)stft_fused_kernel<T, N, CPLX, true, 0, STREAM>;
-        else kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, false, 1, STREAM> : (Kern)stft_fused_kernel<T, N, CPLX, false, 0, STREAM>;
+        if (tma) kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, true, 1> : (Kern)stft_fused_kernel<T, N, CPLX, true, 0>;
+        else kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, false, 1> : (Kern)stft_fused_kernel<T, N, CPLX, false, 0>;
     } else {
-        kern = tma ? (Kern)stft_fused_kernel<T, N, CPLX, true, -1, STREAM> : (Kern)stft_fused_kernel<T, N, CPLX, false, -1, STREAM>;
+        kern = tma ? (Kern)stft_fused_kernel<T, N, CPLX, true, -1> : (Kern)stft_fused_kernel<T, N, CPLX, false, -1>;
     }
     DSP_TRY(set_smem(kern, smem));
     int per_sm = 1;
@@ -1451,28 +1407,9 @@ template <typename T> static int welch_generic_acc(SpecPlanImpl* p, const void* 
     return DSPB200_OK;
 }
 
-template <typename T> static int stft_generic(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan, int64_t k,
-                                               double r, int psd_only, void* out, cudaStream_t st) {
-    for (int64_t c = 0; c < nchan; ++c) {
-        for (int64_t b0 = 0; b0 < k; b0 += p->batch) {
-            const int64_t nseg = k - b0 < p->batch ? k - b0 : p->batch;
-            DSP_TRY(generic_segments<T>(p, s, c * len + b0 * p->hop, nseg, st));
-            const int64_t total = nseg * p->nout;
-            const int threads = 256;
-            const int grid = (int)(cdiv(total, threads) < 65535 * 8 ? cdiv(total, threads) : 65535 * 8);
-            stft_store_kernel<T><<<grid, threads, 0, st>>>(reinterpret_cast<const cx<T>*>(p->specbuf.p), p->nbins_fft,
-                                                           p->nfft, p->nout, nseg, psd_only, p->onesided, (T)(1.0 / r),
-                                                           (T)(2.0 / r), out, c * k + b0);
-            DSP_LAUNCH_OK();
-        }
-    }
-    return DSPB200_OK;
-}
-
-// Streaming call, cuFFT sizes: the nchan x k (channel, segment) pairs fill the plan's batch in order, three launches per batch
-template <typename T> static int stft_stream_generic(SpecPlanImpl* p, const StftStreamArgs& sa, const void* x, int64_t nx,
-                                                      int64_t nchan, int64_t k, double r, int psd_only, void* out,
-                                                      cudaStream_t st) {
+// STFT call, cuFFT sizes: the nchan x k (channel, segment) pairs fill the plan's batch in order, three launches per batch
+template <typename T> static int stft_generic(SpecPlanImpl* p, const StftStreamArgs& sa, const void* x, int64_t nx,
+                                               int64_t nchan, int64_t k, double r, int psd_only, void* out, cudaStream_t st) {
     const int64_t pairs = nchan * k;
     const int threads = 256;
     const auto* w = reinterpret_cast<const typename win_t<T>::type*>(p->d_window);
@@ -1485,17 +1422,17 @@ template <typename T> static int stft_stream_generic(SpecPlanImpl* p, const Stft
         const int64_t nf = pairs - f0 < p->batch ? pairs - f0 : p->batch;
         const dim3 gseg(cols(p->nfft), (unsigned)p->batch);
         if (p->cplx)
-            stft_stream_seg_kernel<T, true><<<gseg, threads, 0, st>>>(sa.hist, sa.h, sa.ldh, x, nx, f0, nf, k, p->hop, p->n, p->nfft,
-                                                                     w, p->segbuf.p);
+            stft_seg_kernel<T, true><<<gseg, threads, 0, st>>>(sa.hist, sa.h, sa.ldh, x, nx, f0, nf, k, p->hop, p->n, p->nfft, w,
+                                                              p->segbuf.p);
         else
-            stft_stream_seg_kernel<T, false><<<gseg, threads, 0, st>>>(sa.hist, sa.h, sa.ldh, x, nx, f0, nf, k, p->hop, p->n, p->nfft,
-                                                                      w, p->segbuf.p);
+            stft_seg_kernel<T, false><<<gseg, threads, 0, st>>>(sa.hist, sa.h, sa.ldh, x, nx, f0, nf, k, p->hop, p->n, p->nfft, w,
+                                                               p->segbuf.p);
         DSP_LAUNCH_OK();
         DSP_TRY(generic_fft(p, st));
         const dim3 gout(cols(p->nout), (unsigned)nf);
-        stft_stream_store_kernel<T><<<gout, threads, 0, st>>>(reinterpret_cast<const cx<T>*>(p->specbuf.p), p->nbins_fft, p->nfft,
-                                                              p->nout, f0, k, sa.ldo, psd_only, p->onesided, (T)(1.0 / r),
-                                                              (T)(2.0 / r), out);
+        stft_store_kernel<T><<<gout, threads, 0, st>>>(reinterpret_cast<const cx<T>*>(p->specbuf.p), p->nbins_fft, p->nfft,
+                                                       p->nout, f0, k, sa.ldo, psd_only, p->onesided, (T)(1.0 / r), (T)(2.0 / r),
+                                                       out);
         DSP_LAUNCH_OK();
     }
     return DSPB200_OK;
@@ -1992,6 +1929,21 @@ int dspb200_arraysplit_exec(dspb200_spec_plan* plan, const void* s, int64_t len,
     });
 }
 
+// Segments 0 .. k - 1 of every channel's virtual column [history (sa); x (the nx x nchan chunk)], one-shot or streaming
+static int stft_launch(SpecPlanImpl* p, const StftStreamArgs& sa, const void* x, int64_t nx, int64_t nchan, int64_t k, double r,
+                       int psd_only, void* out, cudaStream_t st) {
+    if (p->fused)
+        return fused_dispatch(p, "STFT", [&](auto t, auto nn) {
+            using T = decltype(t);
+            constexpr int N = decltype(nn)::value;
+            return p->cplx ? launch_stft_fused<T, N, true>(p, x, nx, nchan, k, r, psd_only, out, st, sa)
+                           : launch_stft_fused<T, N, false>(p, x, nx, nchan, k, r, psd_only, out, st, sa);
+        });
+    DSP_TRY(generic_prepare(p));
+    return p->f64 ? stft_generic<double>(p, sa, x, nx, nchan, k, r, psd_only, out, st)
+                  : stft_generic<float>(p, sa, x, nx, nchan, k, r, psd_only, out, st);
+}
+
 int dspb200_stft_exec_dev(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, double r, int psd_only,
                           void* out, void* stream) {
     DSP_RANGE("dspb200_stft_exec_dev");
@@ -1999,21 +1951,13 @@ int dspb200_stft_exec_dev(dspb200_spec_plan* plan, const void* s, int64_t len, i
     DSP_REQUIRE(r != 0.0 || !psd_only, "r must be nonzero");
     DSP_REQUIRE(nchan >= 0 && len >= 0, "negative size");
     SpecPlanImpl* p = &plan->impl;
-    cudaStream_t st = (cudaStream_t)stream;
     const int64_t k = nsegments(p, len);
     if (k == 0 || nchan == 0) return DSPB200_OK;
     DSP_REQUIRE(s && out, "NULL argument");
     if (r == 0.0) r = 1.0;
-    if (p->fused)
-        return fused_dispatch(p, "STFT", [&](auto t, auto nn) {
-            using T = decltype(t);
-            constexpr int N = decltype(nn)::value;
-            return p->cplx ? launch_stft_fused<T, N, true>(p, s, len, nchan, k, r, psd_only, out, st)
-                           : launch_stft_fused<T, N, false>(p, s, len, nchan, k, r, psd_only, out, st);
-        });
-    DSP_TRY(generic_prepare(p));
-    return p->f64 ? stft_generic<double>(p, s, len, nchan, k, r, psd_only, out, st)
-                  : stft_generic<float>(p, s, len, nchan, k, r, psd_only, out, st);
+    StftStreamArgs sa;                                   // no history; columns k apart
+    sa.ldo = k;
+    return stft_launch(p, sa, s, len, nchan, k, r, psd_only, out, (cudaStream_t)stream);
 }
 
 int dspb200_stft_exec(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, double r, int psd_only,
@@ -2077,6 +2021,7 @@ int dspb200_stft_stream_exec_dev(dspb200_spec_plan* plan, const void* hist_in, i
     if (r == 0.0) r = 1.0;
     cudaStream_t st = (cudaStream_t)stream;
     StftStreamArgs sa{hist_in, nhist, ldh, ldo};
+    sa.keep_plan = true;                                 // the same rounding whatever the chunking
     // launch 1: the seam copy (fused sizes: v[0, ls) of every channel, the samples of the units that start in the history)
     // and the new history
     int64_t ls = 0;
@@ -2107,17 +2052,8 @@ int dspb200_stft_stream_exec_dev(dspb200_spec_plan* plan, const void* hist_in, i
         DSP_LAUNCH_OK();
     }
     if (nseg == 0) return DSPB200_OK;
-    // launch 2 (fused sizes): the transforms
-    if (p->fused)
-        return fused_dispatch(p, "STFT", [&](auto t, auto nn) {
-            using T = decltype(t);
-            constexpr int N = decltype(nn)::value;
-            return p->cplx ? launch_stft_fused<T, N, true, true>(p, x, nx, nchan, nseg, r, psd_only, out, st, sa)
-                           : launch_stft_fused<T, N, false, true>(p, x, nx, nchan, nseg, r, psd_only, out, st, sa);
-        });
-    DSP_TRY(generic_prepare(p));
-    return p->f64 ? stft_stream_generic<double>(p, sa, x, nx, nchan, nseg, r, psd_only, out, st)
-                  : stft_stream_generic<float>(p, sa, x, nx, nchan, nseg, r, psd_only, out, st);
+    // launch 2 (fused sizes; cuFFT sizes: three per batch): the transforms
+    return stft_launch(p, sa, x, nx, nchan, nseg, r, psd_only, out, st);
 }
 
 // Host twin (returns when the work is done): the chunk and the ldh x nchan histories are staged; the rows of hist_out past

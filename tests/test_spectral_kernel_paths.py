@@ -170,7 +170,8 @@ def w1k_smem(dt, n, hop, windowed):
 
 
 def stft_route(dt, N, n, hop, length, nchan, base_aligned, windowed):
-    """The kernel launch_stft_fused runs: ("w1k", dtype, WIN) or ("fused", dtype, N, TMA, WIN)."""
+    """The kernel launch_stft_fused runs for a one-shot call: ("w1k", dtype, WIN) or ("fused", dtype, N, TMA, WIN).
+    (A stream runs the route of an aligned call of its plan; tests/test_stft_stream.py.)"""
     f64, cplx = _f64(dt), _cplx(dt)
     esz = dt.itemsize
     aligned = base_aligned and ((length * esz) % 16 == 0 or nchan == 1) and (hop * esz) % 16 == 0 and (n * esz) % 16 == 0
@@ -185,7 +186,8 @@ def stft_route(dt, N, n, hop, length, nchan, base_aligned, windowed):
 
 
 def stft_instances():
-    """Every stft_fused_kernel instance that launch_stft_fused can reach, and the four stft_w1k_kernel instances."""
+    """Every stft_fused_kernel instance that launch_stft_fused can reach, and the four stft_w1k_kernel instances: all the
+    STFT instances spectral.cu compiles, which one-shot and streaming calls share."""
     inst = set()
     for dt, N in FAMILIES:
         for tma in (False, True):
