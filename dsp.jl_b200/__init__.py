@@ -8,6 +8,7 @@ the same thin layer over the same C ABI, include/dspb200.h):
     fftfilt, fftfilt_, tdfilt, tdfilt_, resample, resample_filter      (src/Filters)
     periodogram, welch_pgram, welch_pgram_, WelchConfig, spectrogram, stft, power, freq, time
     STFTStream (an extension: stft / spectrogram of a chunked multichannel stream)
+    WelchStream (an extension: welch_pgram of a chunked multichannel stream)
                                                                        (src/periodograms.jl)
     hanning, hamming, rect, bartlett, kaiser, nextfastfft              (src/windows.jl, src/util.jl)
 
@@ -26,7 +27,7 @@ from .df2t import DF2TFilter, PolynomialRatio, coefa, coefb
 from .filters import (FIRFilter, fftfilt, fftfilt_, filt_multirate, inputlength, kaiserord, outputlength, resample,
                       resample_filter, resample_phase, tdfilt, tdfilt_)
 from .filters import filt_ as filt_hx_
-from .periodograms import (Periodogram, Periodogram2, Spectrogram, STFTStream, WelchConfig, arraysplit, arraysplit_count, compute_window, fftshift,
+from .periodograms import (Periodogram, Periodogram2, Spectrogram, STFTStream, WelchConfig, WelchStream, arraysplit, arraysplit_count, compute_window, fftshift,
                            filt_welch, freq, periodogram, power, spectrogram, stft, time, welch_pgram, welch_pgram_)
 
 from .multitaper import (Coherence, CrossPowerSpectra, MTConfig, MTCrossSpectraConfig, dpss, dpss_config, dpsseig,

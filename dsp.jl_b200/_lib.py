@@ -92,6 +92,10 @@ SIGNATURES = {
     "dspb200_stft_exec_dev": (_int, [_vp, _vp, _i64, _i64, _dbl, _int, _vp, _vp]),
     "dspb200_stft_stream_exec": (_int, [_vp, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _i64, _dbl, _int, _vp, _i64]),
     "dspb200_stft_stream_exec_dev": (_int, [_vp, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _i64, _dbl, _int, _vp, _i64, _vp]),
+    "dspb200_welch_stream_exec": (_int, [_vp, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _i64, _vp, _int]),
+    "dspb200_welch_stream_exec_dev": (_int, [_vp, _vp, _i64, _vp, _i64, _vp, _i64, _i64, _i64, _vp, _int, _vp]),
+    "dspb200_welch_stream_power": (_int, [_vp, _vp, _i64, _dbl, _vp]),
+    "dspb200_welch_stream_power_dev": (_int, [_vp, _vp, _i64, _dbl, _vp, _vp]),
     "dspb200_arraysplit_exec": (_int, [_vp, _vp, _i64, _vp]),
     "dspb200_periodogram2_exec": (_int, [_int, _vp, _i64, _i64, _i64, _i64, _dbl, _int, _vp]),
     "dspb200_periodogram2_exec_dev": (_int, [_int, _vp, _i64, _i64, _i64, _i64, _dbl, _int, _vp, _vp]),
@@ -317,6 +321,23 @@ class SpecPlan(_Plan):
         """One chunk of a device STFTStream (dspb200_stft_stream_exec_dev): device pointers."""
         check(lib.dspb200_stft_stream_exec_dev(self.handle, hist_in_ptr, int(nhist), hist_out_ptr, int(ldh), x_ptr, int(nx),
                                                int(nchan), int(nseg), float(r), 1 if psd_only else 0, out_ptr, int(ldo), stream))
+
+    def welch_stream(self, hist_in, nhist, hist_out, ldh, x, nx, nchan, nseg, acc, add):
+        """One chunk of a host WelchStream: Fortran-ordered host arrays, histories ldh x nchan (hist_in None: empty), acc the
+        nout x nchan float64 accumulator (read when add, written when nseg > 0)."""
+        check(lib.dspb200_welch_stream_exec(self.handle, None if hist_in is None else ptr(hist_in), int(nhist), ptr(hist_out),
+                                            int(ldh), ptr(x), int(nx), int(nchan), int(nseg), ptr(acc), 1 if add else 0))
+
+    def welch_stream_dev(self, hist_in_ptr, nhist, hist_out_ptr, ldh, x_ptr, nx, nchan, nseg, acc_ptr, add, stream=0):
+        """One chunk of a device WelchStream (dspb200_welch_stream_exec_dev): device pointers."""
+        check(lib.dspb200_welch_stream_exec_dev(self.handle, hist_in_ptr, int(nhist), hist_out_ptr, int(ldh), x_ptr, int(nx),
+                                                int(nchan), int(nseg), acc_ptr, 1 if add else 0, stream))
+
+    def welch_stream_power(self, acc, nchan, r, out):
+        check(lib.dspb200_welch_stream_power(self.handle, ptr(acc), int(nchan), float(r), ptr(out)))
+
+    def welch_stream_power_dev(self, acc_ptr, nchan, r, out_ptr, stream=0):
+        check(lib.dspb200_welch_stream_power_dev(self.handle, acc_ptr, int(nchan), float(r), out_ptr, stream))
 
 
 class MtPlan(SpecPlan):

@@ -997,6 +997,83 @@ __global__ void per2_pad_kernel(const T* __restrict__ s, int64_t n1, int64_t n2,
     }
 }
 
+// ---------------------------------------------------------------------------------------------- streaming Welch
+// Fused sizes: the partial rows of one call's two batched transform launches (welch_fused_kernel<..., BATCH = true>),
+// channel blockIdx.y, summed in Float64 and written (add = 0) or added to column blockIdx.y of acc (nout x nchan).  The
+// interior launch's ri rows are summed in welch_finalize_kernel's order -- warp sl of nw = min(ri, 32) sums rows sl, sl + nw,
+// ..., then the warps' sums are added in order -- and then the seam launch's rs rows the same way, and the two sums are added.
+// So a call with no seam rows puts into acc exactly the sum the one-shot finalize kernel scales.  Real input: bin k sums
+// rows k and N - k of the two-for-one transform; welch_stream_power_kernel applies the factor 1/2.
+template <typename T, int N>
+__global__ void __launch_bounds__(1024) welch_stream_reduce_kernel(const T* __restrict__ seam_rows, int rs,
+                                                                   const T* __restrict__ rows, int ri, double* __restrict__ acc,
+                                                                   int nout, int real_in, int add) {
+    __shared__ double red[2][32][33];
+    const int b = threadIdx.x & 31, sl = threadIdx.x >> 5;
+    const int k = blockIdx.x * 32 + b;
+    auto part = [&](const T* base, int nrows, int which) {
+        const int nw = nrows < 32 ? nrows : 32;
+        double sum = 0.0;
+        if (k < nout && sl < nw) {
+            const T* chan = base + (int64_t)blockIdx.y * nrows * N;
+            const T* c0 = chan + k;
+            const T* c1 = chan + ((N - k) & (N - 1));
+            if (real_in) {
+                for (int c = sl; c < nrows; c += nw) sum += (double)c0[(int64_t)c * N] + (double)c1[(int64_t)c * N];
+            } else {
+                for (int c = sl; c < nrows; c += nw) sum += (double)c0[(int64_t)c * N];
+            }
+        }
+        red[which][sl][b] = sum;
+    };
+    part(rows, ri, 0);
+    part(seam_rows, rs, 1);
+    __syncthreads();
+    if (sl == 0 && k < nout) {
+        const int nwi = ri < 32 ? ri : 32, nws = rs < 32 ? rs : 32;
+        double sum = red[0][0][b];
+        for (int i = 1; i < nwi; ++i) sum += red[0][i][b];
+        if (rs > 0) {
+            double s2 = red[1][0][b];
+            for (int i = 1; i < nws; ++i) s2 += red[1][i][b];
+            sum += s2;
+        }
+        double* q = acc + (int64_t)blockIdx.y * nout + k;
+        *q = add ? *q + sum : sum;
+    }
+}
+
+// cuFFT sizes: the spectra of (channel, segment) pairs f0 .. f0 + nf - 1 (f = c k + j, batch slot f - f0) into acc.  Thread
+// (bin kk, channel f0 / k + blockIdx.y) sums |X|^2 over its channel's slots in segment order, then writes the sum (add = 0
+// and the channel's first pair is in this batch) or adds it.  Two-sided real output: bin kk >= nbins_fft reads nfft - kk.
+template <typename T>
+__global__ void welch_stream_acc_kernel(const cx<T>* __restrict__ X, int64_t nbins_fft, int64_t nfft, int64_t nout, int64_t f0,
+                                        int64_t nf, int64_t k, int add, double* __restrict__ acc) {
+    const int64_t kk = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (kk >= nout) return;
+    const int64_t c = f0 / k + blockIdx.y;
+    const int64_t a = c * k > f0 ? c * k : f0, e = (c + 1) * k < f0 + nf ? (c + 1) * k : f0 + nf;
+    const int64_t src = kk < nbins_fft ? kk : nfft - kk;
+    double sum = 0.0;
+    for (int64_t f = a; f < e; ++f) sum += (double)cabs2(X[(f - f0) * nbins_fft + src]);
+    double* q = acc + c * nout + kk;
+    *q = (add || a > c * k) ? *q + sum : sum;
+}
+
+// Power of a streaming accumulation, column blockIdx.y: the fft2pow! scale (m1 = 1/r, m2 = 2/r; :142-172) of welch_finalize_kernel
+// (half: fused real plans, whose acc holds twice the power) and pow_finalize_kernel
+template <typename T>
+__global__ void welch_stream_power_kernel(const double* __restrict__ acc, int64_t nout, int64_t nfft, int onesided, int half,
+                                          double m1, double m2, T* __restrict__ out) {
+    const int64_t kk = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (kk >= nout) return;
+    const int64_t i = (int64_t)blockIdx.y * nout + kk;
+    double sum = acc[i];
+    if (half) sum *= 0.5;
+    const double m = (onesided && kk != 0 && 2 * kk != nfft) ? m2 : m1;
+    out[i] = (T)(sum * m);
+}
+
 // ---------------------------------------------------------------------------------------------- dispatch
 static bool fused_size_ok(int64_t nfft, bool f64) {
     if (nfft < 256 || (nfft & (nfft - 1))) return false;
@@ -1178,29 +1255,51 @@ static int64_t welch_batch_slices(int64_t gc, int64_t upc, int64_t nv, int64_t m
     return best;
 }
 
+// TMA staging of a batched launch needs every unit start 16-byte aligned: the base, the channel stride (launch_stft_fused's
+// rule), hop and n
+static bool welch_batch_aligned(const SpecPlanImpl* p, const void* s, int64_t stride, int64_t nchan, size_t esz) {
+    return ((uintptr_t)s % 16 == 0) && ((stride * (int64_t)esz) % 16 == 0 || nchan == 1) && ((p->hop * (int64_t)esz) % 16 == 0) &&
+           ((p->n * (int64_t)esz) % 16 == 0);
+}
+
+// One batched transform launch (welch_fused_kernel<..., BATCH = true>) over gc channels of k segments each: the channels are
+// sliced for the resident virtual CTAs of `cfg`, at most max_slices slices per channel, one partial row per (channel, slice)
+struct WelchBatchWork { int64_t k = 0, upc = 0, slices = 0, per = 0, nitems = 0; };
+static WelchBatchWork welch_batch_work(const SpecPlanImpl* p, const SpecPlanImpl::WelchCfg& cfg, bool cplx, int64_t gc, int64_t k,
+                                       int64_t max_slices) {
+    WelchBatchWork w;
+    w.k = k;
+    w.upc = cplx ? k : (k + 1) / 2;
+    w.slices = welch_batch_slices(gc, w.upc, welch_wave(p, cfg) * cfg.g, max_slices);
+    w.per = cdiv(w.upc, w.slices);
+    w.nitems = gc * w.slices;
+    return w;
+}
+// channel c's first sample at s + c * stride; rows: w.nitems rows of N
+template <typename T, bool CPLX>
+static int welch_batch_launch(SpecPlanImpl* p, SpecPlanImpl::WelchCfg& cfg, const WelchBatchWork& w, const void* s, int64_t stride,
+                              void* rows, cudaStream_t st) {
+    return welch_launch<T, true>(p, cfg, w.nitems, s, stride, Nil(), w.k, w.upc, w.per, (int)w.slices, w.nitems, Nil(), rows, Nil(),
+                                 st);
+}
+
 // Batched Welch over the nchan columns of a len x nchan matrix (k segments each): one kernel and one finalize launch per
 // channel group
 template <typename T, int N, bool CPLX>
 static int launch_welch_batch(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan, int64_t k, double r, void* out,
                               cudaStream_t st) {
     using In = typename in_type<T, CPLX>::type;
-    // TMA staging needs every unit start 16-byte aligned: the base, the channel stride (launch_stft_fused's rule), hop and n
-    const bool aligned = ((uintptr_t)s % 16 == 0) && ((len * sizeof(In)) % 16 == 0 || nchan == 1) &&
-                         ((p->hop * sizeof(In)) % 16 == 0) && ((p->n * sizeof(In)) % 16 == 0);
+    const bool aligned = welch_batch_aligned(p, s, len, nchan, sizeof(In));
     SpecPlanImpl::WelchCfg& cfg = p->welch_batch_cfg[aligned ? 1 : 0];
     DSP_TRY((welch_select<T, N, CPLX, true>(p, cfg, aligned, 0)));
-    const int64_t upc = CPLX ? k : (k + 1) / 2;
-    const int64_t nv = welch_wave(p, cfg) * cfg.g;                   // resident virtual CTAs
     const int64_t rows_cap = (int64_t)(WELCH_BATCH_SCRATCH / ((size_t)N * sizeof(T)));
     const int64_t gc_max = nchan < rows_cap ? nchan : rows_cap;
     for (int64_t c0 = 0; c0 < nchan; c0 += gc_max) {
         const int64_t gc = nchan - c0 < gc_max ? nchan - c0 : gc_max;
-        const int64_t slices = welch_batch_slices(gc, upc, nv, rows_cap / gc);
-        const int64_t per = cdiv(upc, slices);
-        const int64_t nitems = gc * slices;
-        DSP_TRY(p->bpartial.reserve((size_t)nitems * N * sizeof(T)));
-        DSP_TRY((welch_launch<T, true>(p, cfg, nitems, (const In*)s + c0 * len, len, Nil(), k, upc, per, (int)slices, nitems,
-                                       Nil(), p->bpartial.p, Nil(), st)));
+        const WelchBatchWork w = welch_batch_work(p, cfg, CPLX, gc, k, rows_cap / gc);
+        const int64_t slices = w.slices;
+        DSP_TRY(p->bpartial.reserve((size_t)w.nitems * N * sizeof(T)));
+        DSP_TRY((welch_batch_launch<T, CPLX>(p, cfg, w, (const In*)s + c0 * len, len, p->bpartial.p, st)));
         const int nw = slices < 32 ? (int)slices : 32;
         welch_finalize_kernel<T, N><<<dim3((unsigned)cdiv(p->nout, 32), (unsigned)gc), 32 * nw, 0, st>>>(
             reinterpret_cast<const T*>(p->bpartial.p), (int)slices, reinterpret_cast<T*>(out) + c0 * p->nout, (int)p->nout,
@@ -1407,29 +1506,36 @@ template <typename T> static int welch_generic_acc(SpecPlanImpl* p, const void* 
     return DSPB200_OK;
 }
 
+// Streaming calls, cuFFT sizes: blocks along one grid row per batch slot, enough for about 16 waves of the whole batch
+static unsigned stream_generic_cols(const SpecPlanImpl* p, int64_t len, int threads) {
+    const int64_t want = cdiv(len, threads), cap = cdiv((int64_t)p->sm_count * 16, p->batch);
+    return (unsigned)(want < cap ? want : cap);
+}
+
+// The spectra of (channel, segment) pairs f0 .. f0 + nf - 1 of the virtual columns [hist; x] (f = c k + j) in the plan's
+// batch buffer: stft_seg_kernel, then the plan's cuFFT transform
+template <typename T> static int stream_generic_fft(SpecPlanImpl* p, const void* hist, int64_t h, int64_t ldh, const void* x,
+                                                     int64_t nx, int64_t f0, int64_t nf, int64_t k, cudaStream_t st) {
+    const int threads = 256;
+    const auto* w = reinterpret_cast<const typename win_t<T>::type*>(p->d_window);
+    const dim3 gseg(stream_generic_cols(p, p->nfft, threads), (unsigned)p->batch);
+    if (p->cplx)
+        stft_seg_kernel<T, true><<<gseg, threads, 0, st>>>(hist, h, ldh, x, nx, f0, nf, k, p->hop, p->n, p->nfft, w, p->segbuf.p);
+    else
+        stft_seg_kernel<T, false><<<gseg, threads, 0, st>>>(hist, h, ldh, x, nx, f0, nf, k, p->hop, p->n, p->nfft, w, p->segbuf.p);
+    DSP_LAUNCH_OK();
+    return generic_fft(p, st);
+}
+
 // STFT call, cuFFT sizes: the nchan x k (channel, segment) pairs fill the plan's batch in order, three launches per batch
 template <typename T> static int stft_generic(SpecPlanImpl* p, const StftStreamArgs& sa, const void* x, int64_t nx,
                                                int64_t nchan, int64_t k, double r, int psd_only, void* out, cudaStream_t st) {
     const int64_t pairs = nchan * k;
     const int threads = 256;
-    const auto* w = reinterpret_cast<const typename win_t<T>::type*>(p->d_window);
-    // one grid row per batch slot, enough blocks along it for about 16 waves of the whole batch
-    auto cols = [&](int64_t len) {
-        const int64_t want = cdiv(len, threads), cap = cdiv((int64_t)p->sm_count * 16, p->batch);
-        return (unsigned)(want < cap ? want : cap);
-    };
     for (int64_t f0 = 0; f0 < pairs; f0 += p->batch) {
         const int64_t nf = pairs - f0 < p->batch ? pairs - f0 : p->batch;
-        const dim3 gseg(cols(p->nfft), (unsigned)p->batch);
-        if (p->cplx)
-            stft_seg_kernel<T, true><<<gseg, threads, 0, st>>>(sa.hist, sa.h, sa.ldh, x, nx, f0, nf, k, p->hop, p->n, p->nfft, w,
-                                                              p->segbuf.p);
-        else
-            stft_seg_kernel<T, false><<<gseg, threads, 0, st>>>(sa.hist, sa.h, sa.ldh, x, nx, f0, nf, k, p->hop, p->n, p->nfft, w,
-                                                               p->segbuf.p);
-        DSP_LAUNCH_OK();
-        DSP_TRY(generic_fft(p, st));
-        const dim3 gout(cols(p->nout), (unsigned)nf);
+        DSP_TRY(stream_generic_fft<T>(p, sa.hist, sa.h, sa.ldh, x, nx, f0, nf, k, st));
+        const dim3 gout(stream_generic_cols(p, p->nout, threads), (unsigned)nf);
         stft_store_kernel<T><<<gout, threads, 0, st>>>(reinterpret_cast<const cx<T>*>(p->specbuf.p), p->nbins_fft, p->nfft,
                                                        p->nout, f0, k, sa.ldo, psd_only, p->onesided, (T)(1.0 / r), (T)(2.0 / r),
                                                        out);
@@ -1457,6 +1563,105 @@ template <typename T> static int welch_batch_generic(SpecPlanImpl* p, const void
         const int threads = 128;
         pow_finalize_kernel<T><<<(int)cdiv(p->nout, threads), threads, 0, st>>>(acc, p->nbins_fft, p->nfft, p->nout, p->onesided,
                                                                                 1.0 / r, 2.0 / r, reinterpret_cast<T*>(out) + c * p->nout);
+        DSP_LAUNCH_OK();
+    }
+    return DSPB200_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- streaming calls
+// The seam of a streaming call, fused sizes: the nsu units per channel that start in the history (a unit is one complex
+// segment or two consecutive real ones) read v[0, ls) of the virtual column, which stft_stream_edge_kernel copies to
+// p->seam with column stride lds (16-byte aligned columns, for TMA)
+struct StreamSeam { int64_t nsu = 0, ls = 0, lds = 0; };
+static StreamSeam stream_seam(const SpecPlanImpl* p, int64_t nhist, int64_t nx, int64_t nseg) {
+    StreamSeam sm;
+    if (p->fused && nseg > 0 && nhist > 0) {
+        const int64_t us = p->cplx ? p->hop : 2 * p->hop, upc = p->cplx ? nseg : (nseg + 1) / 2;
+        sm.nsu = cdiv(nhist, us) < upc ? cdiv(nhist, us) : upc;
+        const int64_t end = (sm.nsu - 1) * us + (p->cplx ? p->n : p->hop + p->n);
+        sm.ls = end < nhist + nx ? end : nhist + nx;
+    }
+    const int64_t esz = (int64_t)dtype_size(p->dtype);
+    sm.lds = cdiv(sm.ls * esz, 16) * 16 / esz;
+    return sm;
+}
+
+// Launch 1 of a streaming call: the seam copy and the new history v[skip, skip + newh) of every channel
+static int stream_edge(SpecPlanImpl* p, const StreamSeam& sm, const void* hist_in, int64_t nhist, int64_t ldh, const void* x,
+                       int64_t nx, int64_t nchan, int64_t skip, int64_t newh, void* hist_out, cudaStream_t st) {
+    const size_t esz = dtype_size(p->dtype);
+    if (sm.ls > 0) DSP_TRY(p->seam.reserve((size_t)(sm.lds * nchan) * esz));
+    if (sm.ls + newh == 0) return DSPB200_OK;
+    const int64_t total = nchan * (sm.ls + newh);
+    const int threads = 256;
+    const unsigned grid = (unsigned)(cdiv(total, threads) < (int64_t)p->sm_count * 8 ? cdiv(total, threads) : (int64_t)p->sm_count * 8);
+#define DSP_EDGE(E) stft_stream_edge_kernel<E><<<grid, threads, 0, st>>>((const E*)hist_in, nhist, ldh, (const E*)x, nx, nchan, \
+                                                                         (E*)p->seam.p, sm.ls, sm.lds, skip, newh, (E*)hist_out)
+    switch (esz) {
+        case 4: DSP_EDGE(float); break;
+        case 8: DSP_EDGE(double); break;
+        default: DSP_EDGE(cx<double>); break;
+    }
+#undef DSP_EDGE
+    DSP_LAUNCH_OK();
+    return DSPB200_OK;
+}
+
+// Streaming Welch, fused sizes: segments 0 .. nseg - 1 of every channel's virtual column [history (h); x] into acc, per channel
+// group one batched transform launch over the seam units (in p->seam, column stride lds), one over the rest of x (column
+// stride nx) and welch_stream_reduce_kernel.  With no seam units the transform launch is launch_welch_batch's on x: the
+// same base, stride, alignment class, slices and instance.  The groups follow launch_welch_batch's scratch rule, with the
+// rows of both transform launches of a group in the scratch.
+template <typename T, int N, bool CPLX>
+static int welch_stream_fused(SpecPlanImpl* p, const StreamSeam& sm, const void* x, int64_t nx, int64_t h, int64_t nchan,
+                              int64_t nseg, double* acc, int add, cudaStream_t st) {
+    using In = typename in_type<T, CPLX>::type;
+    const int64_t spu = CPLX ? 1 : 2;
+    const int64_t seg_s = sm.nsu * spu < nseg ? sm.nsu * spu : nseg;           // segments of the seam units
+    const int64_t seg_i = nseg - seg_s;
+    const In* xi = reinterpret_cast<const In*>(x) + (seg_i ? seg_s * p->hop - h : 0);
+    const bool al_s = welch_batch_aligned(p, p->seam.p, sm.lds, nchan, sizeof(In));
+    const bool al_i = welch_batch_aligned(p, xi, nx, nchan, sizeof(In));
+    SpecPlanImpl::WelchCfg& cs = p->welch_batch_cfg[al_s ? 1 : 0];
+    SpecPlanImpl::WelchCfg& ci = p->welch_batch_cfg[al_i ? 1 : 0];
+    if (seg_s) DSP_TRY((welch_select<T, N, CPLX, true>(p, cs, al_s, 0)));
+    if (seg_i) DSP_TRY((welch_select<T, N, CPLX, true>(p, ci, al_i, 0)));
+    const int64_t rows_cap = (int64_t)(WELCH_BATCH_SCRATCH / ((size_t)N * sizeof(T)));
+    const int64_t gcap = seg_s && seg_i ? rows_cap / 2 : rows_cap;
+    const int64_t gc_max = nchan < gcap ? nchan : gcap;
+    for (int64_t c0 = 0; c0 < nchan; c0 += gc_max) {
+        const int64_t gc = nchan - c0 < gc_max ? nchan - c0 : gc_max;
+        const int64_t budget = rows_cap / gc;                                   // rows per channel
+        WelchBatchWork ws, wi;
+        if (seg_s) ws = welch_batch_work(p, cs, CPLX, gc, seg_s, seg_i ? budget / 2 : budget);
+        if (seg_i) wi = welch_batch_work(p, ci, CPLX, gc, seg_i, budget - ws.slices);
+        DSP_TRY(p->bpartial.reserve((size_t)(ws.nitems + wi.nitems) * N * sizeof(T)));
+        T* rows_s = reinterpret_cast<T*>(p->bpartial.p);
+        T* rows_i = rows_s + ws.nitems * N;
+        if (seg_s)
+            DSP_TRY((welch_batch_launch<T, CPLX>(p, cs, ws, reinterpret_cast<const In*>(p->seam.p) + c0 * sm.lds, sm.lds, rows_s, st)));
+        if (seg_i) DSP_TRY((welch_batch_launch<T, CPLX>(p, ci, wi, xi + c0 * nx, nx, rows_i, st)));
+        const int64_t nw = ws.slices > wi.slices ? ws.slices : wi.slices;
+        welch_stream_reduce_kernel<T, N><<<dim3((unsigned)cdiv(p->nout, 32), (unsigned)gc), 32 * (unsigned)(nw < 32 ? nw : 32), 0, st>>>(
+            rows_s, (int)ws.slices, rows_i, (int)wi.slices, acc + c0 * p->nout, (int)p->nout, CPLX ? 0 : 1, add);
+        DSP_LAUNCH_OK();
+    }
+    return DSPB200_OK;
+}
+
+// Streaming Welch, cuFFT sizes: the nchan x k (channel, segment) pairs of the virtual columns through the plan's batch, three
+// launches per batch
+template <typename T> static int welch_stream_generic(SpecPlanImpl* p, const void* hist, int64_t h, int64_t ldh, const void* x,
+                                                       int64_t nx, int64_t nchan, int64_t k, double* acc, int add,
+                                                       cudaStream_t st) {
+    const int64_t pairs = nchan * k;
+    const int threads = 128;
+    for (int64_t f0 = 0; f0 < pairs; f0 += p->batch) {
+        const int64_t nf = pairs - f0 < p->batch ? pairs - f0 : p->batch;
+        DSP_TRY(stream_generic_fft<T>(p, hist, h, ldh, x, nx, f0, nf, k, st));
+        const int64_t nc = (f0 + nf - 1) / k - f0 / k + 1;                  // channels with a pair in this batch
+        welch_stream_acc_kernel<T><<<dim3((unsigned)cdiv(p->nout, threads), (unsigned)nc), threads, 0, st>>>(
+            reinterpret_cast<const cx<T>*>(p->specbuf.p), p->nbins_fft, p->nfft, p->nout, f0, nf, k, add, acc);
         DSP_LAUNCH_OK();
     }
     return DSPB200_OK;
@@ -1974,8 +2179,35 @@ int dspb200_stft_exec(dspb200_spec_plan* plan, const void* s, int64_t len, int64
                       [&] { return dspb200_stft_exec_dev(plan, p->in[0].p, len, nchan, r, psd_only, p->out.p, p->s_exec); });
 }
 
-// Streaming stft / spectrogram.  Checks shared by both forms; *newh = samples of the new history.  Returns with *launch = false
-// when the call has nothing to do (no channel, or no sample and no segment: the history stays in hist_in).
+// Streaming calls (STFT and Welch).  Checks shared by every form: sizes, the history, the segments and, device form, the
+// overlaps of the written buffers (hist_out, and `out` of obytes bytes, named `oname`) with the others.  *newh = samples of
+// the new history.  Returns with *launch = false when the call has nothing to do (no channel, or no sample and no segment:
+// the history stays in hist_in).
+static int stream_check(const SpecPlanImpl* p, const void* hist_in, int64_t nhist, const void* hist_out, int64_t ldh,
+                        const void* x, int64_t nx, int64_t nchan, int64_t nseg, const void* out, size_t obytes, const char* oname,
+                        bool dev, int64_t* newh, bool* launch) {
+    *launch = false;
+    DSP_REQUIRE(hist_in != nullptr || nhist == 0, "hist_in is NULL but nhist = %lld", (long long)nhist);
+    DSP_REQUIRE(nhist <= ldh, "nhist (%lld) exceeds ldh (%lld)", (long long)nhist, (long long)ldh);
+    DSP_REQUIRE(nseg == 0 || (nseg - 1) * p->hop + p->n <= nhist + nx, "segment %lld runs past the virtual column (%lld samples)",
+                (long long)(nseg - 1), (long long)(nhist + nx));
+    *newh = nhist + nx - nseg * p->hop;
+    DSP_REQUIRE(*newh <= ldh, "the new history (%lld samples) exceeds ldh (%lld)", (long long)*newh, (long long)ldh);
+    if (dev) {
+        const size_t esz = dtype_size(p->dtype);
+        const size_t hbytes = (size_t)(ldh * nchan) * esz, xbytes = (size_t)(nx * nchan) * esz;
+        // the kernels read the samples and history of other channels' CTAs: no written buffer may overlap another buffer
+        DSP_REQUIRE(!ranges_overlap(hist_out, hbytes, hist_in, hbytes) && !ranges_overlap(hist_out, hbytes, x, xbytes) &&
+                    !ranges_overlap(hist_out, hbytes, out, obytes), "hist_out overlaps hist_in, x or %s", oname);
+        DSP_REQUIRE(!ranges_overlap(out, obytes, x, xbytes) && !ranges_overlap(out, obytes, hist_in, hbytes),
+                    "%s overlaps x or a history buffer", oname);
+    }
+    if (nchan == 0 || (nx == 0 && nseg == 0)) return DSPB200_OK;
+    DSP_REQUIRE((x != nullptr || nx == 0) && (out != nullptr || nseg == 0) && (hist_out != nullptr || *newh == 0), "NULL argument");
+    *launch = true;
+    return DSPB200_OK;
+}
+
 static int stft_stream_check(const SpecPlanImpl* p, const void* hist_in, int64_t nhist, const void* hist_out, int64_t ldh,
                              const void* x, int64_t nx, int64_t nchan, int64_t nseg, double r, int psd_only, const void* out,
                              int64_t ldo, bool dev, int64_t* newh, bool* launch) {
@@ -1983,27 +2215,10 @@ static int stft_stream_check(const SpecPlanImpl* p, const void* hist_in, int64_t
     DSP_REQUIRE(nhist >= 0 && nx >= 0 && nchan >= 0 && nseg >= 0 && ldh >= 0, "negative size");
     DSP_REQUIRE(psd_only == 0 || psd_only == 1, "psd_only must be 0 (raw spectra) or 1 (PSD columns)");
     DSP_REQUIRE(r != 0.0 || !psd_only, "r must be nonzero");
-    DSP_REQUIRE(hist_in != nullptr || nhist == 0, "hist_in is NULL but nhist = %lld", (long long)nhist);
-    DSP_REQUIRE(nhist <= ldh, "nhist (%lld) exceeds ldh (%lld)", (long long)nhist, (long long)ldh);
     DSP_REQUIRE(ldo >= nseg, "output column stride ldo < nseg");
-    DSP_REQUIRE(nseg == 0 || (nseg - 1) * p->hop + p->n <= nhist + nx, "segment %lld runs past the virtual column (%lld samples)",
-                (long long)(nseg - 1), (long long)(nhist + nx));
-    *newh = nhist + nx - nseg * p->hop;
-    DSP_REQUIRE(*newh <= ldh, "the new history (%lld samples) exceeds ldh (%lld)", (long long)*newh, (long long)ldh);
-    if (dev) {
-        const size_t esz = dtype_size(p->dtype), oel = (psd_only ? 1 : 2) * (p->f64 ? 8 : 4);
-        const size_t hbytes = (size_t)(ldh * nchan) * esz, xbytes = (size_t)(nx * nchan) * esz;
-        const size_t obytes = (nchan && nseg) ? (size_t)(((nchan - 1) * ldo + nseg) * p->nout) * oel : 0;
-        // the kernels read the samples and history of other channels' CTAs: no written buffer may overlap another buffer
-        DSP_REQUIRE(!ranges_overlap(hist_out, hbytes, hist_in, hbytes) && !ranges_overlap(hist_out, hbytes, x, xbytes) &&
-                    !ranges_overlap(hist_out, hbytes, out, obytes), "hist_out overlaps hist_in, x or out");
-        DSP_REQUIRE(!ranges_overlap(out, obytes, x, xbytes) && !ranges_overlap(out, obytes, hist_in, hbytes),
-                    "out overlaps x or a history buffer");
-    }
-    if (nchan == 0 || (nx == 0 && nseg == 0)) return DSPB200_OK;
-    DSP_REQUIRE((x != nullptr || nx == 0) && (out != nullptr || nseg == 0) && (hist_out != nullptr || *newh == 0), "NULL argument");
-    *launch = true;
-    return DSPB200_OK;
+    const size_t oel = (psd_only ? 1 : 2) * (p->f64 ? 8 : 4);
+    const size_t obytes = (nchan && nseg) ? (size_t)(((nchan - 1) * ldo + nseg) * p->nout) * oel : 0;
+    return stream_check(p, hist_in, nhist, hist_out, ldh, x, nx, nchan, nseg, out, obytes, "out", dev, newh, launch);
 }
 
 // Segments 0 .. nseg - 1 of every channel's virtual column [hist_in (nhist); x (nx)] into out (column s of channel c at
@@ -2024,33 +2239,10 @@ int dspb200_stft_stream_exec_dev(dspb200_spec_plan* plan, const void* hist_in, i
     sa.keep_plan = true;                                 // the same rounding whatever the chunking
     // launch 1: the seam copy (fused sizes: v[0, ls) of every channel, the samples of the units that start in the history)
     // and the new history
-    int64_t ls = 0;
-    if (p->fused && nseg > 0 && nhist > 0) {
-        const int64_t us = p->cplx ? p->hop : 2 * p->hop, upc = p->cplx ? nseg : (nseg + 1) / 2;
-        const int64_t nsu = cdiv(nhist, us) < upc ? cdiv(nhist, us) : upc;            // seam units per channel
-        const int64_t end = (nsu - 1) * us + (p->cplx ? p->n : p->hop + p->n);
-        ls = end < nhist + nx ? end : nhist + nx;
-    }
-    const size_t esz = dtype_size(p->dtype);
-    const int64_t lds = cdiv(ls * (int64_t)esz, 16) * 16 / (int64_t)esz;              // 16-byte aligned columns (TMA)
-    if (ls > 0) DSP_TRY(p->seam.reserve((size_t)(lds * nchan) * esz));
+    const StreamSeam sm = stream_seam(p, nhist, nx, nseg);
+    DSP_TRY(stream_edge(p, sm, hist_in, nhist, ldh, x, nx, nchan, nseg * p->hop, newh, hist_out, st));
     sa.seam = p->seam.p;
-    sa.lds = lds;
-    if (ls + newh > 0) {
-        const int64_t total = nchan * (ls + newh);
-        const int threads = 256;
-        const unsigned grid = (unsigned)(cdiv(total, threads) < (int64_t)p->sm_count * 8 ? cdiv(total, threads) : (int64_t)p->sm_count * 8);
-        const int64_t skip = nseg * p->hop;
-#define DSP_EDGE(E) stft_stream_edge_kernel<E><<<grid, threads, 0, st>>>((const E*)hist_in, nhist, ldh, (const E*)x, nx, nchan, \
-                                                                         (E*)p->seam.p, ls, lds, skip, newh, (E*)hist_out)
-        switch (esz) {
-            case 4: DSP_EDGE(float); break;
-            case 8: DSP_EDGE(double); break;
-            default: DSP_EDGE(cx<double>); break;
-        }
-#undef DSP_EDGE
-        DSP_LAUNCH_OK();
-    }
+    sa.lds = sm.lds;
     if (nseg == 0) return DSPB200_OK;
     // launch 2 (fused sizes; cuFFT sizes: three per batch): the transforms
     return stft_launch(p, sa, x, nx, nchan, nseg, r, psd_only, out, st);
@@ -2077,6 +2269,106 @@ int dspb200_stft_stream_exec(dspb200_spec_plan* plan, const void* hist_in, int64
                           return dspb200_stft_stream_exec_dev(plan, hist_in ? p->hin.p : nullptr, nhist, p->hout.p, ldh, p->in[0].p,
                                                               nx, nchan, nseg, r, psd_only, p->out.p, ldo, p->s_exec);
                       });
+}
+
+// Streaming Welch.  Checks shared by both forms (those of the STFT stream, acc in place of out)
+static int welch_stream_check(const SpecPlanImpl* p, const void* hist_in, int64_t nhist, const void* hist_out, int64_t ldh,
+                              const void* x, int64_t nx, int64_t nchan, int64_t nseg, const double* acc, int add, bool dev,
+                              int64_t* newh, bool* launch) {
+    *launch = false;
+    DSP_REQUIRE(nhist >= 0 && nx >= 0 && nchan >= 0 && nseg >= 0 && ldh >= 0, "negative size");
+    DSP_REQUIRE(add == 0 || add == 1, "add must be 0 (write acc) or 1 (add to acc)");
+    const size_t abytes = nseg ? (size_t)(p->nout * nchan) * sizeof(double) : 0;
+    return stream_check(p, hist_in, nhist, hist_out, ldh, x, nx, nchan, nseg, acc, abytes, "acc", dev, newh, launch);
+}
+
+// Segments 0 .. nseg - 1 of every channel's virtual column [hist_in (nhist); x (nx)] into acc, then the new history
+// v[nseg hop, nhist + nx) into hist_out.  Fused sizes: at most four launches per channel group, one without segments.
+int dspb200_welch_stream_exec_dev(dspb200_spec_plan* plan, const void* hist_in, int64_t nhist, void* hist_out, int64_t ldh,
+                                  const void* x, int64_t nx, int64_t nchan, int64_t nseg, double* acc, int add, void* stream) {
+    DSP_RANGE("dspb200_welch_stream_exec_dev");
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    SpecPlanImpl* p = &plan->impl;
+    int64_t newh = 0;
+    bool launch = false;
+    DSP_TRY(welch_stream_check(p, hist_in, nhist, hist_out, ldh, x, nx, nchan, nseg, acc, add, true, &newh, &launch));
+    if (!launch) return DSPB200_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    const StreamSeam sm = stream_seam(p, nhist, nx, nseg);
+    DSP_TRY(stream_edge(p, sm, hist_in, nhist, ldh, x, nx, nchan, nseg * p->hop, newh, hist_out, st));
+    if (nseg == 0) return DSPB200_OK;
+    if (p->fused)
+        return fused_dispatch(p, "Welch", [&](auto t, auto nn) {
+            using T = decltype(t);
+            constexpr int N = decltype(nn)::value;
+            return p->cplx ? welch_stream_fused<T, N, true>(p, sm, x, nx, nhist, nchan, nseg, acc, add, st)
+                           : welch_stream_fused<T, N, false>(p, sm, x, nx, nhist, nchan, nseg, acc, add, st);
+        });
+    DSP_TRY(generic_prepare(p));
+    return p->f64 ? welch_stream_generic<double>(p, hist_in, nhist, ldh, x, nx, nchan, nseg, acc, add, st)
+                  : welch_stream_generic<float>(p, hist_in, nhist, ldh, x, nx, nchan, nseg, acc, add, st);
+}
+
+// Host twin (returns when the work is done): the chunk, the histories and acc are staged
+int dspb200_welch_stream_exec(dspb200_spec_plan* plan, const void* hist_in, int64_t nhist, void* hist_out, int64_t ldh,
+                              const void* x, int64_t nx, int64_t nchan, int64_t nseg, double* acc, int add) {
+    DSP_RANGE("dspb200_welch_stream_exec");
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    SpecPlanImpl* p = &plan->impl;
+    int64_t newh = 0;
+    bool launch = false;
+    DSP_TRY(welch_stream_check(p, hist_in, nhist, hist_out, ldh, x, nx, nchan, nseg, acc, add, false, &newh, &launch));
+    if (!launch) return DSPB200_OK;
+    DSP_TRY(ensure_streams(p));
+    const size_t esz = dtype_size(p->dtype);
+    const size_t hbytes = (size_t)(ldh * nchan) * esz, abytes = nseg ? (size_t)(p->nout * nchan) * sizeof(double) : 0;
+    return run_staged(p->s_exec, {{x, (size_t)(nx * nchan) * esz, &p->in[0]}, {hist_in, hist_in ? hbytes : 0, &p->hin}, {acc, add ? abytes : 0, &p->out}},
+                      {{acc, abytes, &p->out}, {hist_out, newh ? hbytes : 0, &p->hout}}, [&] {
+                          return dspb200_welch_stream_exec_dev(plan, hist_in ? p->hin.p : nullptr, nhist, p->hout.p, ldh, p->in[0].p,
+                                                               nx, nchan, nseg, reinterpret_cast<double*>(p->out.p), add, p->s_exec);
+                      });
+}
+
+int dspb200_welch_stream_power_dev(dspb200_spec_plan* plan, const double* acc, int64_t nchan, double r, void* out, void* stream) {
+    DSP_RANGE("dspb200_welch_stream_power_dev");
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    DSP_REQUIRE(nchan >= 0, "negative size");
+    DSP_REQUIRE(r != 0.0, "r must be nonzero");
+    SpecPlanImpl* p = &plan->impl;
+    if (nchan == 0) return DSPB200_OK;
+    DSP_REQUIRE(acc && out, "NULL argument");
+    DSP_REQUIRE(!ranges_overlap(out, (size_t)(p->nout * nchan) * (p->f64 ? 8 : 4), acc, (size_t)(p->nout * nchan) * sizeof(double)),
+                "out overlaps acc");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int threads = 128;
+    const int half = p->fused && !p->cplx;
+    for (int64_t c0 = 0; c0 < nchan; c0 += 65535) {
+        const int64_t gc = nchan - c0 < 65535 ? nchan - c0 : 65535;
+        const dim3 grid((unsigned)cdiv(p->nout, threads), (unsigned)gc);
+        if (p->f64)
+            welch_stream_power_kernel<double><<<grid, threads, 0, st>>>(acc + c0 * p->nout, p->nout, p->nfft, p->onesided, half,
+                                                                       1.0 / r, 2.0 / r, (double*)out + c0 * p->nout);
+        else
+            welch_stream_power_kernel<float><<<grid, threads, 0, st>>>(acc + c0 * p->nout, p->nout, p->nfft, p->onesided, half,
+                                                                      1.0 / r, 2.0 / r, (float*)out + c0 * p->nout);
+        DSP_LAUNCH_OK();
+    }
+    return DSPB200_OK;
+}
+
+int dspb200_welch_stream_power(dspb200_spec_plan* plan, const double* acc, int64_t nchan, double r, void* out) {
+    DSP_RANGE("dspb200_welch_stream_power");
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    DSP_REQUIRE(nchan >= 0, "negative size");
+    DSP_REQUIRE(r != 0.0, "r must be nonzero");
+    SpecPlanImpl* p = &plan->impl;
+    if (nchan == 0) return DSPB200_OK;
+    DSP_REQUIRE(acc && out, "NULL argument");
+    DSP_TRY(ensure_streams(p));
+    const size_t n = (size_t)(p->nout * nchan);
+    return run_staged(p->s_exec, {{acc, n * sizeof(double), &p->in[0]}}, {{out, n * (p->f64 ? 8 : 4), &p->out}}, [&] {
+        return dspb200_welch_stream_power_dev(plan, reinterpret_cast<const double*>(p->in[0].p), nchan, r, p->out.p, p->s_exec);
+    });
 }
 
 // Multitaper (SURVEY.md 8f rank 1; src/multitaper.jl:117-242, 262-404).  The plan's window holds `ntapers` rows of n

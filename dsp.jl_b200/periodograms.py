@@ -460,7 +460,73 @@ def stft_stream_step(h, nx, n, noverlap, paired, final=False):
     return kc, h + nx - kc * (n - noverlap)
 
 
-class STFTStream:
+class _ChunkStream:
+    """What STFTStream and WelchStream share: the chunk checks (residency, eltype and channel shape fixed by the first chunk, a
+    refused first call fixing nothing) and the pair of history buffers that every call reads one of and writes the other."""
+    _a_name = ""
+
+    def _check(self, x):
+        name = type(self).__name__
+        if self.device and not isinstance(x, DeviceArray):
+            raise ArgumentError(f"a device {name} takes DeviceArrays (construct it without device=True for host arrays)")
+        if not self.device and isinstance(x, DeviceArray):
+            raise ArgumentError(f"a host {name} takes host arrays (construct it with device=True for DeviceArrays)")
+        if self._finished:
+            raise ArgumentError("the stream is finished: reset() starts a new one")
+        if not self.device:
+            x = np.asarray(x)
+        if x.ndim not in (1, 2):
+            raise ArgumentError(f"{self._a_name} chunk is a vector or a len x nchan matrix")
+        dt = x.dtype if self.device else fftintype(x.dtype)
+        if self.device and dt != fftintype(dt):
+            raise ArgumentError("device chunks must be Float32, Float64, ComplexF32 or ComplexF64")
+        key = (np.dtype(dt), tuple(x.shape[1:]))
+        if self._key is None:
+            self._setup(key[0], key[1])
+        elif key != self._key:
+            raise ArgumentError(f"this {name} streams {self._key[0]} chunks of channel shape {self._key[1]}; got "
+                                f"{key[0]} {key[1]} (reset() starts a new stream)")
+        if not self.device:
+            x = np.asfortranarray(x, dtype=dt)
+        return x
+
+    def _nchan(self):
+        return int(np.prod(self._key[1])) if self._key[1] else 1
+
+    def _advance(self, launch, nx, nseg):
+        """One library call with nx new samples and nseg segments -- launch(cur, nxt, h, nchan): history buffer cur (None: an
+        empty history) in, nxt out -- then the swap of the history buffers and the new counts."""
+        nchan = self._nchan()
+        h = self.history_len
+        newh = h + nx - nseg * self.hop
+        if nchan and (nx or nseg):
+            if self._hist is None:
+                hshape = (self.ldh,) + self._key[1]
+                self._hist = ([None, DeviceArray(hshape, self._key[0])] if self.device
+                              else [None, np.zeros(hshape, dtype=self._key[0], order="F")])
+            cur, nxt = self._hist
+            launch(cur, nxt, h, nchan)
+            if cur is None:                                 # the first call: an empty history in, none to reuse
+                cur = (DeviceArray(nxt.shape, nxt.dtype) if self.device
+                       else np.zeros(nxt.shape, dtype=nxt.dtype, order="F"))
+            self._hist = [nxt, cur]
+        self.history_len = newh
+        if self._hist is not None:
+            self.history = self._hist[0] if self.device else self._hist[0][:newh]
+        self.nsegments += nseg
+
+    def _chunk(self, x, *args):
+        fresh = self._key is None
+        x = self._check(x)
+        try:
+            return self._emit(x, *args)
+        except ArgumentError:
+            if fresh:                   # a refused first call leaves the stream as it was: no eltype or channel shape fixed
+                self._key = None
+            raise
+
+
+class STFTStream(_ChunkStream):
     """stft / spectrogram of a signal that arrives in chunks (an extension: the reference's stft takes one vector).
 
     STFTStream(n, noverlap=n>>1, psdonly=False, onesided=None, nfft=nextfastfft(n), fs=1, window=None, device=False) takes
@@ -518,29 +584,7 @@ class STFTStream:
         self.ldh = max(1, self.n - 1 + (0 if cplx else self.hop))
         self._key = (dt, chan_shape)
 
-    def _check(self, x):
-        if self.device and not isinstance(x, DeviceArray):
-            raise ArgumentError("a device STFTStream takes DeviceArrays (construct it without device=True for host arrays)")
-        if not self.device and isinstance(x, DeviceArray):
-            raise ArgumentError("a host STFTStream takes host arrays (construct it with device=True for DeviceArrays)")
-        if self._finished:
-            raise ArgumentError("the stream is finished: reset() starts a new one")
-        if not self.device:
-            x = np.asarray(x)
-        if x.ndim not in (1, 2):
-            raise ArgumentError("an STFTStream chunk is a vector or a len x nchan matrix")
-        dt = x.dtype if self.device else fftintype(x.dtype)
-        if self.device and dt != fftintype(dt):
-            raise ArgumentError("device chunks must be Float32, Float64, ComplexF32 or ComplexF64")
-        key = (np.dtype(dt), tuple(x.shape[1:]))
-        if self._key is None:
-            self._setup(key[0], key[1])
-        elif key != self._key:
-            raise ArgumentError(f"this STFTStream streams {self._key[0]} chunks of channel shape {self._key[1]}; got "
-                                f"{key[0]} {key[1]} (reset() starts a new stream)")
-        if not self.device:
-            x = np.asfortranarray(x, dtype=dt)
-        return x
+    _a_name = "an STFTStream"
 
     def _out_shape(self, cols):
         return (self.nout, cols) + self._key[1]
@@ -549,16 +593,9 @@ class STFTStream:
         """One library call on chunk x (nx may be 0): nseg segments into out (ldo columns per channel), then the swap of the
         history buffers."""
         nx = x.shape[0] if x is not None else 0
-        nchan = int(np.prod(self._key[1])) if self._key[1] else 1
         plan = self._plans[self._key[0]]
-        h = self.history_len
-        newh = h + nx - nseg * self.hop
-        if nchan and (nx or nseg):
-            if self._hist is None:
-                hshape = (self.ldh,) + self._key[1]
-                self._hist = ([None, DeviceArray(hshape, self._key[0])] if self.device
-                              else [None, np.zeros(hshape, dtype=self._key[0], order="F")])
-            cur, nxt = self._hist
+
+        def launch(cur, nxt, h, nchan):
             if self.device:
                 plan.stft_stream_dev(cur.ptr if cur is not None else None, h, nxt.ptr, self.ldh,
                                      x.ptr if x is not None else None, nx, nchan, nseg, self.r, self.psdonly,
@@ -567,26 +604,9 @@ class STFTStream:
                 xx = x if x is not None else np.zeros((1,) + self._key[1], dtype=self._key[0], order="F")
                 oo = out if out is not None else np.zeros(1, dtype=self.odt)
                 plan.stft_stream(cur, h, nxt, self.ldh, xx, nx, nchan, nseg, self.r, self.psdonly, oo, ldo)
-            if cur is None:                                 # the first call: an empty history in, none to reuse
-                cur = (DeviceArray(nxt.shape, nxt.dtype) if self.device
-                       else np.zeros(nxt.shape, dtype=nxt.dtype, order="F"))
-            self._hist = [nxt, cur]
-        self.history_len = newh
-        if self._hist is not None:
-            self.history = self._hist[0] if self.device else self._hist[0][:newh]
-        self.nsegments += nseg
+        self._advance(launch, nx, nseg)
 
-    def _chunk(self, x, out=None):
-        fresh = self._key is None
-        x = self._check(x)
-        try:
-            return self._emit(x, out)
-        except ArgumentError:
-            if fresh:                   # a refused first call leaves the stream as it was: no eltype or channel shape fixed
-                self._key = None
-            raise
-
-    def _emit(self, x, out):
+    def _emit(self, x, out=None):
         kc, _ = stft_stream_step(self.history_len, x.shape[0], self.n, self.noverlap, not self.cplx)
         if out is None:
             out = (DeviceArray if self.device else (lambda s, d: np.zeros(s, dtype=d, order="F")))(self._out_shape(kc), self.odt)
@@ -642,3 +662,131 @@ class STFTStream:
             self._run(None, kc, out, kc)
         self._finished = True
         return out
+
+
+# --------------------------------------------------------------------------------------------- streaming welch_pgram
+
+class WelchStream(_ChunkStream):
+    """welch_pgram of a signal that arrives in chunks (an extension: the reference's welch_pgram takes one vector).
+
+    WelchStream(n, noverlap=n>>1, onesided=None, nfft=nextfastfft(n), fs=1, window=None, device=False) takes the parameters
+    and checks of WelchConfig.  Every chunk `x` is a vector (nx,) or a column-major (nx, nchan) matrix of channels that share
+    one sample count; `update(x)` adds the power spectra of the segments the chunk completes -- every complete segment of
+    the concatenation of all chunks so far, segment i starting at sample i*hop -- to a Float64 accumulator per channel and
+    bin, and keeps the samples the next segment needs as the history (at most n - 1).  `welch_pgram()` can be read at any
+    time and does not change the stream: it is welch_pgram of everything so far, r = nsegments*fs*norm2 (zeros before the
+    first complete segment, as welch_pgram of a signal shorter than n).  One chunk from an empty history gives the power of
+    welch_pgram of that chunk bit for bit for power-of-two nfft that have fused kernels; more chunks round differently, within
+    the bound of DESIGN.md section 4.  The same chunks give the same bits.
+
+    device=True: chunks and results are DeviceArrays and the accumulator stays in device memory; a chunk costs at most four
+    kernel launches per group of channels for power-of-two nfft (one when it completes no segment), three per batch of
+    segments plus one for cuFFT sizes, no copy of the chunk and no host synchronisation.  `history` is then the current
+    history buffer -- (ldh,) or (ldh, nchan), the first `history_len` rows valid.  A host stream takes host arrays (its
+    `history` is the (history_len,) or (history_len, nchan) array).  The first chunk fixes the eltype and channel shape;
+    reset() drops them."""
+
+    _a_name = "a WelchStream"
+
+    def __init__(self, n, noverlap=None, onesided=None, nfft=None, fs=1, window=None, device=False):
+        self.n = int(n)
+        self.noverlap = self.n >> 1 if noverlap is None else int(noverlap)
+        self.nfft = nextfastfft(self.n) if nfft is None else int(nfft)
+        if self.nfft < self.n:
+            raise DomainError("nfft must be >= n")                                        # :565
+        self.window, norm2 = compute_window(window, self.n)
+        if not (0 <= self.noverlap < self.n):
+            raise DomainError("noverlap must be between zero and n")                     # ArraySplit :44
+        self.hop = self.n - self.noverlap
+        self.fs, self.device = fs, bool(device)
+        self._onesided_arg = onesided
+        self.r = fs * norm2                                                               # :568
+        self._plans = {}
+        self._finished = False
+        self.reset()
+
+    def reset(self):
+        """Start a new stream: drops the history, the accumulated power, the segment count, the eltype and the channel shape."""
+        self.nsegments = 0
+        self.history_len = 0
+        self.history = None
+        self._key = None             # (eltype, channel shape) fixed by the first chunk
+        self._hist = None            # [current, next] history buffers
+        self._acc = None             # nout x nchan Float64 accumulator, written (not added to) by the first segment's call
+        return self
+
+    def _setup(self, dt, chan_shape):
+        cplx = dt.kind == "c"
+        onesided = (not cplx) if self._onesided_arg is None else bool(self._onesided_arg)
+        if onesided and cplx:
+            raise ArgumentError("cannot compute one-sided FFT of a complex signal")      # :564
+        if dt not in self._plans:
+            self._plans[dt] = _lib.SpecPlan(dt, self.n, self.noverlap, self.nfft, onesided, self.window)
+        self.onesided, self.cplx = onesided, cplx
+        self.nout = self.nfft // 2 + 1 if onesided else self.nfft
+        self.odt = fftabs2type(dt)
+        self.freq = rfftfreq(self.nfft, self.fs) if onesided else fftfreq(self.nfft, self.fs)   # :573
+        self.ldh = max(1, self.n - 1)
+        self._key = (dt, chan_shape)
+
+    def _emit(self, x):
+        nx = x.shape[0]
+        kc, _ = stft_stream_step(self.history_len, nx, self.n, self.noverlap, False)
+        plan = self._plans[self._key[0]]
+        if self._acc is None:
+            shape = (self.nout,) + self._key[1]
+            self._acc = DeviceArray(shape, np.float64) if self.device else np.zeros(shape, dtype=np.float64, order="F")
+        add = self.nsegments > 0                 # the first call that completes a segment writes the accumulator
+
+        def launch(cur, nxt, h, nchan):
+            if self.device:
+                plan.welch_stream_dev(cur.ptr if cur is not None else None, h, nxt.ptr, self.ldh, x.ptr if nx else None, nx,
+                                      nchan, kc, self._acc.ptr, add, 0)
+            else:
+                xx = x if nx else np.zeros((1,) + self._key[1], dtype=self._key[0], order="F")
+                plan.welch_stream(cur, h, nxt, self.ldh, xx, nx, nchan, kc, self._acc, add)
+        self._advance(launch, nx, kc)
+        return kc
+
+    def update(self, x):
+        """Adds the segments chunk x completes to the accumulator; returns their number (per channel)."""
+        return self._chunk(x)
+
+    def welch_pgram(self):
+        """Periodogram(power, freq) of everything streamed so far: power is (nout,) for vector chunks, (nout, nchan) for
+        matrix chunks (a DeviceArray for a device stream)."""
+        self._require_chunk()
+        shape = (self.nout,) + self._key[1]
+        out = DeviceArray(shape, self.odt) if self.device else np.empty(shape, dtype=self.odt, order="F")
+        return self.welch_pgram_(out)
+
+    def welch_pgram_(self, out):
+        """welch_pgram() into `out` (shape (nout,) or (nout, nchan), the real eltype of the stream); returns the Periodogram."""
+        self._require_chunk()
+        shape = (self.nout,) + self._key[1]
+        if self.device != isinstance(out, DeviceArray):
+            raise ArgumentError("out must be a DeviceArray for a device WelchStream and a host array for a host one")
+        if out.dtype != self.odt or tuple(out.shape) != shape:
+            raise ArgumentError(f"out must be a {self.odt} array of shape {shape}")
+        if self.device:
+            if out.overlaps(self._acc):
+                raise ArgumentError("out must not overlap the stream's accumulator")
+        elif not out.flags.f_contiguous:
+            raise ArgumentError("out must be Fortran-ordered (column-major)")
+        nchan = self._nchan()
+        plan = self._plans[self._key[0]]
+        if self.nsegments == 0 or nchan == 0:                                  # fill!(out, 0), src/periodograms.jl:747
+            if self.device:
+                if out.nbytes:
+                    out.copy_from_host(np.zeros(shape, dtype=self.odt, order="F"))
+            else:
+                out[...] = 0
+        elif self.device:
+            plan.welch_stream_power_dev(self._acc.ptr, nchan, self.nsegments * self.r, out.ptr, 0)
+        else:
+            plan.welch_stream_power(self._acc, nchan, self.nsegments * self.r, out)
+        return Periodogram(out, self.freq)
+
+    def _require_chunk(self):
+        if self._key is None:
+            raise ArgumentError("the WelchStream has had no chunk yet: its eltype and channel shape are not known")

@@ -265,6 +265,29 @@ DSPB200_API int dspb200_stft_stream_exec_dev(dspb200_spec_plan* plan, const void
 DSPB200_API int dspb200_stft_stream_exec(dspb200_spec_plan* plan, const void* hist_in, int64_t nhist, void* hist_out, int64_t ldh,
                                          const void* x, int64_t nx, int64_t nchan, int64_t nseg, double r, int psd_only,
                                          void* out, int64_t ldo);
+/* Streaming Welch (an extension; the reference's welch_pgram takes one vector): the virtual columns, histories and checks of
+ * dspb200_stft_stream_exec_dev.  The call adds the power spectra |FFT(window .* segment)|^2 of segments 0 .. nseg-1 of every
+ * channel's v = [hist_in; x] to acc -- an nout x nchan Float64 matrix, column-major, bin k of channel c at acc[c*nout + k]
+ * (add = 1), or writes them there (add = 0: a fresh accumulation, no separate zeroing) -- then writes the new history
+ * v[nseg*hop, nhist + nx) to hist_out.  A call with nseg == 0 leaves acc as it is.  Every segment of a call is summed
+ * in a fixed order: the result is deterministic.  DSPB200_EINVALID, before any launch, for the rules of the STFT stream
+ * (overlapping buffers, acc in place of out; segments past the virtual column; a new history larger than ldh) and add not
+ * 0 or 1.  Fused sizes: at most four launches per group of channels (see dspb200_welch_batch_exec_dev); a call whose
+ * segments all lie in x (nhist == 0) runs the launch of dspb200_welch_batch_exec_dev on x, so one call over the whole
+ * matrix followed by dspb200_welch_stream_power_dev gives the batched welch_pgram bit for bit.  cuFFT sizes: three
+ * launches per batch of (channel, segment) pairs plus the history. */
+DSPB200_API int dspb200_welch_stream_exec_dev(dspb200_spec_plan* plan, const void* hist_in, int64_t nhist, void* hist_out,
+                                              int64_t ldh, const void* x, int64_t nx, int64_t nchan, int64_t nseg, double* acc,
+                                              int add, void* stream);
+/* host pointers; acc is read (add = 1) and written on the host */
+DSPB200_API int dspb200_welch_stream_exec(dspb200_spec_plan* plan, const void* hist_in, int64_t nhist, void* hist_out,
+                                          int64_t ldh, const void* x, int64_t nx, int64_t nchan, int64_t nseg, double* acc,
+                                          int add);
+/* The Welch power of a streaming accumulation: out (nout x nchan, real eltype of the plan) = acc with the fft2pow! scaling
+ * of welch_pgram (src/periodograms.jl:142-172), r = nsegments*fs*norm2.  One launch; out may not overlap acc. */
+DSPB200_API int dspb200_welch_stream_power_dev(dspb200_spec_plan* plan, const double* acc, int64_t nchan, double r, void* out,
+                                               void* stream);
+DSPB200_API int dspb200_welch_stream_power(dspb200_spec_plan* plan, const double* acc, int64_t nchan, double r, void* out);
 /* arraysplit(s, n, noverlap, nfft, window) / ArraySplit: src/periodograms.jl:32-73, 134-137.  out = k x nfft matrix, row i =
  * [window .* s[i*hop .. i*hop+n) ; zeros(nfft-n)] (the reference yields the rows one at a time into one reused buffer). */
 DSPB200_API int dspb200_arraysplit_exec(dspb200_spec_plan* plan, const void* s, int64_t len, void* out);
