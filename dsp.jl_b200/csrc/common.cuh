@@ -6,6 +6,7 @@
 #include <stdio.h>
 #include <string.h>
 #include <stdarg.h>
+#include <functional>
 #include <initializer_list>
 #include <type_traits>
 
@@ -142,6 +143,36 @@ int run_staged(cudaStream_t st, std::initializer_list<HostIn> in, std::initializ
     return settle(st, queue());
 }
 
+// The streams, events and device slots of a plan's host-pointer calls.  One-shot calls stage through in[0] / out[0] on
+// s_exec (run_staged); chunked calls (run_chunked) give chunk c slot c % 2, copied in on s_in, computed on s_exec and
+// drained on s_out, so that chunk c+1's copy in and chunk c-1's copy out overlap chunk c's kernels.
+struct HostPipe {
+    cudaStream_t s_in = nullptr, s_exec = nullptr, s_out = nullptr;
+    cudaEvent_t ev_in[2] = {}, ev_exec[2] = {}, ev_out[2] = {};
+    DevBuf in[2], out[2];
+    int ensure(int device);   // makes `device` current and creates the streams and events on first use
+    void release();
+};
+
+// One chunk of run_chunked: `bytes` of host input at `src` are copied into the slot's input buffer, read(in, out) queues on
+// s_exec the work that reads the slot's input buffer and writes its output buffer, after() (optional) queues further work
+// on s_exec that uses neither buffer, and `out_bytes` (optional) of the output buffer are then copied to `dst`.
+struct Chunk {
+    const void* src;
+    size_t bytes;
+    std::function<int(const void* in, void* out)> read;
+    std::function<int()> after;
+    void* dst = nullptr;
+    size_t out_bytes = 0;
+};
+
+// Host-pointer calls that stream the caller's buffers through the two slots of `hp`: reserve in_cap (and out_cap, if any)
+// bytes per slot used, queue chunk(0) ... chunk(nchunks - 1) and then tail() (optional) on s_exec, and return once all
+// three streams are idle, on success and failure alike (the first error is the one reported).  A slot is refilled once its
+// last read is done and written once its last output has been drained.
+int run_chunked(HostPipe& hp, int64_t nchunks, size_t in_cap, size_t out_cap, const std::function<Chunk(int64_t)>& chunk,
+                const std::function<int()>& tail);
+
 // Stateful FIR and overlap-save calls (DF2TFilter): ns state elements of esz bytes per column, in si_in (NULL: zero state)
 // and out to si_out (NULL: not wanted).
 // Device form: the size and overlap checks -- CTAs read the samples, halo and state behind other CTAs' outputs, so a
@@ -149,12 +180,13 @@ int run_staged(cudaStream_t st, std::initializer_list<HostIn> in, std::initializ
 // passed through on `st`.  The caller returns after this when nx == 0 or ncols == 0.
 int state_prologue_dev(const void* x, int64_t nx, int64_t ncols, const void* si_in, void* si_out, void* out, int64_t ns,
                        size_t esz, cudaStream_t st);
-// Host form, for a plan P with `device`, `s_exec` and ensure_streams(P*): x and the state are staged apart (bx, bout, bsi,
-// bso), so out may be x and si_out may be si_in; nx == 0 passes the state through on the host.
-// dev(d_x, d_si_in, d_si_out, d_out) runs the device form on p->s_exec.
+// Host form, for a plan P with ensure_streams(P*), which creates the plan's execute stream `s_exec` (hence taken by
+// reference: it is read after ensure_streams has run): x and the state are staged apart (bx, bout, bsi, bso), so out may
+// be x and si_out may be si_in; nx == 0 passes the state through on the host.
+// dev(d_x, d_si_in, d_si_out, d_out) runs the device form on s_exec.
 template <class P, class F>
-int exec_state_host(P* p, const void* x, int64_t nx, int64_t ncols, const void* si_in, void* si_out, void* out, int64_t ns,
-                    size_t esz, DevBuf& bx, DevBuf& bout, DevBuf& bsi, DevBuf& bso, F&& dev) {
+int exec_state_host(P* p, const cudaStream_t& s_exec, const void* x, int64_t nx, int64_t ncols, const void* si_in, void* si_out,
+                    void* out, int64_t ns, size_t esz, DevBuf& bx, DevBuf& bout, DevBuf& bsi, DevBuf& bso, F&& dev) {
     DSP_REQUIRE(nx >= 0 && ncols >= 0, "negative size");
     if (ncols == 0) return DSPB200_OK;
     DSP_REQUIRE(nx == 0 || (x && out), "NULL argument");
@@ -167,7 +199,7 @@ int exec_state_host(P* p, const void* x, int64_t nx, int64_t ncols, const void* 
         return DSPB200_OK;
     }
     DSP_TRY(ensure_streams(p));
-    return run_staged(p->s_exec, {{x, bytes, &bx}, {si_in, si_in ? sbytes : 0, &bsi}},
+    return run_staged(s_exec, {{x, bytes, &bx}, {si_in, si_in ? sbytes : 0, &bsi}},
                       {{out, bytes, &bout}, {si_out, si_out ? sbytes : 0, &bso}},
                       [&] { return dev(bx.p, si_in ? bsi.p : nullptr, si_out ? bso.p : nullptr, bout.p); });
 }

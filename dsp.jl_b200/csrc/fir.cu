@@ -169,7 +169,7 @@ int dspb200_fir_exec_state(dspb200_fir_plan* plan, const void* x, int64_t nx, in
     DSP_RANGE("dspb200_fir_exec_state");
     DSP_REQUIRE(plan != nullptr, "plan is NULL");
     FirPlanImpl* p = &plan->impl;
-    return exec_state_host(p, x, nx, ncols, si_in, si_out, out, p->nb - 1, dtype_size(p->dtype), p->in, p->out, p->si_in,
+    return exec_state_host(p, p->s_exec, x, nx, ncols, si_in, si_out, out, p->nb - 1, dtype_size(p->dtype), p->in, p->out, p->si_in,
                            p->si_out, [&](const void* d_x, const void* d_si_in, void* d_si_out, void* d_out) {
                                return dspb200_fir_exec_state_dev(plan, d_x, nx, ncols, d_si_in, d_si_out, d_out, p->s_exec);
                            });

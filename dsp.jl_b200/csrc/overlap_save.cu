@@ -36,10 +36,7 @@ struct OsPlanImpl {
     bool fft_ok = false;
     int64_t batch = 0, nbins = 0;
     DevBuf td, fd;
-    // host path
-    DevBuf in[2], out[2];
-    cudaStream_t s_in = nullptr, s_exec = nullptr, s_out = nullptr;
-    cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_exec[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr};
+    HostPipe pipe;          // host-pointer calls
 };
 
 template <typename T, bool CPLX> struct os_elt { using type = T; };
@@ -895,19 +892,7 @@ static int64_t auto_nfft(int64_t nv, bool f64) {
     return n;
 }
 
-// makes the plan's device current and creates its streams and events on first use (s_exec last: it marks the set complete)
-static int ensure_streams(OsPlanImpl* p) {
-    DSP_CUDA(cudaSetDevice(p->device));
-    if (p->s_exec) return DSPB200_OK;
-    DSP_TRY(ensure_stream(&p->s_in));
-    DSP_TRY(ensure_stream(&p->s_out));
-    for (int i = 0; i < 2; ++i) {
-        if (!p->ev_in[i]) DSP_CUDA(cudaEventCreateWithFlags(&p->ev_in[i], cudaEventDisableTiming));
-        if (!p->ev_exec[i]) DSP_CUDA(cudaEventCreateWithFlags(&p->ev_exec[i], cudaEventDisableTiming));
-        if (!p->ev_out[i]) DSP_CUDA(cudaEventCreateWithFlags(&p->ev_out[i], cudaEventDisableTiming));
-    }
-    return ensure_stream(&p->s_exec);
-}
+static int ensure_streams(OsPlanImpl* p) { return p->pipe.ensure(p->device); }
 
 }  // namespace dspb200
 
@@ -1197,8 +1182,8 @@ int dspb200_os_exec_state_dev(dspb200_os_plan* plan, const void* x, int64_t nx, 
     return os_run<true>(p, a, OsStateArgs{si_in, si_out, nx}, st);
 }
 
-// Host pointers.  One long column is streamed: chunk c+1 is copied in while chunk c is convolved and chunk
-// c-1 is copied out (three streams, two buffers each); otherwise copy in -> run -> copy out.
+// Host pointers.  One long column is streamed in chunks of whole blocks (run_chunked): chunk c+1 is copied in while chunk
+// c is convolved and chunk c-1 is copied out; otherwise copy in -> run -> copy out.
 int dspb200_os_exec(dspb200_os_plan* plan, const void* u, int64_t nu, int64_t ncols, void* out, int64_t nout) {
     DSP_RANGE("dspb200_os_exec");
     DSP_REQUIRE(plan != nullptr, "plan is NULL");
@@ -1206,39 +1191,26 @@ int dspb200_os_exec(dspb200_os_plan* plan, const void* u, int64_t nu, int64_t nc
     if (nout == 0 || ncols == 0) return DSPB200_OK;
     DSP_REQUIRE(out != nullptr && (u != nullptr || nu == 0), "NULL argument");
     OsPlanImpl* p = &plan->impl;
+    HostPipe& hp = p->pipe;
     DSP_TRY(ensure_streams(p));
     const size_t esz = dtype_size(p->dtype);
     const int64_t chunk_out = ((int64_t(32) << 20) / (int64_t)esz / p->L + 1) * p->L;   // ~32 MiB, whole blocks
     if (ncols == 1 && nout > 2 * chunk_out && nu > 0) {
         const int64_t nfull = nu + p->nv - 1;
-        const size_t in_cap = (size_t)(chunk_out + p->nv - 1) * esz, out_cap = (size_t)chunk_out * esz;
-        for (int i = 0; i < 2; ++i) { DSP_TRY(p->in[i].reserve(in_cap)); DSP_TRY(p->out[i].reserve(out_cap)); }
-        bool used[2] = {false, false};
-        int slot = 0;
-        for (int64_t m0 = 0; m0 < nout; m0 += chunk_out, slot ^= 1) {
-            const int64_t cnt = nout - m0 < chunk_out ? nout - m0 : chunk_out;
+        auto chunk = [&](int64_t c) -> Chunk {
+            const int64_t m0 = c * chunk_out, cnt = nout - m0 < chunk_out ? nout - m0 : chunk_out;
             int64_t i_lo = m0 - (p->nv - 1); if (i_lo < 0) i_lo = 0;
             int64_t i_hi = m0 + cnt; if (i_hi > nu) i_hi = nu;
             const int64_t ni = i_hi > i_lo ? i_hi - i_lo : 0;
-            if (used[slot]) DSP_CUDA(cudaStreamWaitEvent(p->s_in, p->ev_exec[slot], 0));    // input buffer free
-            if (ni > 0) DSP_CUDA(cudaMemcpyAsync(p->in[slot].p, (const char*)u + (size_t)i_lo * esz, (size_t)ni * esz, cudaMemcpyHostToDevice, p->s_in));
-            DSP_CUDA(cudaEventRecord(p->ev_in[slot], p->s_in));
-            DSP_CUDA(cudaStreamWaitEvent(p->s_exec, p->ev_in[slot], 0));
-            if (used[slot]) DSP_CUDA(cudaStreamWaitEvent(p->s_exec, p->ev_out[slot], 0));  // output buffer drained
-            OsRange a{p->in[slot].p, i_lo, ni, 0, p->out[slot].p, m0, cnt, 0, nfull, 1};
-            DSP_TRY(os_run(p, a, p->s_exec));
-            DSP_CUDA(cudaEventRecord(p->ev_exec[slot], p->s_exec));
-            DSP_CUDA(cudaStreamWaitEvent(p->s_out, p->ev_exec[slot], 0));
-            DSP_CUDA(cudaMemcpyAsync((char*)out + (size_t)m0 * esz, p->out[slot].p, (size_t)cnt * esz, cudaMemcpyDeviceToHost, p->s_out));
-            DSP_CUDA(cudaEventRecord(p->ev_out[slot], p->s_out));
-            used[slot] = true;
-        }
-        DSP_CUDA(cudaStreamSynchronize(p->s_out));
-        DSP_CUDA(cudaStreamSynchronize(p->s_exec));
-        return DSPB200_OK;
+            auto run = [=, &hp](const void* in, void* o) {
+                return os_run(p, OsRange{in, i_lo, ni, 0, o, m0, cnt, 0, nfull, 1}, hp.s_exec);
+            };
+            return {(const char*)u + (size_t)i_lo * esz, (size_t)ni * esz, run, nullptr, (char*)out + (size_t)m0 * esz, (size_t)cnt * esz};
+        };
+        return run_chunked(hp, cdiv(nout, chunk_out), (size_t)(chunk_out + p->nv - 1) * esz, (size_t)chunk_out * esz, chunk, nullptr);
     }
-    return run_staged(p->s_exec, {{u, (size_t)(nu * ncols) * esz, &p->in[0]}}, {{out, (size_t)(nout * ncols) * esz, &p->out[0]}},
-                      [&] { return dspb200_os_exec_dev(plan, p->in[0].p, nu, ncols, p->out[0].p, nout, p->s_exec); });
+    return run_staged(hp.s_exec, {{u, (size_t)(nu * ncols) * esz, &hp.in[0]}}, {{out, (size_t)(nout * ncols) * esz, &hp.out[0]}},
+                      [&] { return dspb200_os_exec_dev(plan, hp.in[0].p, nu, ncols, hp.out[0].p, nout, hp.s_exec); });
 }
 
 // Host pointers: x and the state are staged apart (x in in[0], out in out[0], si_in in in[1], si_out in out[1]).
@@ -1247,9 +1219,10 @@ int dspb200_os_exec_state(dspb200_os_plan* plan, const void* x, int64_t nx, int6
     DSP_RANGE("dspb200_os_exec_state");
     DSP_REQUIRE(plan != nullptr, "plan is NULL");
     OsPlanImpl* p = &plan->impl;
-    return exec_state_host(p, x, nx, ncols, si_in, si_out, out, p->nv - 1, dtype_size(p->dtype), p->in[0], p->out[0], p->in[1],
-                           p->out[1], [&](const void* d_x, const void* d_si_in, void* d_si_out, void* d_out) {
-                               return dspb200_os_exec_state_dev(plan, d_x, nx, ncols, d_si_in, d_si_out, d_out, p->s_exec);
+    HostPipe& hp = p->pipe;
+    return exec_state_host(p, hp.s_exec, x, nx, ncols, si_in, si_out, out, p->nv - 1, dtype_size(p->dtype), hp.in[0], hp.out[0],
+                           hp.in[1], hp.out[1], [&](const void* d_x, const void* d_si_in, void* d_si_out, void* d_out) {
+                               return dspb200_os_exec_state_dev(plan, d_x, nx, ncols, d_si_in, d_si_out, d_out, hp.s_exec);
                            });
 }
 
@@ -1262,15 +1235,7 @@ int dspb200_os_plan_destroy(dspb200_os_plan* plan) {
     if (p->d_H) cudaFree(p->d_H);
     if (p->fft_ok) { cufftDestroy(p->fwd); cufftDestroy(p->inv); }
     p->td.release(); p->fd.release();
-    for (int i = 0; i < 2; ++i) {
-        p->in[i].release(); p->out[i].release();
-        if (p->ev_in[i]) cudaEventDestroy(p->ev_in[i]);
-        if (p->ev_exec[i]) cudaEventDestroy(p->ev_exec[i]);
-        if (p->ev_out[i]) cudaEventDestroy(p->ev_out[i]);
-    }
-    if (p->s_in) cudaStreamDestroy(p->s_in);
-    if (p->s_exec) cudaStreamDestroy(p->s_exec);
-    if (p->s_out) cudaStreamDestroy(p->s_out);
+    p->pipe.release();
     delete plan;
     return DSPB200_OK;
 }

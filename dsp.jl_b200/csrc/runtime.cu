@@ -61,6 +61,59 @@ int settle(cudaStream_t st, int rc) {
     return e == cudaSuccess ? DSPB200_OK : cuda_fail(e, "cudaStreamSynchronize", __FILE__, __LINE__);
 }
 
+int HostPipe::ensure(int device) {
+    DSP_CUDA(cudaSetDevice(device));
+    if (s_exec) return DSPB200_OK;                                       // s_exec is created last: it marks the set complete
+    DSP_TRY(ensure_stream(&s_in));
+    DSP_TRY(ensure_stream(&s_out));
+    for (cudaEvent_t* ev : {ev_in, ev_exec, ev_out})
+        for (int i = 0; i < 2; ++i)
+            if (!ev[i]) DSP_CUDA(cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming));
+    return ensure_stream(&s_exec);
+}
+
+void HostPipe::release() {
+    for (int i = 0; i < 2; ++i) {
+        in[i].release(); out[i].release();
+        for (cudaEvent_t ev : {ev_in[i], ev_exec[i], ev_out[i]})
+            if (ev) cudaEventDestroy(ev);
+    }
+    for (cudaStream_t st : {s_in, s_exec, s_out})
+        if (st) cudaStreamDestroy(st);
+}
+
+int run_chunked(HostPipe& hp, int64_t nchunks, size_t in_cap, size_t out_cap, const std::function<Chunk(int64_t)>& chunk,
+                const std::function<int()>& tail) {
+    auto queue = [&]() -> int {
+        for (int s = 0; s < 2 && s < nchunks; ++s) {
+            DSP_TRY(hp.in[s].reserve(in_cap));
+            if (out_cap) DSP_TRY(hp.out[s].reserve(out_cap));
+        }
+        bool read[2] = {false, false}, draining[2] = {false, false};
+        for (int64_t c = 0; c < nchunks; ++c) {
+            const int s = (int)(c & 1);
+            const Chunk ch = chunk(c);
+            if (read[s]) DSP_CUDA(cudaStreamWaitEvent(hp.s_in, hp.ev_exec[s], 0));
+            if (ch.bytes) DSP_CUDA(cudaMemcpyAsync(hp.in[s].p, ch.src, ch.bytes, cudaMemcpyHostToDevice, hp.s_in));
+            DSP_CUDA(cudaEventRecord(hp.ev_in[s], hp.s_in));
+            DSP_CUDA(cudaStreamWaitEvent(hp.s_exec, hp.ev_in[s], 0));
+            if (draining[s]) DSP_CUDA(cudaStreamWaitEvent(hp.s_exec, hp.ev_out[s], 0));
+            DSP_TRY(ch.read(hp.in[s].p, hp.out[s].p));
+            DSP_CUDA(cudaEventRecord(hp.ev_exec[s], hp.s_exec));
+            read[s] = true;
+            if (ch.after) DSP_TRY(ch.after());
+            if (ch.out_bytes) {
+                DSP_CUDA(cudaStreamWaitEvent(hp.s_out, hp.ev_exec[s], 0));
+                DSP_CUDA(cudaMemcpyAsync(ch.dst, hp.out[s].p, ch.out_bytes, cudaMemcpyDeviceToHost, hp.s_out));
+                DSP_CUDA(cudaEventRecord(hp.ev_out[s], hp.s_out));
+                draining[s] = true;
+            }
+        }
+        return tail ? tail() : DSPB200_OK;
+    };
+    return settle(hp.s_out, settle(hp.s_exec, settle(hp.s_in, queue())));
+}
+
 int state_prologue_dev(const void* x, int64_t nx, int64_t ncols, const void* si_in, void* si_out, void* out, int64_t ns,
                        size_t esz, cudaStream_t st) {
     DSP_REQUIRE(nx >= 0 && ncols >= 0, "negative size");

@@ -66,11 +66,10 @@ struct SpecPlanImpl {
     int64_t nbins_fft = 0;        // nfft/2+1 (real) or nfft (complex)
     DevBuf segbuf, specbuf, acc;  // acc: double[nbins_fft]
     // host-pointer path
-    DevBuf in[2], out;
+    HostPipe pipe;
     DevBuf hin, hout;             // dspb200_stft_stream_exec: the staged histories
     DevBuf seam;                  // streaming STFT, fused sizes: the seam samples of the last call (stft_stream_edge_kernel)
-    cudaStream_t s_copy = nullptr, s_exec = nullptr;
-    cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr};
+    DevBuf y;                     // dspb200_filt_welch_exec: the filter output, n samples
 };
 
 // ---------------------------------------------------------------------------------------------- helpers
@@ -1710,17 +1709,7 @@ static int64_t nsegments(const SpecPlanImpl* p, int64_t len) {
     return len >= p->n ? (len - p->n) / p->hop + 1 : 0;   // src/periodograms.jl:49-50
 }
 
-// makes the plan's device current and creates its streams and events on first use (s_exec last: it marks the set complete)
-static int ensure_streams(SpecPlanImpl* p) {
-    DSP_CUDA(cudaSetDevice(p->device));
-    if (p->s_exec) return DSPB200_OK;
-    DSP_TRY(ensure_stream(&p->s_copy));
-    for (int i = 0; i < 2; ++i) {
-        if (!p->ev_in[i]) DSP_CUDA(cudaEventCreateWithFlags(&p->ev_in[i], cudaEventDisableTiming));
-        if (!p->ev_done[i]) DSP_CUDA(cudaEventCreateWithFlags(&p->ev_done[i], cudaEventDisableTiming));
-    }
-    return ensure_stream(&p->s_exec);
-}
+static int ensure_streams(SpecPlanImpl* p) { return p->pipe.ensure(p->device); }
 
 }  // namespace dspb200
 
@@ -1740,12 +1729,12 @@ static int mt_cross_run(dspb200_spec_plan* plan, const void* signal, int64_t nch
     SpecPlanImpl* p = &plan->impl;
     const int64_t n = p->n, cnt = nchan * nchan * nf;
     const size_t cs_bytes = (size_t)cnt * sizeof(cx<T>), out_bytes = coherence ? (size_t)cnt * sizeof(T) : cs_bytes;
-    if (!dev) DSP_TRY(p->in[0].reserve((size_t)(n * nchan) * sizeof(T)));
-    DSP_TRY(p->in[1].reserve((size_t)(n * nchan) * sizeof(T)));
+    if (!dev) DSP_TRY(p->pipe.in[0].reserve((size_t)(n * nchan) * sizeof(T)));
+    DSP_TRY(p->pipe.in[1].reserve((size_t)(n * nchan) * sizeof(T)));
     DSP_TRY(p->tmp.reserve((size_t)(p->nout * nchan) * sizeof(cx<T>)));
-    DSP_TRY(p->out.reserve(cs_bytes + (coherence ? out_bytes : 0)));
-    if (!dev) DSP_CUDA(cudaMemcpyAsync(p->in[0].p, signal, (size_t)(n * nchan) * sizeof(T), cudaMemcpyHostToDevice, st));
-    cs_prep_kernel<T><<<(unsigned)nchan, 256, 0, st>>>(dev ? (const T*)signal : (const T*)p->in[0].p, nchan, n, demean, (T*)p->in[1].p);
+    DSP_TRY(p->pipe.out[0].reserve(cs_bytes + (coherence ? out_bytes : 0)));
+    if (!dev) DSP_CUDA(cudaMemcpyAsync(p->pipe.in[0].p, signal, (size_t)(n * nchan) * sizeof(T), cudaMemcpyHostToDevice, st));
+    cs_prep_kernel<T><<<(unsigned)nchan, 256, 0, st>>>(dev ? (const T*)signal : (const T*)p->pipe.in[0].p, nchan, n, demean, (T*)p->pipe.in[1].p);
     DSP_LAUNCH_OK();
     const int threads = 256;
     const int grid = (int)(cdiv(cnt, threads) < device_sm_count() * 32 ? cdiv(cnt, threads) : device_sm_count() * 32);
@@ -1753,19 +1742,19 @@ static int mt_cross_run(dspb200_spec_plan* plan, const void* signal, int64_t nch
     int rc = DSPB200_OK;
     for (int64_t t = 0; t < p->ntapers && rc == DSPB200_OK; ++t) {
         p->d_window = (char*)base + (size_t)t * win_row_bytes(p);
-        rc = dspb200_stft_exec_dev(plan, p->in[1].p, n, nchan, 1.0, 0, p->tmp.p, st);     // raw spectra, nout x nchan
+        rc = dspb200_stft_exec_dev(plan, p->pipe.in[1].p, n, nchan, 1.0, 0, p->tmp.p, st);     // raw spectra, nout x nchan
         if (rc == DSPB200_OK) {
-            cs_acc_kernel<T><<<grid, threads, 0, st>>>((cx<T>*)p->out.p, (const cx<T>*)p->tmp.p, p->nout, nchan, f_lo, nf,
+            cs_acc_kernel<T><<<grid, threads, 0, st>>>((cx<T>*)p->pipe.out[0].p, (const cx<T>*)p->tmp.p, p->nout, nchan, f_lo, nf,
                                                        (p->nfft % 2 == 0) ? 1 : 0, t == 0 ? 1 : 0);
             count_launch(1);
         }
     }
     p->d_window = base;
     DSP_TRY(rc);
-    void* res = p->out.p;
+    void* res = p->pipe.out[0].p;
     if (coherence) {
-        res = (char*)p->out.p + cs_bytes;
-        coherence_kernel<T><<<grid, threads, 0, st>>>((T*)res, (const cx<T>*)p->out.p, nchan, nf);
+        res = (char*)p->pipe.out[0].p + cs_bytes;
+        coherence_kernel<T><<<grid, threads, 0, st>>>((T*)res, (const cx<T>*)p->pipe.out[0].p, nchan, nf);
         DSP_LAUNCH_OK();
     }
     DSP_CUDA(cudaMemcpyAsync(out, res, out_bytes, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
@@ -2062,51 +2051,86 @@ int dspb200_welch_batch_exec(dspb200_spec_plan* plan, const void* s, int64_t len
     DSP_REQUIRE(!any || s != nullptr, "s is NULL");
     DSP_TRY(ensure_streams(p));
     const size_t in_bytes = any ? (size_t)(len * nchan) * dtype_size(p->dtype) : 0;
-    return run_staged(p->s_exec, {{s, in_bytes, &p->in[0]}}, {{out, (size_t)(p->nout * nchan) * (p->f64 ? 8 : 4), &p->out}},
-                      [&] { return dspb200_welch_batch_exec_dev(plan, p->in[0].p, len, nchan, r, p->out.p, p->s_exec); });
+    return run_staged(p->pipe.s_exec, {{s, in_bytes, &p->pipe.in[0]}}, {{out, (size_t)(p->nout * nchan) * (p->f64 ? 8 : 4), &p->pipe.out[0]}},
+                      [&] { return dspb200_welch_batch_exec_dev(plan, p->pipe.in[0].p, len, nchan, r, p->pipe.out[0].p, p->pipe.s_exec); });
 }
 
-// Host-pointer Welch: the signal is streamed through two device buffers in segment-aligned chunks so the
+// The tail of the chunked host-pointer Welch calls: the PSD into out[0] (reserved before the first chunk), then to the host.
+static int welch_finalize_host(SpecPlanImpl* p, double r, void* out) {
+    HostPipe& hp = p->pipe;
+    DSP_TRY(welch_finalize(p, r, hp.out[0].p, hp.s_exec));
+    DSP_CUDA(cudaMemcpyAsync(out, hp.out[0].p, (size_t)p->nout * (p->f64 ? 8 : 4), cudaMemcpyDeviceToHost, hp.s_exec));
+    return DSPB200_OK;
+}
+
+// Host-pointer Welch: the signal is streamed through the plan's two slots in segment-aligned chunks (run_chunked), so the
 // H2D copy of chunk c+1 overlaps the kernel of chunk c (effective when `s` is pinned).
 int dspb200_welch_exec(dspb200_spec_plan* plan, const void* s, int64_t len, double r, void* out) {
     DSP_RANGE("dspb200_welch_exec");
     DSP_REQUIRE(plan && out, "NULL argument");
     DSP_REQUIRE(r != 0.0, "r must be nonzero");
     SpecPlanImpl* p = &plan->impl;
+    HostPipe& hp = p->pipe;
+    const int64_t k = nsegments(p, len);
+    DSP_REQUIRE(k == 0 || s != nullptr, "s is NULL");
     DSP_TRY(ensure_streams(p));
     const size_t esz = dtype_size(p->dtype);
-    const int64_t k = nsegments(p, len);
-    const size_t out_bytes = (size_t)p->nout * (p->f64 ? 8 : 4);
-    DSP_TRY(p->out.reserve(out_bytes));
-    DSP_TRY(welch_begin(p, p->s_exec));
-    if (k > 0) {
-        DSP_REQUIRE(s != nullptr, "s is NULL");
-        int64_t chunk_segs = ((int64_t(32) << 20) / (int64_t)esz) / p->hop;   // ~32 MiB of new samples per chunk
-        if (chunk_segs < 64) chunk_segs = 64;
-        if (chunk_segs > k) chunk_segs = k;
-        const size_t chunk_bytes = (size_t)((chunk_segs - 1) * p->hop + p->n) * esz;
-        DSP_TRY(p->in[0].reserve(chunk_bytes));
-        if (chunk_segs < k) DSP_TRY(p->in[1].reserve(chunk_bytes));
-        int slot = 0;
-        bool used[2] = {false, false};
-        for (int64_t b0 = 0; b0 < k; b0 += chunk_segs, slot ^= 1) {
-            const int64_t b1 = b0 + chunk_segs < k ? b0 + chunk_segs : k;
-            const int64_t first = b0 * p->hop;
-            const int64_t cnt = (b1 - 1 - b0) * p->hop + p->n;
-            if (used[slot]) DSP_CUDA(cudaStreamWaitEvent(p->s_copy, p->ev_done[slot], 0));
-            DSP_CUDA(cudaMemcpyAsync(p->in[slot].p, (const char*)s + (size_t)first * esz, (size_t)cnt * esz,
-                                     cudaMemcpyHostToDevice, p->s_copy));
-            DSP_CUDA(cudaEventRecord(p->ev_in[slot], p->s_copy));
-            DSP_CUDA(cudaStreamWaitEvent(p->s_exec, p->ev_in[slot], 0));
-            DSP_TRY(welch_accumulate(p, p->in[slot].p, first, b0, b1, p->s_exec));
-            DSP_CUDA(cudaEventRecord(p->ev_done[slot], p->s_exec));
-            used[slot] = true;
-        }
-    }
-    DSP_TRY(welch_finalize(p, r, p->out.p, p->s_exec));
-    DSP_CUDA(cudaMemcpyAsync(out, p->out.p, out_bytes, cudaMemcpyDeviceToHost, p->s_exec));
-    DSP_CUDA(cudaStreamSynchronize(p->s_exec));
-    return DSPB200_OK;
+    int64_t chunk_segs = ((int64_t(32) << 20) / (int64_t)esz) / p->hop;   // ~32 MiB of new samples per chunk
+    if (chunk_segs < 64) chunk_segs = 64;
+    if (chunk_segs > k) chunk_segs = k;
+    DSP_TRY(hp.out[0].reserve((size_t)p->nout * (p->f64 ? 8 : 4)));
+    DSP_TRY(welch_begin(p, hp.s_exec));
+    auto chunk = [&](int64_t c) -> Chunk {
+        const int64_t b0 = c * chunk_segs, b1 = b0 + chunk_segs < k ? b0 + chunk_segs : k;
+        const int64_t first = b0 * p->hop, cnt = (b1 - 1 - b0) * p->hop + p->n;
+        auto accumulate = [=, &hp](const void* in, void*) { return welch_accumulate(p, in, first, b0, b1, hp.s_exec); };
+        return {(const char*)s + (size_t)first * esz, (size_t)cnt * esz, accumulate};
+    };
+    return run_chunked(hp, k > 0 ? cdiv(k, chunk_segs) : 0, (size_t)((chunk_segs - 1) * p->hop + p->n) * esz, 0, chunk,
+                       [&] { return welch_finalize_host(p, r, out); });
+}
+
+// welch_pgram(filt(b, x), config) (src/dspbase.jl:14-15, src/periodograms.jl:702-759) for a stream that lives in host
+// memory.  The filter output y never crosses PCIe: chunk c's samples (plus the nv - 1 sample halo) are copied into a slot
+// while the execute stream runs, for chunk c - 1, the overlap-save convolution of its output range into y
+// (dspb200_os_exec_range_dev) and then the Welch accumulation of the segments that range completes.  The slot is free
+// once the convolution has read it, so the next copy in does not wait for the Welch kernel.
+int dspb200_filt_welch_exec(dspb200_os_plan* os, dspb200_spec_plan* spec, const void* x_host, int64_t n, double r,
+                            void* out_host) {
+    DSP_RANGE("dspb200_filt_welch_exec");
+    DSP_REQUIRE(os && spec && out_host, "NULL argument");
+    DSP_REQUIRE(n >= 0, "n must be >= 0");
+    DSP_REQUIRE(r != 0.0, "r must be nonzero");
+    SpecPlanImpl* p = &spec->impl;
+    HostPipe& hp = p->pipe;
+    int64_t nv = 0, nfft = 0;
+    int dt_os = 0;
+    DSP_TRY(dspb200_os_plan_geometry(os, &dt_os, &nv, &nfft));
+    DSP_REQUIRE(dt_os == p->dtype, "filter plan dtype (%d) and Welch plan dtype (%d) differ", dt_os, p->dtype);
+    const int64_t k = nsegments(p, n);
+    DSP_REQUIRE(k == 0 || x_host != nullptr, "x is NULL");
+    DSP_TRY(ensure_streams(p));
+    const size_t esz = dtype_size(p->dtype);
+    const int64_t halo = nv - 1, L = nfft - nv + 1;
+    int64_t chunk = ((int64_t(32) << 20) / (int64_t)esz) / L * L;         // whole overlap-save blocks, ~32 MiB of new samples
+    if (chunk < L) chunk = L;
+    if (chunk > n) chunk = n;
+    DSP_TRY(hp.out[0].reserve((size_t)p->nout * (p->f64 ? 8 : 4)));
+    if (k > 0) DSP_TRY(p->y.reserve((size_t)n * esz));
+    DSP_TRY(welch_begin(p, hp.s_exec));
+    auto chunk_at = [&](int64_t c) -> Chunk {
+        const int64_t c0 = c * chunk, c1 = c0 + chunk < n ? c0 + chunk : n, in0 = c0 - halo > 0 ? c0 - halo : 0;
+        char* y = (char*)p->y.p;
+        auto filter = [=, &hp](const void* in, void*) {    // y[c0, c1) = (b * x)[c0, c1); the slot holds x[in0, c1)
+            return dspb200_os_exec_range_dev(os, in, in0, c1 - in0, y + (size_t)c0 * esz, c0, c1 - c0, hp.s_exec);
+        };
+        auto accumulate = [=, &hp] {                       // the segments that end in [c0, c1)
+            return welch_accumulate(p, y, 0, nsegments(p, c0), nsegments(p, c1), hp.s_exec);
+        };
+        return {(const char*)x_host + (size_t)in0 * esz, (size_t)(c1 - in0) * esz, filter, accumulate};
+    };
+    return run_chunked(hp, k > 0 ? cdiv(n, chunk) : 0, (size_t)(chunk + halo) * esz, 0, chunk_at,
+                       [&] { return welch_finalize_host(p, r, out_host); });
 }
 
 // arraysplit / ArraySplit (src/periodograms.jl:32-73, 134-137): all k windowed, zero-padded segments as a k x nfft
@@ -2120,12 +2144,12 @@ int dspb200_arraysplit_exec(dspb200_spec_plan* plan, const void* s, int64_t len,
     DSP_REQUIRE(s && out, "NULL argument");
     DSP_TRY(ensure_streams(p));
     const size_t esz = dtype_size(p->dtype);
-    return run_staged(p->s_exec, {{s, (size_t)len * esz, &p->in[0]}}, {{out, (size_t)(k * p->nfft) * esz, &p->out}}, [&]() -> int {
+    return run_staged(p->pipe.s_exec, {{s, (size_t)len * esz, &p->pipe.in[0]}}, {{out, (size_t)(k * p->nfft) * esz, &p->pipe.out[0]}}, [&]() -> int {
         const int64_t total = k * p->nfft;
         const int threads = 256;
         const int grid = (int)(cdiv(total, threads) < 65535 * 8 ? cdiv(total, threads) : 65535 * 8);
-#define SEGK(T_, C_) seg_window_kernel<T_, C_><<<grid, threads, 0, p->s_exec>>>(p->in[0].p, 0, p->hop, p->n, p->nfft, k, k, \
-        reinterpret_cast<const typename win_t<T_>::type*>(p->d_window), p->out.p)
+#define SEGK(T_, C_) seg_window_kernel<T_, C_><<<grid, threads, 0, p->pipe.s_exec>>>(p->pipe.in[0].p, 0, p->hop, p->n, p->nfft, k, k, \
+        reinterpret_cast<const typename win_t<T_>::type*>(p->d_window), p->pipe.out[0].p)
         if (p->f64) { if (p->cplx) SEGK(double, true); else SEGK(double, false); }
         else { if (p->cplx) SEGK(float, true); else SEGK(float, false); }
 #undef SEGK
@@ -2175,8 +2199,8 @@ int dspb200_stft_exec(dspb200_spec_plan* plan, const void* s, int64_t len, int64
     DSP_REQUIRE(s && out, "NULL argument");
     DSP_TRY(ensure_streams(p));
     const size_t oel = psd_only ? (p->f64 ? 8 : 4) : (p->f64 ? 16 : 8);
-    return run_staged(p->s_exec, {{s, (size_t)len * nchan * dtype_size(p->dtype), &p->in[0]}}, {{out, (size_t)p->nout * k * nchan * oel, &p->out}},
-                      [&] { return dspb200_stft_exec_dev(plan, p->in[0].p, len, nchan, r, psd_only, p->out.p, p->s_exec); });
+    return run_staged(p->pipe.s_exec, {{s, (size_t)len * nchan * dtype_size(p->dtype), &p->pipe.in[0]}}, {{out, (size_t)p->nout * k * nchan * oel, &p->pipe.out[0]}},
+                      [&] { return dspb200_stft_exec_dev(plan, p->pipe.in[0].p, len, nchan, r, psd_only, p->pipe.out[0].p, p->pipe.s_exec); });
 }
 
 // Streaming calls (STFT and Welch).  Checks shared by every form: sizes, the history, the segments and, device form, the
@@ -2264,10 +2288,10 @@ int dspb200_stft_stream_exec(dspb200_spec_plan* plan, const void* hist_in, int64
     const size_t esz = dtype_size(p->dtype), oel = (psd_only ? 1 : 2) * (p->f64 ? 8 : 4);
     const size_t hbytes = (size_t)(ldh * nchan) * esz;
     const size_t obytes = nseg ? (size_t)(((nchan - 1) * ldo + nseg) * p->nout) * oel : 0;
-    return run_staged(p->s_exec, {{x, (size_t)(nx * nchan) * esz, &p->in[0]}, {hist_in, hist_in ? hbytes : 0, &p->hin}},
-                      {{out, obytes, &p->out}, {hist_out, newh ? hbytes : 0, &p->hout}}, [&] {
-                          return dspb200_stft_stream_exec_dev(plan, hist_in ? p->hin.p : nullptr, nhist, p->hout.p, ldh, p->in[0].p,
-                                                              nx, nchan, nseg, r, psd_only, p->out.p, ldo, p->s_exec);
+    return run_staged(p->pipe.s_exec, {{x, (size_t)(nx * nchan) * esz, &p->pipe.in[0]}, {hist_in, hist_in ? hbytes : 0, &p->hin}},
+                      {{out, obytes, &p->pipe.out[0]}, {hist_out, newh ? hbytes : 0, &p->hout}}, [&] {
+                          return dspb200_stft_stream_exec_dev(plan, hist_in ? p->hin.p : nullptr, nhist, p->hout.p, ldh, p->pipe.in[0].p,
+                                                              nx, nchan, nseg, r, psd_only, p->pipe.out[0].p, ldo, p->pipe.s_exec);
                       });
 }
 
@@ -2322,10 +2346,10 @@ int dspb200_welch_stream_exec(dspb200_spec_plan* plan, const void* hist_in, int6
     DSP_TRY(ensure_streams(p));
     const size_t esz = dtype_size(p->dtype);
     const size_t hbytes = (size_t)(ldh * nchan) * esz, abytes = nseg ? (size_t)(p->nout * nchan) * sizeof(double) : 0;
-    return run_staged(p->s_exec, {{x, (size_t)(nx * nchan) * esz, &p->in[0]}, {hist_in, hist_in ? hbytes : 0, &p->hin}, {acc, add ? abytes : 0, &p->out}},
-                      {{acc, abytes, &p->out}, {hist_out, newh ? hbytes : 0, &p->hout}}, [&] {
-                          return dspb200_welch_stream_exec_dev(plan, hist_in ? p->hin.p : nullptr, nhist, p->hout.p, ldh, p->in[0].p,
-                                                               nx, nchan, nseg, reinterpret_cast<double*>(p->out.p), add, p->s_exec);
+    return run_staged(p->pipe.s_exec, {{x, (size_t)(nx * nchan) * esz, &p->pipe.in[0]}, {hist_in, hist_in ? hbytes : 0, &p->hin}, {acc, add ? abytes : 0, &p->pipe.out[0]}},
+                      {{acc, abytes, &p->pipe.out[0]}, {hist_out, newh ? hbytes : 0, &p->hout}}, [&] {
+                          return dspb200_welch_stream_exec_dev(plan, hist_in ? p->hin.p : nullptr, nhist, p->hout.p, ldh, p->pipe.in[0].p,
+                                                               nx, nchan, nseg, reinterpret_cast<double*>(p->pipe.out[0].p), add, p->pipe.s_exec);
                       });
 }
 
@@ -2366,8 +2390,8 @@ int dspb200_welch_stream_power(dspb200_spec_plan* plan, const double* acc, int64
     DSP_REQUIRE(acc && out, "NULL argument");
     DSP_TRY(ensure_streams(p));
     const size_t n = (size_t)(p->nout * nchan);
-    return run_staged(p->s_exec, {{acc, n * sizeof(double), &p->in[0]}}, {{out, n * (p->f64 ? 8 : 4), &p->out}}, [&] {
-        return dspb200_welch_stream_power_dev(plan, reinterpret_cast<const double*>(p->in[0].p), nchan, r, p->out.p, p->s_exec);
+    return run_staged(p->pipe.s_exec, {{acc, n * sizeof(double), &p->pipe.in[0]}}, {{out, n * (p->f64 ? 8 : 4), &p->pipe.out[0]}}, [&] {
+        return dspb200_welch_stream_power_dev(plan, reinterpret_cast<const double*>(p->pipe.in[0].p), nchan, r, p->pipe.out[0].p, p->pipe.s_exec);
     });
 }
 
@@ -2405,8 +2429,8 @@ int dspb200_mt_pgram_exec(dspb200_spec_plan* plan, const void* s, int64_t len, v
     DSP_TRY(mt_pgram_check(plan, s, len, out));
     SpecPlanImpl* p = &plan->impl;
     DSP_TRY(ensure_streams(p));
-    return run_staged(p->s_exec, {{s, (size_t)len * dtype_size(p->dtype), &p->in[0]}}, {{out, (size_t)p->nout * (p->f64 ? 8 : 4), &p->out}},
-                      [&] { return dspb200_mt_pgram_exec_dev(plan, p->in[0].p, len, p->out.p, p->s_exec); });
+    return run_staged(p->pipe.s_exec, {{s, (size_t)len * dtype_size(p->dtype), &p->pipe.in[0]}}, {{out, (size_t)p->nout * (p->f64 ? 8 : 4), &p->pipe.out[0]}},
+                      [&] { return dspb200_mt_pgram_exec_dev(plan, p->pipe.in[0].p, len, p->pipe.out[0].p, p->pipe.s_exec); });
 }
 
 int dspb200_mt_spectrogram_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t len, void* d_out, void* stream) {
@@ -2453,8 +2477,8 @@ int dspb200_mt_spectrogram_exec(dspb200_spec_plan* plan, const void* s, int64_t 
     if (k == 0) return DSPB200_OK;
     DSP_REQUIRE(s && out, "NULL argument");
     DSP_TRY(ensure_streams(p));
-    return run_staged(p->s_exec, {{s, (size_t)len * dtype_size(p->dtype), &p->in[0]}}, {{out, (size_t)(p->nout * k) * (p->f64 ? 8 : 4), &p->out}},
-                      [&] { return dspb200_mt_spectrogram_exec_dev(plan, p->in[0].p, len, p->out.p, p->s_exec); });
+    return run_staged(p->pipe.s_exec, {{s, (size_t)len * dtype_size(p->dtype), &p->pipe.in[0]}}, {{out, (size_t)(p->nout * k) * (p->f64 ? 8 : 4), &p->pipe.out[0]}},
+                      [&] { return dspb200_mt_spectrogram_exec_dev(plan, p->pipe.in[0].p, len, p->pipe.out[0].p, p->pipe.s_exec); });
 }
 
 static int mt_cross_entry(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int demean, int64_t f_lo, int64_t nf,
@@ -2469,7 +2493,7 @@ static int mt_cross_entry(dspb200_spec_plan* plan, const void* signal, int64_t n
     if (nf == 0) return DSPB200_OK;
     DSP_REQUIRE(signal && out, "NULL argument");
     DSP_TRY(ensure_streams(p));
-    if (!dev) st = p->s_exec;
+    if (!dev) st = p->pipe.s_exec;
     return settle(st, p->f64 ? mt_cross_run<double>(plan, signal, nchan, demean, f_lo, nf, coherence, out, dev, st)
                              : mt_cross_run<float>(plan, signal, nchan, demean, f_lo, nf, coherence, out, dev, st));
 }
@@ -2516,14 +2540,9 @@ int dspb200_spec_plan_destroy(dspb200_spec_plan* plan) {
     if (p->d_t32) cudaFree(p->d_t32);
     if (p->d_t256) cudaFree(p->d_t256);
     p->partial.release(); p->bpartial.release(); p->bacc.release(); p->segbuf.release(); p->specbuf.release(); p->acc.release();
-    p->in[0].release(); p->in[1].release(); p->out.release(); p->tmp.release(); p->hin.release(); p->hout.release(); p->seam.release();
+    p->tmp.release(); p->hin.release(); p->hout.release(); p->seam.release(); p->y.release();
     if (p->fft_ok) cufftDestroy(p->fft);
-    for (int i = 0; i < 2; ++i) {
-        if (p->ev_in[i]) cudaEventDestroy(p->ev_in[i]);
-        if (p->ev_done[i]) cudaEventDestroy(p->ev_done[i]);
-    }
-    if (p->s_copy) cudaStreamDestroy(p->s_copy);
-    if (p->s_exec) cudaStreamDestroy(p->s_exec);
+    p->pipe.release();
     delete plan;
     return DSPB200_OK;
 }
