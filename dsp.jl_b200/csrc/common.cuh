@@ -211,11 +211,29 @@ void count_launch(int n = 1);
 // cached: round 1 created and destroyed two plans and up to six allocations per call.  `plan_cache_get` returns a handle
 // owned by the cache (never destroy it); `embed` selects inembed = onembed = n with the given distances (hilbert's
 // real -> complex plan), otherwise the default packed layout.  The cache keeps the 32 most recently used plans per
-// process; callers serialise on `convenience_lock()` for the duration of the call (the entry points are synchronous).
+// process; the calls that use them go through `convenience_call` below, which serialises them (they are synchronous).
 int plan_cache_get(int* handle, int rank, const long long* n, bool embed, long long idist, long long odist, int type, long long batch);
 DevBuf& scratch_buf(int slot);            // per-process grow-only device buffers, slot 0..7
 void scratch_trim(size_t keep_bytes);     // release the buffers larger than keep_bytes
 struct ConvenienceLock { ConvenienceLock(); ~ConvenienceLock(); };
+
+// The one exit of the plan-less entry points: under the ConvenienceLock, queue(st) queues the call's work on st, the call
+// returns once st is idle, on success and failure alike, and the arena then drops its large buffers (the plans and the
+// small buffers stay for the next call).  queue() neither locks nor trims, so that no buffer it uses is freed under it.
+// Device-pointer form:
+template <class F> int convenience_call(cudaStream_t st, F&& queue) {
+    ConvenienceLock lock;
+    const int rc = settle(st, queue(st));
+    scratch_trim((size_t)256 << 20);
+    return rc;
+}
+// Host-pointer form: queue(0) between the copies of run_staged (the staging buffers are arena slots).
+template <class F> int convenience_call(std::initializer_list<HostIn> in, std::initializer_list<HostOut> out, F&& queue) {
+    ConvenienceLock lock;
+    const int rc = run_staged(0, in, out, [&] { return queue(cudaStream_t(0)); });
+    scratch_trim((size_t)256 << 20);
+    return rc;
+}
 
 // after every kernel launch
 #define DSP_LAUNCH_OK()                                                              \

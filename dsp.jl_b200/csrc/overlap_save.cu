@@ -11,7 +11,7 @@
 // H carries the 1/nfft of the unnormalised inverse (src/dspbase.jl:516, src/Filters/filt.jl:498).
 #include "fft_core.cuh"
 #include "async_copy.cuh"
-#include <cufft.h>
+#include "cufft_exec.cuh"
 #include <math.h>
 #include <stdlib.h>
 #include <new>
@@ -526,8 +526,9 @@ __global__ void nd_copy_kernel(const E* __restrict__ src, Dims3 s, E* __restrict
 // _conv_td!, src/dspbase.jl:646-660, N-D: out[k] = sum of u[m] * v[n] over m + n = k, one output per thread.  The reference
 // loops `for m in CartesianIndices(u), n in CartesianIndices(v)` when size(u,1) <= size(v,1), else with n outer: every
 // output sums its products in the column-major order of the outer array's index (dim 1 fastest), each step
-// muladd(u[m], v[n], acc).  The walk below is over that array (w), the other one (o) read at k - j.
-template <typename T, bool CPLX>
+// muladd(u[m], v[n], acc).  The walk below is over that array (w), the other one (o) read at k - j.  RANK1: rank 1, no index
+// decomposition (its 64-bit divisions took a 2048 x 31 Float32 call from 0.035 to 0.040 ms: H100 80GB HBM3, 700 W).
+template <typename T, bool CPLX, bool RANK1>
 __global__ void conv_direct_nd_kernel(const void* __restrict__ u_, Dims3 su, const void* __restrict__ v_, Dims3 sv,
                                       void* __restrict__ out_) {
     using E = typename os_elt<T, CPLX>::type;
@@ -539,7 +540,7 @@ __global__ void conv_direct_nd_kernel(const void* __restrict__ u_, Dims3 su, con
     const int64_t o0 = su.n[0] + sv.n[0] - 1, o1 = su.n[1] + sv.n[1] - 1, o2 = su.n[2] + sv.n[2] - 1;
     const int64_t total = o0 * o1 * o2;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t k0 = i % o0, k1 = (i / o0) % o1, k2 = i / (o0 * o1);
+        const int64_t k0 = RANK1 ? i : i % o0, k1 = RANK1 ? 0 : (i / o0) % o1, k2 = RANK1 ? 0 : i / (o0 * o1);
         T ar = T(0), ai = T(0);
         for (int64_t m2 = max(k2 - (so.n[2] - 1), (int64_t)0); m2 <= min(k2, sw.n[2] - 1); ++m2)
             for (int64_t m1 = max(k1 - (so.n[1] - 1), (int64_t)0); m1 <= min(k1, sw.n[1] - 1); ++m1)
@@ -649,39 +650,6 @@ __global__ void scale_cplx_kernel(cx<T>* __restrict__ X, int64_t n, T scale) {
         X[i] = cscale(X[i], scale);
 }
 
-// direct convolution, src/dspbase.jl:646-660, 1-D.  The reference loops `for m in u, n in v` when length(u) <= length(v)
-// and `for n in v, m in u` otherwise; the first iterator is the outer one, so every output sums its products in ascending
-// index of the SHORTER array (u on a tie), each step muladd(u[m], v[n], acc): the walk below, one output per thread.
-template <typename T, bool CPLX>
-__global__ void conv_direct_kernel(const void* __restrict__ u_, int64_t nu, const void* __restrict__ v_, int64_t nv,
-                                   void* __restrict__ out_) {
-    using E = typename os_elt<T, CPLX>::type;
-    const bool walk_u = nu <= nv;
-    const E* w = reinterpret_cast<const E*>(walk_u ? u_ : v_);          // the array whose index is the outer loop
-    const E* o = reinterpret_cast<const E*>(walk_u ? v_ : u_);
-    const int64_t nw = walk_u ? nu : nv, no = walk_u ? nv : nu;
-    E* out = reinterpret_cast<E*>(out_);
-    const int64_t nout = nu + nv - 1;
-    for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < nout; k += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t lo = k - (no - 1) > 0 ? k - (no - 1) : 0;
-        const int64_t hi = k < nw - 1 ? k : nw - 1;
-        if constexpr (CPLX) {
-            cx<T> acc = mkc<T>(T(0), T(0));
-            for (int64_t j = lo; j <= hi; ++j) {
-                const cx<T> p = w[j], q = o[k - j];
-                const cx<T> a = walk_u ? p : q, b = walk_u ? q : p;      // a = u[m], b = v[n]: Base.muladd(a, b, acc)
-                acc.x = fma(a.x, b.x, fma(-a.y, b.y, acc.x));
-                acc.y = fma(a.x, b.y, fma(a.y, b.x, acc.y));
-            }
-            out[k] = acc;
-        } else {
-            T acc = T(0);
-            for (int64_t j = lo; j <= hi; ++j) acc = fma(w[j], o[k - j], acc);
-            out[k] = acc;
-        }
-    }
-}
-
 // ---------------------------------------------------------------------------------------------- dispatch
 #define DSP_OS_SIZES(X) X(32) X(64) X(128) X(256) X(512) X(1024) X(2048) X(4096) X(8192) X(16384)
 
@@ -785,64 +753,12 @@ template <typename T> static int os_filter_dispatch(OsPlanImpl* p, const void* d
     return DSPB200_EUNSUPPORTED;
 }
 
-static int cufft_fail(cufftResult r, const char* what) {
-    set_error("cuFFT error %d in %s", (int)r, what);
-    return DSPB200_ECUFFT;
-}
-#define DSP_CUFFT(call)                                          \
-    do {                                                         \
-        cufftResult r__ = (call);                                \
-        if (r__ != CUFFT_SUCCESS) return cufft_fail(r__, #call); \
-    } while (0)
-
 static int grid_for(int64_t total, int threads) {
     int64_t g = cdiv(total, threads);
     const int64_t cap = (int64_t)device_sm_count() * 64;
     if (g > cap) g = cap;
     if (g < 1) g = 1;
     return (int)g;
-}
-
-// forward / inverse transforms of `batch` rows held in td (time) and fd (frequency)
-static int generic_exec_fwd(OsPlanImpl* p, cufftHandle h, void* td, void* fd, cudaStream_t st) {
-    DSP_CUFFT(cufftSetStream(h, st));
-    if (p->cplx) {
-        if (p->f64) DSP_CUFFT(cufftExecZ2Z(h, (cufftDoubleComplex*)td, (cufftDoubleComplex*)fd, CUFFT_FORWARD));
-        else DSP_CUFFT(cufftExecC2C(h, (cufftComplex*)td, (cufftComplex*)fd, CUFFT_FORWARD));
-    } else {
-        if (p->f64) DSP_CUFFT(cufftExecD2Z(h, (cufftDoubleReal*)td, (cufftDoubleComplex*)fd));
-        else DSP_CUFFT(cufftExecR2C(h, (cufftReal*)td, (cufftComplex*)fd));
-    }
-    count_launch(1);
-    return DSPB200_OK;
-}
-static int generic_exec_inv(OsPlanImpl* p, cufftHandle h, void* fd, void* td, cudaStream_t st) {
-    DSP_CUFFT(cufftSetStream(h, st));
-    if (p->cplx) {
-        if (p->f64) DSP_CUFFT(cufftExecZ2Z(h, (cufftDoubleComplex*)fd, (cufftDoubleComplex*)td, CUFFT_INVERSE));
-        else DSP_CUFFT(cufftExecC2C(h, (cufftComplex*)fd, (cufftComplex*)td, CUFFT_INVERSE));
-    } else {
-        if (p->f64) DSP_CUFFT(cufftExecZ2D(h, (cufftDoubleComplex*)fd, (cufftDoubleReal*)td));
-        else DSP_CUFFT(cufftExecC2R(h, (cufftComplex*)fd, (cufftReal*)td));
-    }
-    count_launch(1);
-    return DSPB200_OK;
-}
-
-static int make_plans(bool cplx, bool f64, int64_t nfft, int64_t batch, cufftHandle* fwd, cufftHandle* inv) {
-    long long nn[1] = {(long long)nfft};
-    size_t ws = 0;
-    DSP_CUFFT(cufftCreate(fwd));
-    DSP_CUFFT(cufftCreate(inv));
-    if (cplx) {
-        const cufftType t = f64 ? CUFFT_Z2Z : CUFFT_C2C;
-        DSP_CUFFT(cufftMakePlanMany64(*fwd, 1, nn, nullptr, 1, 0, nullptr, 1, 0, t, batch, &ws));
-        DSP_CUFFT(cufftMakePlanMany64(*inv, 1, nn, nullptr, 1, 0, nullptr, 1, 0, t, batch, &ws));
-    } else {
-        DSP_CUFFT(cufftMakePlanMany64(*fwd, 1, nn, nullptr, 1, 0, nullptr, 1, 0, f64 ? CUFFT_D2Z : CUFFT_R2C, batch, &ws));
-        DSP_CUFFT(cufftMakePlanMany64(*inv, 1, nn, nullptr, 1, 0, nullptr, 1, 0, f64 ? CUFFT_Z2D : CUFFT_C2R, batch, &ws));
-    }
-    return DSPB200_OK;
 }
 
 template <typename T, bool STATE> static int os_generic_run(OsPlanImpl* p, const OsRange& a, const OsStateArgs& s, cudaStream_t st) {
@@ -858,10 +774,10 @@ template <typename T, bool STATE> static int os_generic_run(OsPlanImpl* p, const
             if (p->cplx) os_gather_kernel<T, true><<<grid_for(p->batch * p->nfft, threads), threads, 0, st>>>(ucol, a.u_begin, a.nu_local, m_first, p->L, p->nv, p->nfft, p->batch, p->td.p);
             else os_gather_kernel<T, false><<<grid_for(p->batch * p->nfft, threads), threads, 0, st>>>(ucol, a.u_begin, a.nu_local, m_first, p->L, p->nv, p->nfft, p->batch, p->td.p);
             DSP_LAUNCH_OK();
-            DSP_TRY(generic_exec_fwd(p, p->fwd, p->td.p, p->fd.p, st));
+            DSP_TRY(fft_exec(p->fwd, p->cplx, p->f64, CUFFT_FORWARD, p->td.p, p->fd.p, st));
             os_cmul_kernel<T><<<grid_for(p->batch * p->nbins, threads), threads, 0, st>>>(reinterpret_cast<cx<T>*>(p->fd.p), reinterpret_cast<const cx<T>*>(p->d_H), p->nbins, p->batch);
             DSP_LAUNCH_OK();
-            DSP_TRY(generic_exec_inv(p, p->inv, p->fd.p, p->td.p, st));
+            DSP_TRY(fft_exec(p->inv, p->cplx, p->f64, CUFFT_INVERSE, p->fd.p, p->td.p, st));
             if (p->cplx) os_scatter_kernel<T, true, STATE><<<grid_for(nblk * p->L, threads), threads, 0, st>>>(p->td.p, m_first, p->L, p->nv, p->nfft, nblk, ocol, a.out_begin, a.out_begin + a.out_count, a.zero_from, os_state_arg<cx<T>, STATE>(s, c * (p->nv - 1)));
             else os_scatter_kernel<T, false, STATE><<<grid_for(nblk * p->L, threads), threads, 0, st>>>(p->td.p, m_first, p->L, p->nv, p->nfft, nblk, ocol, a.out_begin, a.out_begin + a.out_count, a.zero_from, os_state_arg<T, STATE>(s, c * (p->nv - 1)));
             DSP_LAUNCH_OK();
@@ -902,7 +818,7 @@ struct dspb200_os_plan {
     OsPlanImpl impl;
 };
 
-// conv(u, v) for rank-2 / rank-3 arrays on device pointers: _conv_td! (mode 0), _conv_kern_fft! (mode 1: one N-D FFT pair of
+// conv(u, v) for arrays of rank 1 to 3 on device pointers: _conv_td! (mode 0), _conv_kern_fft! (mode 1: one N-D FFT pair of
 // size nffts) or unsafe_conv_kern_os! (mode 2: blocks of nffts, batched).  Plans and scratch come from the cache / arena of
 // runtime.cu; the caller holds the ConvenienceLock and synchronises the stream before the arena is reused.
 enum { ND_DIRECT = 0, ND_FFT = 1, ND_OS = 2 };
@@ -920,7 +836,8 @@ static int conv_nd_dev(int mode, int rank, const int64_t* usize, const void* d_u
     const int64_t no = so.n[0] * so.n[1] * so.n[2];
     const int threads = 256;
     if (mode == ND_DIRECT) {
-        conv_direct_nd_kernel<T, CPLX><<<grid_for(no, 128), 128, 0, st>>>(d_u, su, d_v, sv, d_out);
+        auto kern = rank == 1 ? conv_direct_nd_kernel<T, CPLX, true> : conv_direct_nd_kernel<T, CPLX, false>;
+        kern<<<grid_for(no, 128), 128, 0, st>>>(d_u, su, d_v, sv, d_out);
         DSP_LAUNCH_OK();
         return DSPB200_OK;
     }
@@ -932,10 +849,7 @@ static int conv_nd_dev(int mode, int rank, const int64_t* usize, const void* d_u
     long long nn[3];                                         // cuFFT is row-major: slowest dimension first
     for (int d = 0; d < rank; ++d) nn[d] = (long long)sf.n[rank - 1 - d];
     const bool f64 = sizeof(T) == 8;
-    const int tf = CPLX ? (f64 ? CUFFT_Z2Z : CUFFT_C2C) : (f64 ? CUFFT_D2Z : CUFFT_R2C);
-    const int ti = CPLX ? tf : (f64 ? CUFFT_Z2D : CUFFT_C2R);
-    OsPlanImpl tmp;
-    tmp.cplx = CPLX; tmp.f64 = f64;
+    const int tf = fft_type(CPLX, f64, CUFFT_FORWARD), ti = fft_type(CPLX, f64, CUFFT_INVERSE);
     E zero;
     if constexpr (CPLX) zero = mkc<T>(T(0), T(0)); else zero = T(0);
     int h1f = 0;
@@ -947,14 +861,14 @@ static int conv_nd_dev(int mode, int rank, const int64_t* usize, const void* d_u
         DSP_TRY(fu.reserve((size_t)nb * sizeof(cx<T>))); DSP_TRY(fv.reserve((size_t)nb * sizeof(cx<T>)));
         nd_copy_kernel<E><<<grid_for(nf, threads), threads, 0, st>>>((const E*)d_u, su, (E*)tu.p, sf, zero);
         DSP_LAUNCH_OK();
-        DSP_TRY(generic_exec_fwd(&tmp, (cufftHandle)h1f, tu.p, fu.p, st));
+        DSP_TRY(fft_exec((cufftHandle)h1f, CPLX, f64, CUFFT_FORWARD, tu.p, fu.p, st));
         nd_copy_kernel<E><<<grid_for(nf, threads), threads, 0, st>>>((const E*)d_v, sv, (E*)tu.p, sf, zero);
         DSP_LAUNCH_OK();
-        DSP_TRY(generic_exec_fwd(&tmp, (cufftHandle)h1f, tu.p, fv.p, st));
+        DSP_TRY(fft_exec((cufftHandle)h1f, CPLX, f64, CUFFT_FORWARD, tu.p, fv.p, st));
         scale_cplx_kernel<T><<<grid_for(nb, threads), threads, 0, st>>>((cx<T>*)fv.p, nb, T(1) / (T)nf);
         os_cmul_kernel<T><<<grid_for(nb, threads), threads, 0, st>>>((cx<T>*)fu.p, (const cx<T>*)fv.p, nb, 1);
         count_launch(2);
-        DSP_TRY(generic_exec_inv(&tmp, (cufftHandle)h1i, fu.p, tu.p, st));
+        DSP_TRY(fft_exec((cufftHandle)h1i, CPLX, f64, CUFFT_INVERSE, fu.p, tu.p, st));
         nd_copy_kernel<E><<<grid_for(no, threads), threads, 0, st>>>((const E*)tu.p, sf, (E*)d_out, so, zero);
         DSP_LAUNCH_OK();
         return DSPB200_OK;
@@ -981,16 +895,16 @@ static int conv_nd_dev(int mode, int rank, const int64_t* usize, const void* d_u
     // filter spectrum, scaled once by 1/prod(nffts) (:513-516)
     nd_copy_kernel<E><<<grid_for(nf, threads), threads, 0, st>>>((const E*)d_v, sv, (E*)tu.p, sf, zero);
     DSP_LAUNCH_OK();
-    DSP_TRY(generic_exec_fwd(&tmp, (cufftHandle)h1f, tu.p, fv.p, st));
+    DSP_TRY(fft_exec((cufftHandle)h1f, CPLX, f64, CUFFT_FORWARD, tu.p, fv.p, st));
     scale_cplx_kernel<T><<<grid_for(nb, threads), threads, 0, st>>>((cx<T>*)fv.p, nb, T(1) / (T)nf);
     DSP_LAUNCH_OK();
     for (int64_t b0 = 0; b0 < nblocks; b0 += batch) {
         nd_os_gather_kernel<E><<<grid_for(nf * batch, threads), threads, 0, st>>>((const E*)d_u, g, b0, batch, (E*)tu.p, zero);
         DSP_LAUNCH_OK();
-        DSP_TRY(generic_exec_fwd(&tmp, (cufftHandle)hbf, tu.p, fu.p, st));
+        DSP_TRY(fft_exec((cufftHandle)hbf, CPLX, f64, CUFFT_FORWARD, tu.p, fu.p, st));
         os_cmul_kernel<T><<<grid_for(nb * batch, threads), threads, 0, st>>>((cx<T>*)fu.p, (const cx<T>*)fv.p, nb, batch);
         DSP_LAUNCH_OK();
-        DSP_TRY(generic_exec_inv(&tmp, (cufftHandle)hbi, fu.p, tu.p, st));
+        DSP_TRY(fft_exec((cufftHandle)hbi, CPLX, f64, CUFFT_INVERSE, fu.p, tu.p, st));
         nd_os_scatter_kernel<E><<<grid_for(Lp * batch, threads), threads, 0, st>>>((const E*)tu.p, g, b0, batch, (E*)d_out);
         DSP_LAUNCH_OK();
     }
@@ -1026,10 +940,9 @@ static int conv_nd_dispatch(int dtype, int mode, int rank, const int64_t* usize,
 // device-pointer form: returns after the work on `stream` has completed (the cached plans and the arena are shared)
 static int conv_nd_run_dev(int dtype, int mode, int rank, const int64_t* usize, const void* d_u, const int64_t* vsize, const void* d_v,
                            const int64_t* nffts, void* d_out, cudaStream_t st) {
-    ConvenienceLock lock;
-    const int rc = settle(st, conv_nd_dispatch(dtype, mode, rank, usize, d_u, vsize, d_v, nffts, d_out, st));
-    scratch_trim((size_t)256 << 20);                             // plans and small buffers stay cached for the next call
-    return rc;
+    return convenience_call(st, [&](cudaStream_t s) {
+        return conv_nd_dispatch(dtype, mode, rank, usize, d_u, vsize, d_v, nffts, d_out, s);
+    });
 }
 
 // host-pointer form
@@ -1038,12 +951,10 @@ static int conv_nd_run_host(int dtype, int mode, int rank, const int64_t* usize,
     int64_t nu = 1, nv = 1, no = 1;
     for (int d = 0; d < rank; ++d) { nu *= usize[d]; nv *= vsize[d]; no *= usize[d] + vsize[d] - 1; }
     const size_t esz = dtype_size(dtype);
-    ConvenienceLock lock;
     DevBuf &du = scratch_buf(0), &dv = scratch_buf(1), &dout = scratch_buf(2);
-    const int rc = run_staged(0, {{u, (size_t)nu * esz, &du}, {v, (size_t)nv * esz, &dv}}, {{out, (size_t)no * esz, &dout}},
-                              [&] { return conv_nd_dispatch(dtype, mode, rank, usize, du.p, vsize, dv.p, nffts, dout.p, 0); });
-    scratch_trim((size_t)256 << 20);
-    return rc;
+    return convenience_call({{u, (size_t)nu * esz, &du}, {v, (size_t)nv * esz, &dv}}, {{out, (size_t)no * esz, &dout}}, [&](cudaStream_t s) {
+        return conv_nd_dispatch(dtype, mode, rank, usize, du.p, vsize, dv.p, nffts, dout.p, s);
+    });
 }
 
 extern "C" {
@@ -1085,7 +996,8 @@ int dspb200_os_plan_create(dspb200_os_plan** plan, int dtype, const void* v_host
             if (b < 1) b = 1;
             if (b > 4096) b = 4096;
             p->batch = b;
-            rc = make_plans(p->cplx, p->f64, p->nfft, b, &p->fwd, &p->inv);
+            rc = fft_plan_1d(&p->fwd, p->cplx, p->f64, CUFFT_FORWARD, p->nfft, b);
+            if (rc == DSPB200_OK) rc = fft_plan_1d(&p->inv, p->cplx, p->f64, CUFFT_INVERSE, p->nfft, b);
             if (rc != DSPB200_OK) break;
             p->fft_ok = true;
             rc = p->td.reserve((size_t)(b * p->nfft) * esz);
@@ -1105,7 +1017,7 @@ int dspb200_os_plan_create(dspb200_os_plan** plan, int dtype, const void* v_host
                 else pad_copy_kernel<float, false><<<grid_for(p->nfft, threads), threads>>>(d_v, nv, p->td.p, p->nfft, 1.0f / (float)p->nfft);
             }
             count_launch(1);
-            rc = generic_exec_fwd(p, p->fwd, p->td.p, p->fd.p, 0);
+            rc = fft_exec(p->fwd, p->cplx, p->f64, CUFFT_FORWARD, p->td.p, p->fd.p, 0);
             if (rc != DSPB200_OK) break;
             e = cudaMemcpy(p->d_H, p->fd.p, (size_t)p->nbins * csz, cudaMemcpyDeviceToDevice);
             if (e == cudaSuccess) e = cudaDeviceSynchronize();
@@ -1240,67 +1152,11 @@ int dspb200_os_plan_destroy(dspb200_os_plan* plan) {
     return DSPB200_OK;
 }
 
-// _conv_kern_fft!, src/dspbase.jl:611-644 (host pointers; cuFFT plans and scratch from the process-wide cache)
+// _conv_kern_fft!, src/dspbase.jl:611-644: the rank-1 transform pair of dspb200_conv_nd_exec (host pointers)
 int dspb200_conv_fft_exec(int dtype, const void* u, int64_t nu, const void* v, int64_t nv, int64_t nfft, void* out) {
     DSP_RANGE("dspb200_conv_fft_exec");
-    DSP_REQUIRE(dtype_valid(dtype), "invalid dtype %d", dtype);
-    DSP_REQUIRE(u && v && out && nu >= 1 && nv >= 1, "empty or NULL input");
-    const int64_t nout = nu + nv - 1;
-    DSP_REQUIRE(nfft >= nout, "nfft (%lld) must be >= nu+nv-1 (%lld)", (long long)nfft, (long long)nout);
-    DSP_REQUIRE(nfft < (int64_t(1) << 31), "nfft too large");
-    OsPlanImpl tmp;
-    tmp.dtype = dtype; tmp.cplx = dtype_is_cplx(dtype); tmp.f64 = dtype_is_f64(dtype);
-    const size_t esz = dtype_size(dtype), csz = tmp.f64 ? 16 : 8;
-    const int64_t nbins = tmp.cplx ? nfft : nfft / 2 + 1;
-    ConvenienceLock lock;                                       // cached plans + scratch arena (common.cuh)
-    DevBuf &du = scratch_buf(0), &dv = scratch_buf(1), &tu = scratch_buf(3), &fu = scratch_buf(4), &fv = scratch_buf(5);
-    cufftHandle fwd = 0, inv = 0;
-    int rc = DSPB200_OK;
-    auto body = [&]() -> int {
-        DSP_TRY(du.reserve((size_t)nu * esz)); DSP_TRY(dv.reserve((size_t)nv * esz));
-        DSP_TRY(tu.reserve((size_t)nfft * esz));
-        DSP_TRY(fu.reserve((size_t)nbins * csz)); DSP_TRY(fv.reserve((size_t)nbins * csz));
-        DSP_CUDA(cudaMemcpy(du.p, u, (size_t)nu * esz, cudaMemcpyHostToDevice));
-        DSP_CUDA(cudaMemcpy(dv.p, v, (size_t)nv * esz, cudaMemcpyHostToDevice));
-        {
-            long long nn[1] = {(long long)nfft};
-            int hf = 0, hi = 0;
-            if (tmp.cplx) {
-                DSP_TRY(plan_cache_get(&hf, 1, nn, false, 0, 0, tmp.f64 ? CUFFT_Z2Z : CUFFT_C2C, 1));
-                hi = hf;
-            } else {
-                DSP_TRY(plan_cache_get(&hf, 1, nn, false, 0, 0, tmp.f64 ? CUFFT_D2Z : CUFFT_R2C, 1));
-                DSP_TRY(plan_cache_get(&hi, 1, nn, false, 0, 0, tmp.f64 ? CUFFT_Z2D : CUFFT_C2R, 1));
-            }
-            fwd = (cufftHandle)hf; inv = (cufftHandle)hi;
-        }
-        const int threads = 256;
-        const int g = grid_for(nfft, threads);
-#define PAD(SRC, N_) \
-        if (tmp.f64) { if (tmp.cplx) pad_copy_kernel<double, true><<<g, threads>>>(SRC, N_, tu.p, nfft, 1.0); else pad_copy_kernel<double, false><<<g, threads>>>(SRC, N_, tu.p, nfft, 1.0); } \
-        else { if (tmp.cplx) pad_copy_kernel<float, true><<<g, threads>>>(SRC, N_, tu.p, nfft, 1.0f); else pad_copy_kernel<float, false><<<g, threads>>>(SRC, N_, tu.p, nfft, 1.0f); } \
-        count_launch(1);
-        PAD(du.p, nu)
-        DSP_TRY(generic_exec_fwd(&tmp, fwd, tu.p, fu.p, 0));
-        PAD(dv.p, nv)
-        DSP_TRY(generic_exec_fwd(&tmp, fwd, tu.p, fv.p, 0));
-#undef PAD
-        // fv *= 1/nfft ; fu *= fv
-        if (tmp.f64) {
-            scale_cplx_kernel<double><<<grid_for(nbins, threads), threads>>>((cx<double>*)fv.p, nbins, 1.0 / (double)nfft);
-            os_cmul_kernel<double><<<grid_for(nbins, threads), threads>>>((cx<double>*)fu.p, (const cx<double>*)fv.p, nbins, 1);
-        } else {
-            scale_cplx_kernel<float><<<grid_for(nbins, threads), threads>>>((cx<float>*)fv.p, nbins, 1.0f / (float)nfft);
-            os_cmul_kernel<float><<<grid_for(nbins, threads), threads>>>((cx<float>*)fu.p, (const cx<float>*)fv.p, nbins, 1);
-        }
-        count_launch(2);
-        DSP_TRY(generic_exec_inv(&tmp, inv, fu.p, tu.p, 0));
-        DSP_CUDA(cudaMemcpy(out, tu.p, (size_t)nout * esz, cudaMemcpyDeviceToHost));
-        return DSPB200_OK;
-    };
-    rc = body();
-    scratch_trim((size_t)256 << 20);
-    return rc;
+    DSP_TRY(conv_nd_check(dtype, ND_FFT, 1, &nu, u, &nv, v, &nfft, out));
+    return conv_nd_run_host(dtype, ND_FFT, 1, &nu, u, &nv, v, &nfft, out);
 }
 
 // conv(u, v) / conv!(out, u, v) for matrices and rank-3 arrays, src/dspbase.jl:611-660, 709-757 (cached plans)
@@ -1339,79 +1195,50 @@ int dspb200_conv_nd_os_set_budget(size_t bytes) {
 }
 
 // hilbert(x), src/util.jl:31-75 (kernel: hilbert_weight_kernel above)
+static int hilbert_check(int dtype, const void* x, int64_t n, int64_t ncols, const void* out) {
+    DSP_REQUIRE(dtype == DSPB200_F32 || dtype == DSPB200_F64, "hilbert takes a real signal (dtype %d)", dtype);
+    DSP_REQUIRE(x && out && n >= 1 && ncols >= 1, "empty or NULL input");
+    DSP_REQUIRE(n < (int64_t(1) << 31), "n too large");
+    return DSPB200_OK;
+}
+
+// queues the transforms and the weighting on st (cached plans: the caller holds the ConvenienceLock)
+static int hilbert_queue(int dtype, const void* d_x, int64_t n, int64_t ncols, void* d_out, cudaStream_t st) {
+    const bool f64 = dtype == DSPB200_F64;
+    long long nn[1] = {(long long)n};
+    int hf = 0, hi = 0;
+    // real -> complex, column c: n reals at c*n  ->  n/2+1 bins at the start of the n-bin output column c
+    DSP_TRY(plan_cache_get(&hf, 1, nn, true, n, n, fft_type(false, f64, CUFFT_FORWARD), ncols));
+    DSP_TRY(plan_cache_get(&hi, 1, nn, false, 0, 0, fft_type(true, f64, CUFFT_INVERSE), ncols));
+    DSP_TRY(fft_exec((cufftHandle)hf, false, f64, CUFFT_FORWARD, d_x, d_out, st));
+    const int threads = 256, g = grid_for(n * ncols, threads);
+    if (f64) hilbert_weight_kernel<double><<<g, threads, 0, st>>>((cx<double>*)d_out, n, ncols, 1.0 / (double)n);
+    else hilbert_weight_kernel<float><<<g, threads, 0, st>>>((cx<float>*)d_out, n, ncols, 1.0f / (float)n);
+    DSP_LAUNCH_OK();
+    return fft_exec((cufftHandle)hi, true, f64, CUFFT_INVERSE, d_out, d_out, st);
+}
+
 int dspb200_hilbert_exec_dev(int dtype, const void* d_x, int64_t n, int64_t ncols, void* d_out, void* stream) {
     DSP_RANGE("dspb200_hilbert_exec_dev");
-    DSP_REQUIRE(dtype == DSPB200_F32 || dtype == DSPB200_F64, "hilbert takes a real signal (dtype %d)", dtype);
-    DSP_REQUIRE(d_x && d_out && n >= 1 && ncols >= 1, "empty or NULL input");
-    DSP_REQUIRE(n < (int64_t(1) << 31), "n too large");
-    const bool f64 = dtype == DSPB200_F64;
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    cufftHandle fwd = 0, inv = 0;
-    ConvenienceLock lock;                                       // cached plans (common.cuh)
-    auto body = [&]() -> int {
-        long long nn[1] = {(long long)n};
-        int hf = 0, hi = 0;
-        // real -> complex, column c: n reals at c*n  ->  n/2+1 bins at the start of the n-bin output column c
-        DSP_TRY(plan_cache_get(&hf, 1, nn, true, n, n, f64 ? CUFFT_D2Z : CUFFT_R2C, ncols));
-        DSP_TRY(plan_cache_get(&hi, 1, nn, false, 0, 0, f64 ? CUFFT_Z2Z : CUFFT_C2C, ncols));
-        fwd = (cufftHandle)hf; inv = (cufftHandle)hi;
-        DSP_CUFFT(cufftSetStream(fwd, st));
-        DSP_CUFFT(cufftSetStream(inv, st));
-        const int threads = 256, g = grid_for(n * ncols, threads);
-        if (f64) {
-            DSP_CUFFT(cufftExecD2Z(fwd, (cufftDoubleReal*)const_cast<void*>(d_x), (cufftDoubleComplex*)d_out));
-            hilbert_weight_kernel<double><<<g, threads, 0, st>>>((cx<double>*)d_out, n, ncols, 1.0 / (double)n);
-            DSP_LAUNCH_OK();
-            DSP_CUFFT(cufftExecZ2Z(inv, (cufftDoubleComplex*)d_out, (cufftDoubleComplex*)d_out, CUFFT_INVERSE));
-        } else {
-            DSP_CUFFT(cufftExecR2C(fwd, (cufftReal*)const_cast<void*>(d_x), (cufftComplex*)d_out));
-            hilbert_weight_kernel<float><<<g, threads, 0, st>>>((cx<float>*)d_out, n, ncols, 1.0f / (float)n);
-            DSP_LAUNCH_OK();
-            DSP_CUFFT(cufftExecC2C(inv, (cufftComplex*)d_out, (cufftComplex*)d_out, CUFFT_INVERSE));
-        }
-        count_launch(2);
-        DSP_CUDA(cudaStreamSynchronize(st));              // the cached plans may be re-targeted to another stream by the next call
-        return DSPB200_OK;
-    };
-    return body();
+    DSP_TRY(hilbert_check(dtype, d_x, n, ncols, d_out));
+    return convenience_call(reinterpret_cast<cudaStream_t>(stream),
+                            [&](cudaStream_t st) { return hilbert_queue(dtype, d_x, n, ncols, d_out, st); });
 }
 
 int dspb200_hilbert_exec(int dtype, const void* x, int64_t n, int64_t ncols, void* out) {
     DSP_RANGE("dspb200_hilbert_exec");
-    DSP_REQUIRE(dtype == DSPB200_F32 || dtype == DSPB200_F64, "hilbert takes a real signal (dtype %d)", dtype);
-    DSP_REQUIRE(x && out && n >= 1 && ncols >= 1, "empty or NULL input");
+    DSP_TRY(hilbert_check(dtype, x, n, ncols, out));
     const size_t bytes = (size_t)(n * ncols) * dtype_size(dtype);
-    ConvenienceLock lock;                                       // scratch arena (common.cuh)
     DevBuf &dx = scratch_buf(0), &dout = scratch_buf(1);
-    const int rc = run_staged(0, {{x, bytes, &dx}}, {{out, 2 * bytes, &dout}},
-                              [&] { return dspb200_hilbert_exec_dev(dtype, dx.p, n, ncols, dout.p, nullptr); });
-    scratch_trim((size_t)256 << 20);
-    return rc;
+    return convenience_call({{x, bytes, &dx}}, {{out, 2 * bytes, &dout}},
+                            [&](cudaStream_t st) { return hilbert_queue(dtype, dx.p, n, ncols, dout.p, st); });
 }
 
-// _conv_td!, src/dspbase.jl:646-660 (host pointers, scratch arena)
+// _conv_td!, src/dspbase.jl:646-660: the rank-1 direct convolution of dspb200_conv_nd_exec (host pointers)
 int dspb200_conv_direct_exec(int dtype, const void* u, int64_t nu, const void* v, int64_t nv, void* out) {
     DSP_RANGE("dspb200_conv_direct_exec");
-    DSP_REQUIRE(dtype_valid(dtype), "invalid dtype %d", dtype);
-    DSP_REQUIRE(u && v && out && nu >= 1 && nv >= 1, "empty or NULL input");
-    const size_t esz = dtype_size(dtype);
-    const int64_t nout = nu + nv - 1;
-    ConvenienceLock lock;
-    DevBuf &du = scratch_buf(0), &dv = scratch_buf(1), &dout = scratch_buf(2);
-    auto launch = [&]() -> int {
-        const int threads = 128, g = grid_for(nout, threads);
-        switch (dtype) {
-            case DSPB200_F32: conv_direct_kernel<float, false><<<g, threads>>>(du.p, nu, dv.p, nv, dout.p); break;
-            case DSPB200_F64: conv_direct_kernel<double, false><<<g, threads>>>(du.p, nu, dv.p, nv, dout.p); break;
-            case DSPB200_C32: conv_direct_kernel<float, true><<<g, threads>>>(du.p, nu, dv.p, nv, dout.p); break;
-            default: conv_direct_kernel<double, true><<<g, threads>>>(du.p, nu, dv.p, nv, dout.p); break;
-        }
-        DSP_LAUNCH_OK();
-        return DSPB200_OK;
-    };
-    const int rc = run_staged(0, {{u, (size_t)nu * esz, &du}, {v, (size_t)nv * esz, &dv}}, {{out, (size_t)nout * esz, &dout}}, launch);
-    scratch_trim((size_t)256 << 20);
-    return rc;
+    DSP_TRY(conv_nd_check(dtype, ND_DIRECT, 1, &nu, u, &nv, v, nullptr, out));
+    return conv_nd_run_host(dtype, ND_DIRECT, 1, &nu, u, &nv, v, nullptr, out);
 }
 
 }  // extern "C"

@@ -1,8 +1,8 @@
 // dspb200 -- runtime entry points: errors, device selection, memory helpers.
 #include "common.cuh"
+#include "cufft_exec.cuh"
 #include "fft_core.cuh"
 #include <atomic>
-#include <cufft.h>
 #include <mutex>
 #include <vector>
 
@@ -32,6 +32,42 @@ int device_sm_count() {
 }
 
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
+
+int cufft_fail(cufftResult r, const char* what) {
+    set_error("cuFFT error %d in %s", (int)r, what);
+    return DSPB200_ECUFFT;
+}
+
+int fft_plan_1d(cufftHandle* h, bool cplx, bool f64, int dir, int64_t n, int64_t batch) {
+    long long nn[1] = {(long long)n};
+    size_t ws = 0;
+    *h = 0;
+    DSP_CUFFT(cufftCreate(h));
+    const cufftResult r = cufftMakePlanMany64(*h, 1, nn, nullptr, 1, 0, nullptr, 1, 0, fft_type(cplx, f64, dir), (long long)batch, &ws);
+    if (r != CUFFT_SUCCESS) {
+        cufftDestroy(*h);
+        *h = 0;
+        return cufft_fail(r, "cufftMakePlanMany64");
+    }
+    return DSPB200_OK;
+}
+
+int fft_exec(cufftHandle h, bool cplx, bool f64, int dir, const void* in, void* out, cudaStream_t st) {
+    void* src = const_cast<void*>(in);                              // cuFFT takes non-const input pointers
+    DSP_CUFFT(cufftSetStream(h, st));
+    if (cplx) {
+        if (f64) DSP_CUFFT(cufftExecZ2Z(h, (cufftDoubleComplex*)src, (cufftDoubleComplex*)out, dir));
+        else DSP_CUFFT(cufftExecC2C(h, (cufftComplex*)src, (cufftComplex*)out, dir));
+    } else if (dir == CUFFT_FORWARD) {
+        if (f64) DSP_CUFFT(cufftExecD2Z(h, (cufftDoubleReal*)src, (cufftDoubleComplex*)out));
+        else DSP_CUFFT(cufftExecR2C(h, (cufftReal*)src, (cufftComplex*)out));
+    } else {
+        if (f64) DSP_CUFFT(cufftExecZ2D(h, (cufftDoubleComplex*)src, (cufftDoubleReal*)out));
+        else DSP_CUFFT(cufftExecC2R(h, (cufftComplex*)src, (cufftReal*)out));
+    }
+    count_launch(1);
+    return DSPB200_OK;
+}
 
 int upload(void** d, const void* h, size_t bytes) {
     DSP_CUDA(cudaMalloc(d, bytes));

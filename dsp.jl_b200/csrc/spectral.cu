@@ -20,7 +20,7 @@
 // stft_store_kernel.
 #include "fft_core.cuh"
 #include "async_copy.cuh"
-#include <cufft.h>
+#include "cufft_exec.cuh"
 #include <math.h>
 #include <stdlib.h>
 #include <new>
@@ -1437,45 +1437,18 @@ static int welch_pin(SpecPlanImpl* p, int mode, int g, int64_t vctas) {
 }
 
 // ---------------------------------------------------------------------------------------------- generic path
-static int cufft_fail(cufftResult r, const char* what) {
-    set_error("cuFFT error %d in %s", (int)r, what);
-    return DSPB200_ECUFFT;
-}
-#define DSP_CUFFT(call)                                          \
-    do {                                                         \
-        cufftResult r__ = (call);                                \
-        if (r__ != CUFFT_SUCCESS) return cufft_fail(r__, #call); \
-    } while (0)
-
 static int generic_prepare(SpecPlanImpl* p) {
     if (p->fft_ok) return DSPB200_OK;
     int64_t b = (int64_t(1) << 22) / p->nfft;
     if (b < 1) b = 1;
     if (b > 8192) b = 8192;
     p->batch = b;
-    cufftType type = p->cplx ? (p->f64 ? CUFFT_Z2Z : CUFFT_C2C) : (p->f64 ? CUFFT_D2Z : CUFFT_R2C);
-    long long nn[1] = {(long long)p->nfft};
-    size_t ws = 0;
-    DSP_CUFFT(cufftCreate(&p->fft));
-    DSP_CUFFT(cufftMakePlanMany64(p->fft, 1, nn, nullptr, 1, 0, nullptr, 1, 0, type, (long long)b, &ws));
+    DSP_TRY(fft_plan_1d(&p->fft, p->cplx, p->f64, CUFFT_FORWARD, p->nfft, b));
     p->fft_ok = true;
     const size_t esz = dtype_size(p->dtype);
     DSP_TRY(p->segbuf.reserve((size_t)(b * p->nfft) * esz));
     DSP_TRY(p->specbuf.reserve((size_t)(b * p->nbins_fft) * (p->f64 ? 16 : 8)));
     DSP_TRY(p->acc.reserve((size_t)p->nbins_fft * sizeof(double)));
-    return DSPB200_OK;
-}
-
-static int generic_fft(SpecPlanImpl* p, cudaStream_t st) {
-    DSP_CUFFT(cufftSetStream(p->fft, st));
-    if (p->cplx) {
-        if (p->f64) DSP_CUFFT(cufftExecZ2Z(p->fft, (cufftDoubleComplex*)p->segbuf.p, (cufftDoubleComplex*)p->specbuf.p, CUFFT_FORWARD));
-        else DSP_CUFFT(cufftExecC2C(p->fft, (cufftComplex*)p->segbuf.p, (cufftComplex*)p->specbuf.p, CUFFT_FORWARD));
-    } else {
-        if (p->f64) DSP_CUFFT(cufftExecD2Z(p->fft, (cufftDoubleReal*)p->segbuf.p, (cufftDoubleComplex*)p->specbuf.p));
-        else DSP_CUFFT(cufftExecR2C(p->fft, (cufftReal*)p->segbuf.p, (cufftComplex*)p->specbuf.p));
-    }
-    count_launch(1);
     return DSPB200_OK;
 }
 
@@ -1489,7 +1462,7 @@ template <typename T> static int generic_segments(SpecPlanImpl* p, const void* s
     else
         seg_window_kernel<T, false><<<grid, threads, 0, st>>>(s, first_sample, p->hop, p->n, p->nfft, nseg, p->batch, reinterpret_cast<const typename win_t<T>::type*>(p->d_window), p->segbuf.p);
     DSP_LAUNCH_OK();
-    return generic_fft(p, st);
+    return fft_exec(p->fft, p->cplx, p->f64, CUFFT_FORWARD, p->segbuf.p, p->specbuf.p, st);
 }
 
 template <typename T> static int welch_generic_acc(SpecPlanImpl* p, const void* s, int64_t sample_offset,
@@ -1523,7 +1496,7 @@ template <typename T> static int stream_generic_fft(SpecPlanImpl* p, const void*
     else
         stft_seg_kernel<T, false><<<gseg, threads, 0, st>>>(hist, h, ldh, x, nx, f0, nf, k, p->hop, p->n, p->nfft, w, p->segbuf.p);
     DSP_LAUNCH_OK();
-    return generic_fft(p, st);
+    return fft_exec(p->fft, p->cplx, p->f64, CUFFT_FORWARD, p->segbuf.p, p->specbuf.p, st);
 }
 
 // STFT call, cuFFT sizes: the nchan x k (channel, segment) pairs fill the plan's batch in order, three launches per batch
@@ -1721,98 +1694,84 @@ struct dspb200_spec_plan {
 
 static size_t win_row_bytes(const SpecPlanImpl* p) { return (size_t)p->n * sizeof(double); }   // float2 pairs are 8 B too
 
-// mt_cross_power_spectra! / mt_coherence!, src/multitaper.jl:553-603, 722-790; queues the work on st (the caller waits for it:
-// the plan's scratch is reused by the next call)
-template <typename T>
-static int mt_cross_run(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int demean, int64_t f_lo, int64_t nf,
-                        int coherence, void* out, bool dev, cudaStream_t st) {
-    SpecPlanImpl* p = &plan->impl;
-    const int64_t n = p->n, cnt = nchan * nchan * nf;
-    const size_t cs_bytes = (size_t)cnt * sizeof(cx<T>), out_bytes = coherence ? (size_t)cnt * sizeof(T) : cs_bytes;
-    if (!dev) DSP_TRY(p->pipe.in[0].reserve((size_t)(n * nchan) * sizeof(T)));
-    DSP_TRY(p->pipe.in[1].reserve((size_t)(n * nchan) * sizeof(T)));
-    DSP_TRY(p->tmp.reserve((size_t)(p->nout * nchan) * sizeof(cx<T>)));
-    DSP_TRY(p->pipe.out[0].reserve(cs_bytes + (coherence ? out_bytes : 0)));
-    if (!dev) DSP_CUDA(cudaMemcpyAsync(p->pipe.in[0].p, signal, (size_t)(n * nchan) * sizeof(T), cudaMemcpyHostToDevice, st));
-    cs_prep_kernel<T><<<(unsigned)nchan, 256, 0, st>>>(dev ? (const T*)signal : (const T*)p->pipe.in[0].p, nchan, n, demean, (T*)p->pipe.in[1].p);
-    DSP_LAUNCH_OK();
-    const int threads = 256;
-    const int grid = (int)(cdiv(cnt, threads) < device_sm_count() * 32 ? cdiv(cnt, threads) : device_sm_count() * 32);
+// Runs f(t) for the tapers t = 0 .. ntapers - 1 of a multitaper plan, with the plan's window set to taper t's row, until one
+// fails; the window is restored on every exit.
+template <class F> static int for_each_taper(SpecPlanImpl* p, F&& f) {
     void* const base = p->d_window;
     int rc = DSPB200_OK;
     for (int64_t t = 0; t < p->ntapers && rc == DSPB200_OK; ++t) {
         p->d_window = (char*)base + (size_t)t * win_row_bytes(p);
-        rc = dspb200_stft_exec_dev(plan, p->pipe.in[1].p, n, nchan, 1.0, 0, p->tmp.p, st);     // raw spectra, nout x nchan
-        if (rc == DSPB200_OK) {
-            cs_acc_kernel<T><<<grid, threads, 0, st>>>((cx<T>*)p->pipe.out[0].p, (const cx<T>*)p->tmp.p, p->nout, nchan, f_lo, nf,
-                                                       (p->nfft % 2 == 0) ? 1 : 0, t == 0 ? 1 : 0);
-            count_launch(1);
-        }
+        rc = f(t);
     }
     p->d_window = base;
-    DSP_TRY(rc);
-    void* res = p->pipe.out[0].p;
+    return rc;
+}
+
+// mt_cross_power_spectra! / mt_coherence!, src/multitaper.jl:553-603, 722-790, device pointers; queues the work on st (the
+// caller waits for it: the plan's scratch is reused by the next call).  The spectra accumulate in `out`, or, for
+// coherence, in pipe.out[0], from which coherence_kernel writes `out`.
+template <typename T>
+static int mt_cross_run(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int demean, int64_t f_lo, int64_t nf,
+                        int coherence, void* out, cudaStream_t st) {
+    SpecPlanImpl* p = &plan->impl;
+    const int64_t n = p->n, cnt = nchan * nchan * nf;
+    DSP_TRY(p->pipe.in[1].reserve((size_t)(n * nchan) * sizeof(T)));
+    DSP_TRY(p->tmp.reserve((size_t)(p->nout * nchan) * sizeof(cx<T>)));
+    if (coherence) DSP_TRY(p->pipe.out[0].reserve((size_t)cnt * sizeof(cx<T>)));
+    cx<T>* const cs = (cx<T>*)(coherence ? p->pipe.out[0].p : out);
+    cs_prep_kernel<T><<<(unsigned)nchan, 256, 0, st>>>((const T*)signal, nchan, n, demean, (T*)p->pipe.in[1].p);
+    DSP_LAUNCH_OK();
+    const int threads = 256;
+    const int grid = (int)(cdiv(cnt, threads) < device_sm_count() * 32 ? cdiv(cnt, threads) : device_sm_count() * 32);
+    DSP_TRY(for_each_taper(p, [&](int64_t t) -> int {
+        DSP_TRY(dspb200_stft_exec_dev(plan, p->pipe.in[1].p, n, nchan, 1.0, 0, p->tmp.p, st));     // raw spectra, nout x nchan
+        cs_acc_kernel<T><<<grid, threads, 0, st>>>(cs, (const cx<T>*)p->tmp.p, p->nout, nchan, f_lo, nf, (p->nfft % 2 == 0) ? 1 : 0,
+                                                   t == 0 ? 1 : 0);
+        DSP_LAUNCH_OK();
+        return DSPB200_OK;
+    }));
     if (coherence) {
-        res = (char*)p->pipe.out[0].p + cs_bytes;
-        coherence_kernel<T><<<grid, threads, 0, st>>>((T*)res, (const cx<T>*)p->pipe.out[0].p, nchan, nf);
+        coherence_kernel<T><<<grid, threads, 0, st>>>((T*)out, cs, nchan, nf);
         DSP_LAUNCH_OK();
     }
-    DSP_CUDA(cudaMemcpyAsync(out, res, out_bytes, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
     return DSPB200_OK;
 }
 
+// periodogram(s::AbstractMatrix; nfft, fs, radialsum, radialavg), src/periodograms.jl:473-509, device pointers: queues the
+// work on st (cached plan + scratch arena: the caller goes through convenience_call)
 template <typename T>
 static int periodogram2_run(const void* s, int64_t n1, int64_t n2, int64_t f1, int64_t f2, double r, int ptype, void* out,
-                            bool dev = false, cudaStream_t st = 0) {
+                            cudaStream_t st) {
     const int64_t h = f1 / 2 + 1, nmin = f1 < f2 ? f1 : f2, kmax = nmin / 2 + 1;
-    const int64_t nout = ptype == 0 ? f1 * f2 : kmax;
     const int threads = 256;
     auto grid = [&](int64_t total) { const int64_t g = cdiv(total, threads); const int64_t cap = (int64_t)device_sm_count() * 32; return (int)(g < cap ? g : cap); };
-    ConvenienceLock lock;                                       // cached plan + scratch arena (common.cuh)
-    DevBuf &ds = scratch_buf(0), &dpad = scratch_buf(1), &dX = scratch_buf(2), &dout = scratch_buf(3), &dacc = scratch_buf(4);
-    cufftHandle plan = 0;
-    auto body = [&]() -> int {
-        if (!dev) DSP_TRY(ds.reserve((size_t)(n1 * n2) * sizeof(T)));
-        DSP_TRY(dpad.reserve((size_t)(f1 * f2) * sizeof(T)));
-        DSP_TRY(dX.reserve((size_t)(h * f2) * sizeof(cx<T>)));
-        if (!dev) {
-            DSP_TRY(dout.reserve((size_t)nout * sizeof(T)));
-            DSP_CUDA(cudaMemcpyAsync(ds.p, s, (size_t)(n1 * n2) * sizeof(T), cudaMemcpyHostToDevice, st));
-        }
-        const T* src = dev ? (const T*)s : (const T*)ds.p;
-        T* dst = dev ? (T*)out : (T*)dout.p;
-        per2_pad_kernel<T><<<grid(f1 * f2), threads, 0, st>>>(src, n1, n2, (T*)dpad.p, f1, f2);
+    DevBuf &dpad = scratch_buf(1), &dX = scratch_buf(2), &dacc = scratch_buf(4);
+    DSP_TRY(dpad.reserve((size_t)(f1 * f2) * sizeof(T)));
+    DSP_TRY(dX.reserve((size_t)(h * f2) * sizeof(cx<T>)));
+    per2_pad_kernel<T><<<grid(f1 * f2), threads, 0, st>>>((const T*)s, n1, n2, (T*)dpad.p, f1, f2);
+    DSP_LAUNCH_OK();
+    const bool f64 = sizeof(T) == 8;
+    long long nn[2] = {(long long)f2, (long long)f1};            // cuFFT is row-major: slowest dimension first
+    int hp = 0;
+    DSP_TRY(plan_cache_get(&hp, 2, nn, false, 0, 0, fft_type(false, f64, CUFFT_FORWARD), 1));
+    DSP_TRY(fft_exec((cufftHandle)hp, false, f64, CUFFT_FORWARD, dpad.p, dX.p, st));
+    if (ptype == 0) {
+        per2_full_kernel<T><<<grid(f1 * f2), threads, 0, st>>>((const cx<T>*)dX.p, f1, f2, (T)(1.0 / r), (T*)out);
         DSP_LAUNCH_OK();
-        long long nn[2] = {(long long)f2, (long long)f1};            // cuFFT is row-major: slowest dimension first
-        int hp = 0;
-        DSP_TRY(plan_cache_get(&hp, 2, nn, false, 0, 0, sizeof(T) == 8 ? CUFFT_D2Z : CUFFT_R2C, 1));
-        plan = (cufftHandle)hp;
-        DSP_CUFFT(cufftSetStream(plan, st));
-        if (sizeof(T) == 8) DSP_CUFFT(cufftExecD2Z(plan, (cufftDoubleReal*)dpad.p, (cufftDoubleComplex*)dX.p));
-        else DSP_CUFFT(cufftExecR2C(plan, (cufftReal*)dpad.p, (cufftComplex*)dX.p));
-        count_launch(1);
-        if (ptype == 0) {
-            per2_full_kernel<T><<<grid(f1 * f2), threads, 0, st>>>((const cx<T>*)dX.p, f1, f2, (T)(1.0 / r), dst);
-            DSP_LAUNCH_OK();
-        } else {
-            DSP_TRY(dacc.reserve((size_t)kmax * 16));
-            DSP_CUDA(cudaMemsetAsync(dacc.p, 0, (size_t)kmax * 16, st));
-            double* acc = (double*)dacc.p;
-            unsigned long long* wc = (unsigned long long*)(acc + kmax);
-            double c1 = 1.0, c2 = 1.0;                               // wavevector scaling for non-square transforms, :193-199
-            if (f1 == nmin) c2 = (double)f1 / (double)f2; else c1 = (double)f2 / (double)f1;
-            const T m1 = (T)(1.0 / r), m2 = (T)(2.0 / r);            // rounded to the signal precision as in the reference
-            per2_radial_kernel<T><<<grid(h * f2), threads, 0, st>>>((const cx<T>*)dX.p, f1, f2, c1, c2, (double)m1, (double)m2, kmax, acc, wc);
-            DSP_LAUNCH_OK();
-            per2_radial_finish_kernel<T><<<(unsigned)cdiv(kmax, threads), threads, 0, st>>>(acc, wc, kmax, ptype == 2, dst);
-            DSP_LAUNCH_OK();
-        }
-        if (!dev) DSP_CUDA(cudaMemcpyAsync(out, dout.p, (size_t)nout * sizeof(T), cudaMemcpyDeviceToHost, st));
         return DSPB200_OK;
-    };
-    const int rc = settle(st, body());                          // the cached plan and the arena are reused by the next call
-    scratch_trim((size_t)256 << 20);
-    return rc;
+    }
+    DSP_TRY(dacc.reserve((size_t)kmax * 16));
+    DSP_CUDA(cudaMemsetAsync(dacc.p, 0, (size_t)kmax * 16, st));
+    double* acc = (double*)dacc.p;
+    unsigned long long* wc = (unsigned long long*)(acc + kmax);
+    double c1 = 1.0, c2 = 1.0;                                   // wavevector scaling for non-square transforms, :193-199
+    if (f1 == nmin) c2 = (double)f1 / (double)f2; else c1 = (double)f2 / (double)f1;
+    const T m1 = (T)(1.0 / r), m2 = (T)(2.0 / r);                // rounded to the signal precision as in the reference
+    per2_radial_kernel<T><<<grid(h * f2), threads, 0, st>>>((const cx<T>*)dX.p, f1, f2, c1, c2, (double)m1, (double)m2, kmax, acc, wc);
+    DSP_LAUNCH_OK();
+    per2_radial_finish_kernel<T><<<(unsigned)cdiv(kmax, threads), threads, 0, st>>>(acc, wc, kmax, ptype == 2, (T*)out);
+    DSP_LAUNCH_OK();
+    return DSPB200_OK;
 }
 
 extern "C" {
@@ -2411,18 +2370,12 @@ int dspb200_mt_pgram_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t 
     SpecPlanImpl* p = &plan->impl;
     DSP_CUDA(cudaSetDevice(p->device));
     cudaStream_t st = (cudaStream_t)stream;
-    DSP_TRY(welch_begin(p, st));
-    void* const base = p->d_window;
-    int rc = DSPB200_OK;
-    for (int64_t t = 0; t < p->ntapers && rc == DSPB200_OK; ++t) {
-        p->d_window = (char*)base + (size_t)t * win_row_bytes(p);
-        rc = welch_accumulate(p, d_s, 0, 0, 1, st);
-    }
-    p->d_window = base;
-    DSP_TRY(rc);
-    DSP_TRY(welch_finalize(p, 1.0, d_out, st));
-    DSP_CUDA(cudaStreamSynchronize(st));
-    return DSPB200_OK;
+    auto queue = [&]() -> int {
+        DSP_TRY(welch_begin(p, st));
+        DSP_TRY(for_each_taper(p, [&](int64_t) { return welch_accumulate(p, d_s, 0, 0, 1, st); }));
+        return welch_finalize(p, 1.0, d_out, st);
+    };
+    return settle(st, queue());
 }
 int dspb200_mt_pgram_exec(dspb200_spec_plan* plan, const void* s, int64_t len, void* out) {
     DSP_RANGE("dspb200_mt_pgram_exec");
@@ -2445,28 +2398,21 @@ int dspb200_mt_spectrogram_exec_dev(dspb200_spec_plan* plan, const void* d_s, in
     cudaStream_t st = (cudaStream_t)stream;
     const size_t oel = p->f64 ? 8 : 4;
     const int64_t cnt = p->nout * k;
-    if (!p->fused) DSP_TRY(p->tmp.reserve((size_t)cnt * oel));
-    void* const base = p->d_window;
-    int rc = DSPB200_OK;
-    for (int64_t t = 0; t < p->ntapers && rc == DSPB200_OK; ++t) {
-        p->d_window = (char*)base + (size_t)t * win_row_bytes(p);
-        if (p->fused) {                                  // tapers after the first add their PSD columns inside the emit step
-            rc = dspb200_stft_exec_dev(plan, d_s, len, 1, 1.0, t == 0 ? 1 : 3, d_out, st);
-            continue;
-        }
-        rc = dspb200_stft_exec_dev(plan, d_s, len, 1, 1.0, 1, t == 0 ? d_out : p->tmp.p, st);
-        if (rc == DSPB200_OK && t > 0) {
+    auto taper = [&](int64_t t) -> int {
+        if (p->fused)                                    // tapers after the first add their PSD columns inside the emit step
+            return dspb200_stft_exec_dev(plan, d_s, len, 1, 1.0, t == 0 ? 1 : 3, d_out, st);
+        DSP_TRY(dspb200_stft_exec_dev(plan, d_s, len, 1, 1.0, 1, t == 0 ? d_out : p->tmp.p, st));
+        if (t > 0) {
             const int threads = 256;
             const int grid = (int)(cdiv(cnt, threads) < device_sm_count() * 32 ? cdiv(cnt, threads) : device_sm_count() * 32);
             if (p->f64) acc_add_kernel<double><<<grid, threads, 0, st>>>((double*)d_out, (const double*)p->tmp.p, cnt);
             else acc_add_kernel<float><<<grid, threads, 0, st>>>((float*)d_out, (const float*)p->tmp.p, cnt);
-            count_launch(1);
+            DSP_LAUNCH_OK();
         }
-    }
-    p->d_window = base;
-    DSP_TRY(rc);
-    DSP_CUDA(cudaStreamSynchronize(st));
-    return DSPB200_OK;
+        return DSPB200_OK;
+    };
+    if (!p->fused) DSP_TRY(p->tmp.reserve((size_t)cnt * oel));
+    return settle(st, for_each_taper(p, taper));
 }
 int dspb200_mt_spectrogram_exec(dspb200_spec_plan* plan, const void* s, int64_t len, void* out) {
     DSP_RANGE("dspb200_mt_spectrogram_exec");
@@ -2481,8 +2427,7 @@ int dspb200_mt_spectrogram_exec(dspb200_spec_plan* plan, const void* s, int64_t 
                       [&] { return dspb200_mt_spectrogram_exec_dev(plan, p->pipe.in[0].p, len, p->pipe.out[0].p, p->pipe.s_exec); });
 }
 
-static int mt_cross_entry(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int demean, int64_t f_lo, int64_t nf,
-                          int coherence, void* out, bool dev, cudaStream_t st) {
+static int mt_cross_check(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int64_t f_lo, int64_t nf, void* out) {
     DSP_REQUIRE(plan != nullptr, "plan is NULL");
     SpecPlanImpl* p = &plan->impl;
     DSP_REQUIRE(p->ntapers >= 1, "not a multitaper plan");
@@ -2490,45 +2435,69 @@ static int mt_cross_entry(dspb200_spec_plan* plan, const void* signal, int64_t n
                 "Only real data is supported (with the default choice of `onesided=true`) for this operation.");   // :411-416
     DSP_REQUIRE(nchan >= 1, "n_channels must be positive");
     DSP_REQUIRE(f_lo >= 0 && nf >= 0 && f_lo + nf <= p->nout, "frequency range outside the spectrum");
-    if (nf == 0) return DSPB200_OK;
-    DSP_REQUIRE(signal && out, "NULL argument");
-    DSP_TRY(ensure_streams(p));
-    if (!dev) st = p->pipe.s_exec;
-    return settle(st, p->f64 ? mt_cross_run<double>(plan, signal, nchan, demean, f_lo, nf, coherence, out, dev, st)
-                             : mt_cross_run<float>(plan, signal, nchan, demean, f_lo, nf, coherence, out, dev, st));
-}
-int dspb200_mt_cross_spectra_exec(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int demean, int64_t f_lo,
-                                  int64_t nf, int coherence, void* out) {
-    DSP_RANGE("dspb200_mt_cross_spectra_exec");
-    return mt_cross_entry(plan, signal, nchan, demean, f_lo, nf, coherence, out, false, 0);
+    DSP_REQUIRE(nf == 0 || (signal && out), "NULL argument");
+    return DSPB200_OK;
 }
 int dspb200_mt_cross_spectra_exec_dev(dspb200_spec_plan* plan, const void* d_signal, int64_t nchan, int demean, int64_t f_lo,
                                       int64_t nf, int coherence, void* d_out, void* stream) {
     DSP_RANGE("dspb200_mt_cross_spectra_exec_dev");
-    return mt_cross_entry(plan, d_signal, nchan, demean, f_lo, nf, coherence, d_out, true, (cudaStream_t)stream);
+    DSP_TRY(mt_cross_check(plan, d_signal, nchan, f_lo, nf, d_out));
+    if (nf == 0) return DSPB200_OK;
+    SpecPlanImpl* p = &plan->impl;
+    DSP_TRY(ensure_streams(p));
+    cudaStream_t st = (cudaStream_t)stream;
+    return settle(st, p->f64 ? mt_cross_run<double>(plan, d_signal, nchan, demean, f_lo, nf, coherence, d_out, st)
+                             : mt_cross_run<float>(plan, d_signal, nchan, demean, f_lo, nf, coherence, d_out, st));
+}
+// Host pointers: the signal is staged in pipe.in[0] and the result in pipe.out[1], which the device form does not use.
+int dspb200_mt_cross_spectra_exec(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int demean, int64_t f_lo,
+                                  int64_t nf, int coherence, void* out) {
+    DSP_RANGE("dspb200_mt_cross_spectra_exec");
+    DSP_TRY(mt_cross_check(plan, signal, nchan, f_lo, nf, out));
+    if (nf == 0) return DSPB200_OK;
+    SpecPlanImpl* p = &plan->impl;
+    DSP_TRY(ensure_streams(p));
+    HostPipe& hp = p->pipe;
+    const size_t esz = p->f64 ? 8 : 4, out_bytes = (size_t)(nchan * nchan * nf) * esz * (coherence ? 1 : 2);
+    return run_staged(hp.s_exec, {{signal, (size_t)(p->n * nchan) * esz, &hp.in[0]}}, {{out, out_bytes, &hp.out[1]}}, [&] {
+        return dspb200_mt_cross_spectra_exec_dev(plan, hp.in[0].p, nchan, demean, f_lo, nf, coherence, hp.out[1].p, hp.s_exec);
+    });
 }
 
 // periodogram(s::AbstractMatrix; nfft, fs, radialsum, radialavg), src/periodograms.jl:473-509 (cached plan + scratch arena)
-static int periodogram2_entry(int dtype, const void* s, int64_t n1, int64_t n2, int64_t nfft1, int64_t nfft2, double r, int ptype,
-                              void* out, bool dev, cudaStream_t st) {
+static int periodogram2_check(int dtype, const void* s, int64_t n1, int64_t n2, int64_t nfft1, int64_t nfft2, double r, int ptype,
+                              void* out) {
     DSP_REQUIRE(dtype == DSPB200_F32 || dtype == DSPB200_F64, "periodogram of a matrix takes a real signal (dtype %d)", dtype);
     DSP_REQUIRE(s && out, "NULL argument");
     DSP_REQUIRE(n1 > 1 && n2 > 1, "dimensions of s must be > 1");                                   // :478
     DSP_REQUIRE(n1 <= nfft1 && n2 <= nfft2, "nfft must be >= size(s)");                             // :477
     DSP_REQUIRE(nfft1 < (int64_t(1) << 31) && nfft2 < (int64_t(1) << 31), "nfft too large");
     DSP_REQUIRE(ptype >= 0 && ptype <= 2 && r != 0.0, "bad ptype or r");
-    return dtype == DSPB200_F64 ? periodogram2_run<double>(s, n1, n2, nfft1, nfft2, r, ptype, out, dev, st)
-                                : periodogram2_run<float>(s, n1, n2, nfft1, nfft2, r, ptype, out, dev, st);
+    return DSPB200_OK;
+}
+static int periodogram2_queue(int dtype, const void* d_s, int64_t n1, int64_t n2, int64_t nfft1, int64_t nfft2, double r, int ptype,
+                              void* d_out, cudaStream_t st) {
+    return dtype == DSPB200_F64 ? periodogram2_run<double>(d_s, n1, n2, nfft1, nfft2, r, ptype, d_out, st)
+                                : periodogram2_run<float>(d_s, n1, n2, nfft1, nfft2, r, ptype, d_out, st);
 }
 int dspb200_periodogram2_exec(int dtype, const void* s, int64_t n1, int64_t n2, int64_t nfft1, int64_t nfft2, double r, int ptype,
                               void* out) {
     DSP_RANGE("dspb200_periodogram2_exec");
-    return periodogram2_entry(dtype, s, n1, n2, nfft1, nfft2, r, ptype, out, false, 0);
+    DSP_TRY(periodogram2_check(dtype, s, n1, n2, nfft1, nfft2, r, ptype, out));
+    const size_t esz = dtype_size(dtype);
+    const int64_t nmin = nfft1 < nfft2 ? nfft1 : nfft2, nout = ptype == 0 ? nfft1 * nfft2 : nmin / 2 + 1;
+    DevBuf &ds = scratch_buf(0), &dout = scratch_buf(3);
+    return convenience_call({{s, (size_t)(n1 * n2) * esz, &ds}}, {{out, (size_t)nout * esz, &dout}}, [&](cudaStream_t st) {
+        return periodogram2_queue(dtype, ds.p, n1, n2, nfft1, nfft2, r, ptype, dout.p, st);
+    });
 }
 int dspb200_periodogram2_exec_dev(int dtype, const void* d_s, int64_t n1, int64_t n2, int64_t nfft1, int64_t nfft2, double r,
                                   int ptype, void* d_out, void* stream) {
     DSP_RANGE("dspb200_periodogram2_exec_dev");
-    return periodogram2_entry(dtype, d_s, n1, n2, nfft1, nfft2, r, ptype, d_out, true, (cudaStream_t)stream);
+    DSP_TRY(periodogram2_check(dtype, d_s, n1, n2, nfft1, nfft2, r, ptype, d_out));
+    return convenience_call((cudaStream_t)stream, [&](cudaStream_t st) {
+        return periodogram2_queue(dtype, d_s, n1, n2, nfft1, nfft2, r, ptype, d_out, st);
+    });
 }
 
 int dspb200_spec_plan_destroy(dspb200_spec_plan* plan) {

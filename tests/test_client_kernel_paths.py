@@ -1,8 +1,8 @@
 """The GPU clients of the core kernels (DESIGN.md §1, "§8f") element by element against a high-precision reference.
 
 Entry points and the kernels they run:
-- `dspb200_conv_fft_exec` (1-D :fft_simple): `pad_copy_kernel`, `scale_cplx_kernel`, `os_cmul_kernel` + cuFFT;
-- `dspb200_conv_nd_exec(_dev)` with nffts (N-D :fft_simple): `nd_copy_kernel`, `scale_cplx_kernel`, `os_cmul_kernel` + cuFFT;
+- `dspb200_conv_nd_exec(_dev)` with nffts (N-D :fft_simple), and `dspb200_conv_fft_exec` (1-D :fft_simple, its rank-1 case):
+  `nd_copy_kernel`, `scale_cplx_kernel`, `os_cmul_kernel` + cuFFT;
 - `dspb200_conv_nd_os_exec(_dev)` (N-D overlap-save): `nd_os_gather_kernel`, `nd_os_scatter_kernel` + batched cuFFT;
 - `dspb200_hilbert_exec(_dev)`: `hilbert_weight_kernel` between a strided R2C and a batched C2C transform;
 - `dspb200_periodogram2_exec(_dev)`: `per2_pad_kernel`, `per2_full_kernel`, `per2_radial_kernel`, `per2_radial_finish_kernel`;

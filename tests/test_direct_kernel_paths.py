@@ -9,10 +9,10 @@ rounded fused multiply-add per step (Base.muladd for Complex: two fmas per part,
   eltypes that is the reference's _filt_fir! (src/dspbase.jl:95-141).  For complex ones the reference forms the last tap's
   term b[nb] * x as a plain complex product where the kernel fuses it (DESIGN section 4): the kernel is checked against
   its own documented chain, and the difference is pinned on the CPU.
-* `conv_direct_kernel` and `conv_direct_nd_kernel` (overlap_save.cu): _conv_td! (src/dspbase.jl:646-660).  Its loop
-  `for m in CartesianIndices(u), n in CartesianIndices(v)` (n outer instead when size(u,1) > size(v,1)) has the FIRST
-  iterator outside, so each output sums its products in the column-major order of the outer array's index, each step
-  muladd(u[m], v[n], acc).
+* `conv_direct_nd_kernel` (overlap_save.cu), ranks 1-3, 1-D also through `dspb200_conv_direct_exec`: _conv_td!
+  (src/dspbase.jl:646-660).  Its loop `for m in CartesianIndices(u), n in CartesianIndices(v)` (n outer instead when
+  size(u,1) > size(v,1)) has the FIRST iterator outside, so each output sums its products in the column-major order of the
+  outer array's index, each step muladd(u[m], v[n], acc).
 
 The restated chains below are vectorised over outputs, one numpy step per tap (or per outer index), with exact fmas
 (oracle.dspbase.fma_f32 / fma_f64 / cmuladd), which are themselves pinned against fractions.Fraction; on small shapes
@@ -707,7 +707,8 @@ def test_fir_front_ends_bit_exact(dsp, fir_cases_on_device, dt):
 @pytest.mark.gpu
 @pytest.mark.parametrize("dt", DTYPES, ids=lambda d: d.name)
 def test_conv_direct_1d_bit_exact(dsp, dt):
-    """dspb200_conv_direct_exec, conv and conv_ (algorithm 'direct' and 'auto' below 2^16) against the reference's order."""
+    """dspb200_conv_direct_exec, conv and conv_ (algorithm 'direct' and 'auto' below 2^16) against the reference's order;
+    dspb200_conv_direct_exec bit-identical to the rank-1 dspb200_conv_nd_exec with nffts = NULL."""
     rng = np.random.default_rng(900 + DTYPES.index(dt))
     for nu, nv in CONV1_SHAPES:
         u, v = _data(rng, nu, dt), _data(rng, nv, dt)
@@ -715,6 +716,9 @@ def test_conv_direct_1d_bit_exact(dsp, dt):
         got = np.empty(nu + nv - 1, dtype=dt)
         dsp._lib.conv_direct(u, v, got)
         assert np.array_equal(got, want), (nu, nv)
+        nd = np.empty(nu + nv - 1, dtype=dt)
+        dsp._lib.conv_nd(u, v, None, nd)
+        assert got.tobytes() == nd.tobytes(), (nu, nv)
         for alg in ("direct", "auto"):
             assert np.array_equal(dsp.conv(u, v, algorithm=alg), want), (nu, nv, alg)
             out = np.full(nu + nv + 2, np.nan, dtype=dt)
