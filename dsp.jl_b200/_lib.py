@@ -104,6 +104,10 @@ SIGNATURES = {
     "dspb200_mt_spectrogram_exec": (_int, [_vp, _vp, _i64, _vp]),
     "dspb200_mt_pgram_exec_dev": (_int, [_vp, _vp, _i64, _vp, _vp]),
     "dspb200_mt_spectrogram_exec_dev": (_int, [_vp, _vp, _i64, _vp, _vp]),
+    "dspb200_mt_pgram_batch_exec": (_int, [_vp, _vp, _i64, _i64, _vp]),
+    "dspb200_mt_spectrogram_batch_exec": (_int, [_vp, _vp, _i64, _i64, _vp]),
+    "dspb200_mt_pgram_batch_exec_dev": (_int, [_vp, _vp, _i64, _i64, _vp, _vp]),
+    "dspb200_mt_spectrogram_batch_exec_dev": (_int, [_vp, _vp, _i64, _i64, _vp, _vp]),
     "dspb200_mt_cross_spectra_exec": (_int, [_vp, _vp, _i64, _int, _i64, _i64, _int, _vp]),
     "dspb200_mt_cross_spectra_exec_dev": (_int, [_vp, _vp, _i64, _int, _i64, _i64, _int, _vp, _vp]),
     "dspb200_spec_plan_destroy": (_int, [_vp]),
@@ -289,9 +293,10 @@ class SpecPlan(_Plan):
         check(lib.dspb200_spec_plan_pin_welch(self.handle, 1 if batched else 0, int(mode), int(groups), int(vctas)))
 
     def welch_config(self, batched, aligned):
-        """(mode, groups, virtual CTAs) of the last fused Welch launch of that form and alignment class; groups = 0: none."""
+        """(mode, groups, virtual CTAs) of the last fused Welch launch of that form (batched = 2: mt_pgram of a multitaper plan)
+        and alignment class; groups = 0: none."""
         m, g, v = _int(0), _int(0), _i64(0)
-        check(lib.dspb200_spec_plan_welch_config(self.handle, 1 if batched else 0, 1 if aligned else 0, C.byref(m), C.byref(g),
+        check(lib.dspb200_spec_plan_welch_config(self.handle, int(batched), 1 if aligned else 0, C.byref(m), C.byref(g),
                                                  C.byref(v)))
         return m.value, g.value, v.value
 
@@ -365,6 +370,20 @@ class MtPlan(SpecPlan):
 
     def mt_spectrogram_dev(self, s_ptr, length, out_ptr, stream=0):
         check(lib.dspb200_mt_spectrogram_exec_dev(self.handle, s_ptr, int(length), out_ptr, stream))
+
+    def mt_pgram_batch(self, s, length, nchan, out):
+        """mt_pgram of every column of the column-major (length, nchan) matrix s; out is (nout, nchan)."""
+        check(lib.dspb200_mt_pgram_batch_exec(self.handle, ptr(s), int(length), int(nchan), ptr(out)))
+
+    def mt_spectrogram_batch(self, s, length, nchan, out):
+        """mt_spectrogram of every column of the column-major (length, nchan) matrix s; out is (nout, k, nchan)."""
+        check(lib.dspb200_mt_spectrogram_batch_exec(self.handle, ptr(s), int(length), int(nchan), ptr(out)))
+
+    def mt_pgram_batch_dev(self, s_ptr, length, nchan, out_ptr, stream=0):
+        check(lib.dspb200_mt_pgram_batch_exec_dev(self.handle, s_ptr, int(length), int(nchan), out_ptr, stream))
+
+    def mt_spectrogram_batch_dev(self, s_ptr, length, nchan, out_ptr, stream=0):
+        check(lib.dspb200_mt_spectrogram_batch_exec_dev(self.handle, s_ptr, int(length), int(nchan), out_ptr, stream))
 
     def cross_spectra_dev(self, signal_ptr, nchan, demean, f_lo, nf, coherence, out_ptr, stream=0):
         check(lib.dspb200_mt_cross_spectra_exec_dev(self.handle, signal_ptr, int(nchan), 1 if demean else 0, int(f_lo), int(nf),

@@ -44,7 +44,7 @@ struct SpecPlanImpl {
     void* d_t256 = nullptr;
     size_t smem_optin = 0;        // cudaDevAttrMaxSharedMemoryPerBlockOptin
     int64_t ntapers = 0;          // multitaper plans: d_window holds ntapers rows of n values
-    DevBuf tmp;                   // multitaper spectrogram: one taper's PSD matrix
+    DevBuf tmp;                   // multitaper spectrogram, cuFFT sizes: one taper's PSD matrices
     // launch configuration of the fused Welch kernel, chosen once per (plan, alignment class): the selection walks up to nine
     // kernel instances through cudaFuncSetAttribute + the occupancy calculator (tens of microseconds per launch otherwise)
     // (mode: MODE of the instance; vctas: virtual CTAs pinned by dspb200_spec_plan_pin_welch, 0 = one resident wave;
@@ -57,6 +57,7 @@ struct SpecPlanImpl {
     // batched Welch (dspb200_welch_batch_exec_dev): its own kernel configuration cache and scratch, so that a streaming
     // accumulation open on the plan (partial / rows_used, acc) is left as it was
     WelchCfg welch_batch_cfg[2];
+    WelchCfg welch_mt_cfg[2];     // the batched kernel's taper-row instances (mt_pgram), which share `bpartial`
     DevBuf bpartial;              // fused: one row of nfft real T per (channel, slice), at most WELCH_BATCH_SCRATCH bytes
     DevBuf bacc;                  // generic: double[nbins_fft], one channel at a time
     // generic path
@@ -129,7 +130,7 @@ template <typename T, int N, int G> struct welch_bounds {
 };
 
 // The two work assignments of welch_fused_kernel; virtual CTA v of nv takes the v-th of nv equal contiguous shares of the
-// work.  One signal (BATCH = false: welch_exec*, range, streaming, multitaper, filt_welch): the work is the units of segments
+// work.  One signal (BATCH = false: welch_exec*, range, streaming, filt_welch): the work is the units of segments
 // seg0 .. seg0 + nseg - 1 (`sample_offset`: the signal index of the buffer's first sample), and v writes partial row v
 // once, at the end.  Many channels (BATCH = true: welch_batch_exec*): the columns of a len x nchan matrix, `chan_stride`
 // samples apart, nseg segments (upc units) each.  The work is nitems (channel, slice) items: slice j of a channel owns its
@@ -138,10 +139,14 @@ template <typename T, int N, int G> struct welch_bounds {
 // the TMA prefetch of the next unit runs across item and channel boundaries.  No atomics: the result is deterministic.
 // Each work assignment's parameters are Nil in the other's instances, and each keeps the parameter order it had as a kernel
 // of its own: ptxas assigns the parameters' uniform registers by offset, and a struct of them compiles to different code.
+// TAPERS (batch only: multitaper periodograms, mt_pgram): unit u of a channel is taper u -- all of a channel's units read the
+// same n samples at the channel's start, unit u under window row u (rows n values apart), and nseg = 1 (no unit has a second
+// real segment).  The staged samples serve every taper of the channel; the next channel's are fetched after the last taper's
+// first pass.  Only MODE 0 / 1 address a window row per unit.
 struct Nil {};
 template <bool USED, typename X> using welch_arg = typename std::conditional<USED, X, Nil>::type;
 
-template <typename T, int N, bool CPLX, int MODE, int G, bool BATCH>
+template <typename T, int N, bool CPLX, int MODE, int G, bool BATCH, bool TAPERS = false>
 __global__ void __launch_bounds__((welch_bounds<T, N, G>::NTG * G), (welch_bounds<T, N, G>::minblocks))
 welch_fused_kernel(const void* __restrict__ s_, welch_arg<BATCH, int64_t> chan_stride, welch_arg<!BATCH, int64_t> seg0,
                    int64_t nseg, welch_arg<BATCH, int64_t> upc, welch_arg<BATCH, int64_t> per, welch_arg<BATCH, int> slices,
@@ -162,6 +167,7 @@ welch_fused_kernel(const void* __restrict__ s_, welch_arg<BATCH, int64_t> chan_s
     constexpr bool TMA = MODE >= 1;
     constexpr bool WSM = MODE == 2;
     constexpr bool WREG = MODE == 3;
+    static_assert(!TAPERS || (BATCH && MODE <= 1), "taper rows: the batched work assignment, window read per unit");
     using W = typename win_t<T>::type;
     cx<T>* tabs = reinterpret_cast<cx<T>*>(smem_raw);
     W* wsm = reinterpret_cast<W*>(smem_raw + L::table_bytes());
@@ -205,7 +211,8 @@ welch_fused_kernel(const void* __restrict__ s_, welch_arg<BATCH, int64_t> chan_s
 
     // unit u (of channel c in a batch)
     auto unit_src = [&](int64_t c, int64_t u) -> const In* {
-        if constexpr (BATCH) return s + c * chan_stride + (CPLX ? u : 2 * u) * hop;
+        if constexpr (TAPERS) return s + c * chan_stride;
+        else if constexpr (BATCH) return s + c * chan_stride + (CPLX ? u : 2 * u) * hop;
         else return s + ((seg0 + (CPLX ? u : 2 * u)) * hop - sample_offset);
     };
     auto unit_bytes = [&](int64_t u) -> uint32_t {
@@ -246,20 +253,23 @@ welch_fused_kernel(const void* __restrict__ s_, welch_arg<BATCH, int64_t> chan_s
             const bool hasB = !CPLX && (2 * u + 1 < nseg);
             const In* pa = TMA ? stage : unit_src(c, u);
             const In* pb = pa + hop;
+            const W* wu = TAPERS ? win + u * n : win;
             if constexpr (TMA) {
-                mbar_wait(bar, parity);
-                parity ^= 1;
+                if (!TAPERS || u == ua) {                    // taper rows: one staged copy per channel
+                    mbar_wait(bar, parity);
+                    parity ^= 1;
+                }
             }
             auto ld0 = [&](int j, int it, int r) -> cx<T> {
                 if (j >= n) return mkc<T>(T(0), T(0));
                 if constexpr (CPLX) {
                     cx<T> v = pa[j];
-                    if (WREG || WSM || win) { const W w = WREG ? wreg[WREG ? it : 0][WREG ? r : 0] : (WSM ? wsm[j] : win[j]); v = mkc<T>(win_mul(v.x, w), win_mul(v.y, w)); }
+                    if (WREG || WSM || wu) { const W w = WREG ? wreg[WREG ? it : 0][WREG ? r : 0] : (WSM ? wsm[j] : wu[j]); v = mkc<T>(win_mul(v.x, w), win_mul(v.y, w)); }
                     return v;
                 } else {
                     T a = pa[j];
                     T b = hasB ? pb[j] : T(0);
-                    if (WREG || WSM || win) { const W w = WREG ? wreg[WREG ? it : 0][WREG ? r : 0] : (WSM ? wsm[j] : win[j]); a = win_mul(a, w); b = win_mul(b, w); }
+                    if (WREG || WSM || wu) { const W w = WREG ? wreg[WREG ? it : 0][WREG ? r : 0] : (WSM ? wsm[j] : wu[j]); a = win_mul(a, w); b = win_mul(b, w); }
                     return mkc<T>(a, b);
                 }
             };
@@ -282,6 +292,7 @@ welch_fused_kernel(const void* __restrict__ s_, welch_arg<BATCH, int64_t> chan_s
                 if (tid == 0) {
                     int64_t nc = c, nu = u + 1, nub = ub;
                     if (nu == ub && item + 1 < w1) item_range(item + 1, nc, nu, nub);
+                    else if (TAPERS) nu = nub;                  // the next taper reads the samples already staged
                     if (nu < nub) {
                         fence_proxy_async_shared();
                         mbar_expect_tx(bar, unit_bytes(nu));
@@ -380,7 +391,7 @@ template <typename T, int N, bool CPLX, int MODE, int HASB, int ONES, bool ACC =
 __device__ __forceinline__ void stft_emit(const cx<T>* __restrict__ sm, void* __restrict__ out_, int64_t colA, int nout,
                                           bool hasB_rt, int onesided_rt, T m1, T m2, int tid) {
     constexpr int NT = fft_threads<N>::value;
-    // ACC: PSD columns are ADDED to what `out` holds (multitaper spectrogram: one launch per taper, no separate add pass).
+    // ACC: PSD columns are ADDED to what `out` holds (psd_only == 3, and the tapers after a unit's first in mt_spectrogram).
     // Compile time: as a run-time predicate the read-modify-write put a scoreboard wait in front of every store (ncu).
     auto put = [&](T* ptr, T val) { if constexpr (ACC) *ptr = add_rn(*ptr, val); else *ptr = val; };
     const bool hasB = HASB < 0 ? hasB_rt : (HASB != 0);
@@ -451,6 +462,7 @@ template <typename In> struct StftStream {
     int64_t lds, h;             // column stride of `seam`, samples of history
     int64_t ldo;                // output columns per channel (replaces k as the column stride)
     int tma;                    // the call meets the TMA alignment conditions (stft_w1k_kernel: stage every unit)
+    int ntapers;                // WIN == 2 instances (mt_spectrogram): taper rows of the window, n values apart
     // first sample of the unit that starts at v[start] of channel c (x: the chunk, chan_stride = nx)
     __device__ __forceinline__ const In* src(const In* x, int64_t chan_stride, int64_t c, int64_t start) const {
         return start < h ? seam + c * lds + start : x + c * chan_stride + (start - h);
@@ -458,19 +470,22 @@ template <typename In> struct StftStream {
 };
 
 // One unit of the STFT kernel.  FAST: n == N (no zero padding) and, for real input, both segments present -- no per-sample
-// predicates; WIN: 1 window table present, 0 none (compile time), -1 run time.
+// predicates; WIN: 1 window table present, 0 none (compile time), -1 run time, 2 one row of a multitaper plan's tapers (PSD
+// columns; `add`: added to what `out` holds, in the emit step).
 template <typename T, int N, bool CPLX, bool TMA, int WIN, bool FAST, class IssueNext>
 __device__ __forceinline__ void stft_unit(const FftCtx<T>& ctx, cx<T>* sm, int tid, const typename in_type<T, CPLX>::type* pa,
                                           int64_t hop, int n, bool hasB_rt, const typename win_t<T>::type* __restrict__ win,
                                           void* __restrict__ out_, int64_t colA, int nout, int psd_only, int onesided, T m1,
-                                          T m2, IssueNext issue_next) {
+                                          T m2, IssueNext issue_next, bool add = false) {
     constexpr int NT = fft_threads<N>::value;
     constexpr int NB16 = N / 16;
     constexpr int ITL = (NB16 + NT - 1) / NT;
     using In = typename in_type<T, CPLX>::type;
     const In* pb = pa + hop;
     const bool hasB = FAST ? !CPLX : hasB_rt;
-    const bool use_win = WIN < 0 ? (win != nullptr) : (WIN != 0);
+    // (Float64 taper rows keep the run-time test of WIN = -1: a product known to be taken is contracted into the first
+    //  butterfly's adds, which rounds differently from the spectrogram of one taper)
+    const bool use_win = (WIN < 0 || (WIN == 2 && sizeof(T) == 8)) ? (win != nullptr) : (WIN != 0);
     auto ld0 = [&](int j, int, int) -> cx<T> {
         if constexpr (!FAST) { if (j >= n) return mkc<T>(T(0), T(0)); }
         if constexpr (CPLX) {
@@ -501,7 +516,10 @@ __device__ __forceinline__ void stft_unit(const FftCtx<T>& ctx, cx<T>* sm, int t
     }
     __syncthreads();
     constexpr int HB = FAST ? (CPLX ? 0 : 1) : -1;
-    if (psd_only & 2) {                                  // bit 1: accumulate into `out` (rare: multitaper)
+    if constexpr (WIN == 2) {
+        if (add) stft_emit<T, N, CPLX, 1, HB, -1, true>(sm, out_, colA, nout, hasB, onesided, m1, m2, tid);
+        else stft_emit<T, N, CPLX, 1, HB, -1, false>(sm, out_, colA, nout, hasB, onesided, m1, m2, tid);
+    } else if (psd_only & 2) {                           // bit 1: accumulate into `out`
         stft_emit<T, N, CPLX, 1, -1, -1, true>(sm, out_, colA, nout, hasB, onesided, m1, m2, tid);
     } else if (psd_only) {
         if (CPLX || !onesided) stft_emit<T, N, CPLX, 1, HB, 0>(sm, out_, colA, nout, hasB, 0, m1, m2, tid);
@@ -580,10 +598,23 @@ stft_fused_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, i
             }
         };
         const int64_t colA = (chan * ss.ldo + segA) * (int64_t)nout;
-        if (full && (CPLX || hasB))
-            stft_unit<T, N, CPLX, TMA, WIN, true>(ctx, sm, tid, pa, hop, n, hasB, win, out_, colA, nout, psd_only, onesided, m1, m2, issue_next);
-        else
-            stft_unit<T, N, CPLX, TMA, WIN, false>(ctx, sm, tid, pa, hop, n, hasB, win, out_, colA, nout, psd_only, onesided, m1, m2, issue_next);
+        if constexpr (WIN == 2) {
+            // every taper transforms the staged unit, in taper order; the staging buffer is refilled after the last one's
+            // first pass
+            for (int t = 0; t < ss.ntapers; ++t) {
+                const auto* wt = win + (int64_t)t * n;
+                auto issue_last = [&]() { if (t + 1 == ss.ntapers) issue_next(); };
+                if (full && (CPLX || hasB))
+                    stft_unit<T, N, CPLX, TMA, WIN, true>(ctx, sm, tid, pa, hop, n, hasB, wt, out_, colA, nout, 1, onesided, m1, m2, issue_last, t > 0);
+                else
+                    stft_unit<T, N, CPLX, TMA, WIN, false>(ctx, sm, tid, pa, hop, n, hasB, wt, out_, colA, nout, 1, onesided, m1, m2, issue_last, t > 0);
+            }
+        } else {
+            if (full && (CPLX || hasB))
+                stft_unit<T, N, CPLX, TMA, WIN, true>(ctx, sm, tid, pa, hop, n, hasB, win, out_, colA, nout, psd_only, onesided, m1, m2, issue_next);
+            else
+                stft_unit<T, N, CPLX, TMA, WIN, false>(ctx, sm, tid, pa, hop, n, hasB, win, out_, colA, nout, psd_only, onesided, m1, m2, issue_next);
+        }
         chan = nchan;
         uin = nuin;
     }
@@ -612,7 +643,9 @@ __host__ __device__ inline size_t warp_bytes(int64_t stage_elems, size_t elt) { 
 }  // namespace w1k
 
 // Arguments as stft_fused_kernel.  A stream keeps this plan whatever the alignment of the call: ss.tma = 0 (unaligned) reads
-// every unit directly from global memory in the first pass instead of staging it.
+// every unit directly from global memory in the first pass instead of staging it.  WIN: 0 no window, 1 the window staged in
+// shared memory, 2 the ss.ntapers taper rows of a multitaper plan, read through L1 (7 rows of 8 KB would cost residency),
+// each unit transformed under every row in turn and its PSD columns summed over them in `out`.
 template <bool CPLX, int WIN, int WARPS>
 __global__ void __launch_bounds__(32 * WARPS)
 stft_w1k_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int64_t units_per_chan, int64_t total_units,
@@ -630,12 +663,12 @@ stft_w1k_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int
     float2* wsm = reinterpret_cast<float2*>(smem_raw + w1k::T32_LEN * sizeof(cx<T>));
     const size_t stage_elems = (size_t)(CPLX ? n : hop + n);
     const size_t wbytes = w1k::warp_bytes((int64_t)stage_elems, sizeof(In));
-    unsigned char* wbase = smem_raw + w1k::T32_LEN * sizeof(cx<T>) + (WIN ? (size_t)n * sizeof(float2) : 0) + (size_t)warp * wbytes;
+    unsigned char* wbase = smem_raw + w1k::T32_LEN * sizeof(cx<T>) + (WIN == 1 ? (size_t)n * sizeof(float2) : 0) + (size_t)warp * wbytes;
     cx<T>* sm = reinterpret_cast<cx<T>*>(wbase);
     In* stage = reinterpret_cast<In*>(sm + w1k::DATA_LEN);
     uint64_t* bar = reinterpret_cast<uint64_t*>(wbase + wbytes - 16);
     for (int i = threadIdx.x; i < w1k::T32_LEN; i += 32 * WARPS) t32[i] = g32[i];
-    if constexpr (WIN != 0) {
+    if constexpr (WIN == 1) {
         for (int i = threadIdx.x; i < n; i += 32 * WARPS) wsm[i] = win[i];
     }
     if (lane == 0) {
@@ -675,100 +708,110 @@ stft_w1k_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int
             mbar_wait(bar, parity);
             parity ^= 1;
         }
-        // first pass: plain 32-point DFT of x[lane + 32 m] (window applied), 32 contiguous slots at block `lane`.  Written
-        // out once per source, so that a staged unit is read by shared-memory loads (through a pointer that may point to
-        // either space they become generic loads); an unaligned streaming call reads its units directly
-        cx<T> v[32];
-        const bool fast = full && (CPLX || hasB);
-        auto first_pass = [&](const In* pa) {
-            const In* pb = pa + hop;
+        // WIN == 2: every taper row transforms the unit in turn, in taper order (the same staged samples)
+        for (int t = 0; t < (WIN == 2 ? ss.ntapers : 1); ++t) {
+            const float2* wrow = WIN == 2 ? win + (int64_t)t * n : wsm;
+            // first pass: plain 32-point DFT of x[lane + 32 m] (window applied), 32 contiguous slots at block `lane`.  Written
+            // out once per source, so that a staged unit is read by shared-memory loads (through a pointer that may point to
+            // either space they become generic loads); an unaligned streaming call reads its units directly
+            cx<T> v[32];
+            const bool fast = full && (CPLX || hasB);
+            auto first_pass = [&](const In* pa) {
+                const In* pb = pa + hop;
 #pragma unroll
-            for (int m = 0; m < 32; ++m) {
-                const int j = lane + 32 * m;
-                if constexpr (CPLX) {
-                    cx<T> x = (fast || j < n) ? pa[j] : mkc<T>(0.f, 0.f);
-                    if constexpr (WIN != 0) { const float2 w = wsm[fast || j < n ? j : 0]; x = mkc<T>(win_mul(x.x, w), win_mul(x.y, w)); }
-                    v[m] = x;
-                } else {
-                    float a = (fast || j < n) ? pa[j] : 0.f;
-                    float b = (fast || (hasB && j < n)) ? pb[j] : 0.f;
-                    if constexpr (WIN != 0) { const float2 w = wsm[fast || j < n ? j : 0]; a = win_mul(a, w); b = win_mul(b, w); }
-                    v[m] = mkc<T>(a, b);
-                }
-            }
-        };
-        if (ss.tma) first_pass(stage);
-        else first_pass(src_of(chan, uin));
-        __syncwarp();                                  // every lane has read the staging buffer (and the previous unit's spectrum)
-        if (lane == 0 && gu + 1 < u1 && ss.tma) {       // refill it with the next unit while this one is transformed
-            fence_proxy_async_shared();
-            mbar_expect_tx(bar, bytes_of(nuin));
-            tma_load_1d(stage, src_of(nchan, nuin), bytes_of(nuin), bar);
-        }
-        fft_bfly<T, 32, true>(v, nullptr);
-        {
-            cx<T>* p = sm + w1k::pad(32 * lane);
-#pragma unroll
-            for (int r = 0; r < 32; r += 2) sts2<T>(p + w1k::pad(r), v[r], v[r + 1]);
-        }
-        __syncwarp();
-        // last pass: radix 32 at stride 32, twiddles W_1024^lane; the spectrum goes back in natural order, in place
-        {
-            cx<T>* p = sm + w1k::pad(lane);
-#pragma unroll
-            for (int r = 0; r < 32; ++r) v[r] = p[38 * r];
-            fft_bfly<T, 32, false>(v, tw);
-#pragma unroll
-            for (int r = 0; r < 32; ++r) p[38 * r] = v[r];
-        }
-        __syncwarp();
-        // emit: bins kk = lane + 32 i; N - kk = (32 - lane) + 32 (31 - i) for lane > 0
-        const int64_t colA = (chan * ss.ldo + segA) * (int64_t)nout;
-        const cx<T>* pk = sm + w1k::pad(lane);
-        const cx<T>* pm = lane ? sm + w1k::pad(32 - lane) : sm;
-        const bool half = !CPLX && onesided;
-        // (the accumulate flag is resolved once per unit: as a run-time predicate inside the stores it put a scoreboard wait
-        //  in front of every one of them)
-        auto emit_all = [&](auto acc_) {
-            constexpr bool ACC = decltype(acc_)::value;
-            auto put = [&](T* ptr, T val) { if constexpr (ACC) *ptr = add_rn(*ptr, val); else *ptr = val; };
-            auto emit = [&](int kk, cx<T> zk, cx<T> zm, bool edge) {
-                if (psd_only) {
-                    T* out = reinterpret_cast<T*>(out_);
+                for (int m = 0; m < 32; ++m) {
+                    const int j = lane + 32 * m;
                     if constexpr (CPLX) {
-                        put(out + colA + kk, cabs2(zk) * m1);
+                        cx<T> x = (fast || j < n) ? pa[j] : mkc<T>(0.f, 0.f);
+                        if constexpr (WIN != 0) { const float2 w = wrow[fast || j < n ? j : 0]; x = mkc<T>(win_mul(x.x, w), win_mul(x.y, w)); }
+                        v[m] = x;
                     } else {
-                        const cx<T> A = mkc<T>(0.5f * (zk.x + zm.x), 0.5f * (zk.y - zm.y));
-                        const cx<T> B = mkc<T>(0.5f * (zk.y + zm.y), 0.5f * (zm.x - zk.x));
-                        const T m = (onesided && !edge) ? m2 : m1;
-                        put(out + colA + kk, cabs2(A) * m);
-                        if (hasB) put(out + colA + nout + kk, cabs2(B) * m);
-                    }
-                } else {
-                    cx<T>* out = reinterpret_cast<cx<T>*>(out_);
-                    if constexpr (CPLX) {
-                        out[colA + kk] = zk;
-                    } else {
-                        out[colA + kk] = mkc<T>(0.5f * (zk.x + zm.x), 0.5f * (zk.y - zm.y));
-                        if (hasB) out[colA + nout + kk] = mkc<T>(0.5f * (zk.y + zm.y), 0.5f * (zm.x - zk.x));
+                        float a = (fast || j < n) ? pa[j] : 0.f;
+                        float b = (fast || (hasB && j < n)) ? pb[j] : 0.f;
+                        if constexpr (WIN != 0) { const float2 w = wrow[fast || j < n ? j : 0]; a = win_mul(a, w); b = win_mul(b, w); }
+                        v[m] = mkc<T>(a, b);
                     }
                 }
             };
+            if (ss.tma) first_pass(stage);
+            else first_pass(src_of(chan, uin));
+            __syncwarp();                                  // every lane has read the staging buffer (and the previous unit's spectrum)
+            // refill it with the next unit while this one is transformed (after the last taper's first pass)
+            if (lane == 0 && gu + 1 < u1 && ss.tma && (WIN != 2 || t + 1 == ss.ntapers)) {
+                fence_proxy_async_shared();
+                mbar_expect_tx(bar, bytes_of(nuin));
+                tma_load_1d(stage, src_of(nchan, nuin), bytes_of(nuin), bar);
+            }
+            fft_bfly<T, 32, true>(v, nullptr);
+            {
+                cx<T>* p = sm + w1k::pad(32 * lane);
 #pragma unroll
-            for (int i = 0; i < 32; ++i) {
-                if (i >= 16 && half) break;
-                const cx<T> zk = pk[38 * i];
-                cx<T> zm = zk;
-                if constexpr (!CPLX) zm = pm[lane ? 38 * (31 - i) : 38 * ((32 - i) & 31)];
-                emit(lane + 32 * i, zk, zm, (i == 0 || i == 16) && lane == 0);
+                for (int r = 0; r < 32; r += 2) sts2<T>(p + w1k::pad(r), v[r], v[r + 1]);
             }
-            if (half && lane == 0) {
-                const cx<T> z = sm[w1k::pad(N / 2)];
-                emit(N / 2, z, z, true);
+            __syncwarp();
+            // last pass: radix 32 at stride 32, twiddles W_1024^lane; the spectrum goes back in natural order, in place
+            {
+                cx<T>* p = sm + w1k::pad(lane);
+#pragma unroll
+                for (int r = 0; r < 32; ++r) v[r] = p[38 * r];
+                fft_bfly<T, 32, false>(v, tw);
+#pragma unroll
+                for (int r = 0; r < 32; ++r) p[38 * r] = v[r];
             }
-        };
-        if (psd_only & 2) emit_all(std::true_type{});
-        else emit_all(std::false_type{});
+            __syncwarp();
+            // emit: bins kk = lane + 32 i; N - kk = (32 - lane) + 32 (31 - i) for lane > 0
+            const int64_t colA = (chan * ss.ldo + segA) * (int64_t)nout;
+            const cx<T>* pk = sm + w1k::pad(lane);
+            const cx<T>* pm = lane ? sm + w1k::pad(32 - lane) : sm;
+            const bool half = !CPLX && onesided;
+            // (the accumulate flag is resolved once per unit: as a run-time predicate inside the stores it put a scoreboard wait
+            //  in front of every one of them)
+            auto emit_all = [&](auto acc_) {
+                constexpr bool ACC = decltype(acc_)::value;
+                auto put = [&](T* ptr, T val) { if constexpr (ACC) *ptr = add_rn(*ptr, val); else *ptr = val; };
+                auto emit = [&](int kk, cx<T> zk, cx<T> zm, bool edge) {
+                    if (psd_only) {
+                        T* out = reinterpret_cast<T*>(out_);
+                        if constexpr (CPLX) {
+                            put(out + colA + kk, cabs2(zk) * m1);
+                        } else {
+                            const cx<T> A = mkc<T>(0.5f * (zk.x + zm.x), 0.5f * (zk.y - zm.y));
+                            const cx<T> B = mkc<T>(0.5f * (zk.y + zm.y), 0.5f * (zm.x - zk.x));
+                            const T m = (onesided && !edge) ? m2 : m1;
+                            put(out + colA + kk, cabs2(A) * m);
+                            if (hasB) put(out + colA + nout + kk, cabs2(B) * m);
+                        }
+                    } else {
+                        cx<T>* out = reinterpret_cast<cx<T>*>(out_);
+                        if constexpr (CPLX) {
+                            out[colA + kk] = zk;
+                        } else {
+                            out[colA + kk] = mkc<T>(0.5f * (zk.x + zm.x), 0.5f * (zk.y - zm.y));
+                            if (hasB) out[colA + nout + kk] = mkc<T>(0.5f * (zk.y + zm.y), 0.5f * (zm.x - zk.x));
+                        }
+                    }
+                };
+#pragma unroll
+                for (int i = 0; i < 32; ++i) {
+                    if (i >= 16 && half) break;
+                    const cx<T> zk = pk[38 * i];
+                    cx<T> zm = zk;
+                    if constexpr (!CPLX) zm = pm[lane ? 38 * (31 - i) : 38 * ((32 - i) & 31)];
+                    emit(lane + 32 * i, zk, zm, (i == 0 || i == 16) && lane == 0);
+                }
+                if (half && lane == 0) {
+                    const cx<T> z = sm[w1k::pad(N / 2)];
+                    emit(N / 2, z, z, true);
+                }
+            };
+            if constexpr (WIN == 2) {                  // later tapers add to the first one's columns
+                if (t > 0) emit_all(std::true_type{});
+                else emit_all(std::false_type{});
+            } else {
+                if (psd_only & 2) emit_all(std::true_type{});
+                else emit_all(std::false_type{});
+            }
+        }
         chan = nchan;
         uin = nuin;
     }
@@ -893,6 +936,47 @@ __global__ void stft_store_kernel(const cx<T>* __restrict__ X, int64_t nbins_fft
 template <typename T>
 __global__ void acc_add_kernel(T* __restrict__ out, const T* __restrict__ add, int64_t n) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] += add[i];
+}
+
+// mt_pgram, cuFFT sizes: the (channel, taper) pairs f0 .. f0 + nf - 1 (f = c ntapers + t) fill the cuFFT batch in order.
+// Slot b = blockIdx.y holds pair f0 + b: buf[b][i] = taper row t [i] * s[c len + i] (i < n), 0 for n <= i < nfft and for slots
+// past the list -- seg_window_kernel's values under row t.
+template <typename T, bool CPLX>
+__global__ void mt_seg_kernel(const void* __restrict__ s_, int64_t len, int64_t f0, int64_t nf, int64_t ntapers, int64_t n,
+                              int64_t nfft, const typename win_t<T>::type* __restrict__ rows, void* __restrict__ buf_) {
+    using In = typename in_type<T, CPLX>::type;
+    const In* s = reinterpret_cast<const In*>(s_);
+    const int64_t b = blockIdx.y;
+    In* buf = reinterpret_cast<In*>(buf_) + b * nfft;
+    const int64_t f = f0 + b, c = f / ntapers, t = f - c * ntapers;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nfft; i += (int64_t)gridDim.x * blockDim.x) {
+        In v;
+        if constexpr (CPLX) v = mkc<T>(T(0), T(0)); else v = T(0);
+        if (b < nf && i < n) {
+            v = s[c * len + i];
+            const auto w = rows[t * n + i];
+            if constexpr (CPLX) v = mkc<T>(win_mul(v.x, w), win_mul(v.y, w)); else v = win_mul(v, w);
+        }
+        buf[i] = v;
+    }
+}
+
+// mt_pgram, cuFFT sizes: thread (bin kk, channel f0 / ntapers + blockIdx.y) adds (double)|X|^2 of its channel's slots to
+// acc (nout x nchan) one taper at a time, in taper order -- continuing the channel's sum when its first tapers were in an
+// earlier batch -- so that every channel gets pow_acc_kernel's sum over its tapers whatever the batch boundaries.  Two-sided
+// real output: bin kk >= nbins_fft reads nfft - kk.
+template <typename T>
+__global__ void mt_pow_acc_kernel(const cx<T>* __restrict__ X, int64_t nbins_fft, int64_t nfft, int64_t nout, int64_t f0,
+                                  int64_t nf, int64_t ntapers, double* __restrict__ acc) {
+    const int64_t kk = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (kk >= nout) return;
+    const int64_t c = f0 / ntapers + blockIdx.y;
+    const int64_t a = c * ntapers > f0 ? c * ntapers : f0, e = (c + 1) * ntapers < f0 + nf ? (c + 1) * ntapers : f0 + nf;
+    const int64_t src = kk < nbins_fft ? kk : nfft - kk;
+    double* q = acc + c * nout + kk;
+    double sum = a > c * ntapers ? *q : 0.0;
+    for (int64_t f = a; f < e; ++f) sum += (double)cabs2(X[(f - f0) * nbins_fft + src]);
+    *q = sum;
 }
 
 // Multitaper cross spectra (src/multitaper.jl:553-616).
@@ -1112,25 +1196,28 @@ using welch_kern_t = void (*)(const void*, welch_arg<BATCH, int64_t>, welch_arg<
 // The fused Welch instances (MODE: staging / window placement, G: thread groups per CTA) in order of preference (measured
 // sweep): f(kernel, shared-memory bytes, MODE, G) for each one that may run on TMA-`aligned` segments with(out) a window, the
 // direct-load instance last.  These are all the instances there are; dspb200_spec_plan_pin_welch names them from this list.
-template <typename T, int N, bool CPLX, bool BATCH, typename F>
+// TAPERS (mt_pgram): a window row per unit, which MODE 2 / 3 (one window, staged once per CTA) cannot address.
+template <typename T, int N, bool CPLX, bool BATCH, bool TAPERS, typename F>
 static int welch_candidates(const SpecPlanImpl* p, bool aligned, bool windowed, F&& f) {
     constexpr bool MULTI = sizeof(T) == 4 && N >= 1024 && N <= 4096;       // sizes that get multi-group variants
     constexpr bool WREGOK = sizeof(T) == 4 && N <= 4096;                   // window in registers: 32 extra registers per thread
 #define DSP_WELCH_CAND(MODE_, G_)                                                                                   \
-    DSP_TRY(f(welch_kern_t<T, BATCH>(welch_fused_kernel<T, N, CPLX, MODE_, G_, BATCH>),                             \
+    DSP_TRY(f(welch_kern_t<T, BATCH>(welch_fused_kernel<T, N, CPLX, MODE_, G_, BATCH, TAPERS>),                     \
               welch_layout<T, N, CPLX, MODE_>::total(p->n, p->hop, G_), MODE_, G_))
     if (aligned) {
-        if (windowed) {
-            if constexpr (CPLX) {
-                // complex: two CTAs per SM with the window in registers, then in shared memory
-                if constexpr (WREGOK) DSP_WELCH_CAND(3, 1);
-                DSP_WELCH_CAND(2, 1);
-                if constexpr (MULTI) { DSP_WELCH_CAND(3, 2); DSP_WELCH_CAND(2, 2); }
-            } else {
-                // real: three thread groups sharing tables + window, then two, then two CTAs
-                if constexpr (MULTI) { DSP_WELCH_CAND(2, 3); DSP_WELCH_CAND(2, 2); }
-                DSP_WELCH_CAND(2, 1);
-                if constexpr (WREGOK) DSP_WELCH_CAND(3, 1);
+        if constexpr (!TAPERS) {
+            if (windowed) {
+                if constexpr (CPLX) {
+                    // complex: two CTAs per SM with the window in registers, then in shared memory
+                    if constexpr (WREGOK) DSP_WELCH_CAND(3, 1);
+                    DSP_WELCH_CAND(2, 1);
+                    if constexpr (MULTI) { DSP_WELCH_CAND(3, 2); DSP_WELCH_CAND(2, 2); }
+                } else {
+                    // real: three thread groups sharing tables + window, then two, then two CTAs
+                    if constexpr (MULTI) { DSP_WELCH_CAND(2, 3); DSP_WELCH_CAND(2, 2); }
+                    DSP_WELCH_CAND(2, 1);
+                    if constexpr (WREGOK) DSP_WELCH_CAND(3, 1);
+                }
             }
         }
         if constexpr (MULTI && !CPLX) DSP_WELCH_CAND(1, 3);
@@ -1156,7 +1243,7 @@ static int welch_per_sm(const SpecPlanImpl* p, K k, int threads, int g, size_t s
 // is taken, otherwise the one with the most, and the direct-load instance only when no other fits.  The selection walks up
 // to nine instances through cudaFuncSetAttribute + the occupancy calculator (tens of microseconds), hence the cache.
 // row_cap: the single-signal path's `nparts` (one wave never has more virtual CTAs than `partial` has rows), 0 for a batch.
-template <typename T, int N, bool CPLX, bool BATCH>
+template <typename T, int N, bool CPLX, bool BATCH, bool TAPERS = false>
 static int welch_select(SpecPlanImpl* p, SpecPlanImpl::WelchCfg& cfg, bool aligned, int64_t row_cap) {
     if (cfg.kern != nullptr) return DSPB200_OK;
     constexpr int NT = fft_threads<N>::value;
@@ -1173,7 +1260,7 @@ static int welch_select(SpecPlanImpl* p, SpecPlanImpl::WelchCfg& cfg, bool align
         if (warps > best.warps) best = Cand{k, smem, mode, g, warps, per_sm};
         return DSPB200_OK;
     };
-    DSP_TRY((welch_candidates<T, N, CPLX, BATCH>(p, aligned, p->d_window != nullptr, consider)));
+    DSP_TRY((welch_candidates<T, N, CPLX, BATCH, TAPERS>(p, aligned, p->d_window != nullptr, consider)));
     DSP_REQUIRE(best.k != nullptr, "no %sWelch kernel configuration fits (nfft=%lld)", BATCH ? "batched " : "", (long long)p->nfft);
     DSP_TRY(set_smem(best.k, best.smem));              // (the last candidate examined may have left a different limit)
     cfg.kern = reinterpret_cast<void*>(best.k); cfg.smem = best.smem; cfg.g = best.g; cfg.per_sm = best.per_sm;
@@ -1311,9 +1398,11 @@ static int launch_welch_batch(SpecPlanImpl* p, const void* s, int64_t len, int64
 // The history side of an STFT call (dspb200_stft_stream_exec_dev); a one-shot call has none and ldo = k
 // (seam, lds: the copy of every channel's first virtual-column samples that the edge kernel wrote; fused sizes only).
 // keep_plan: run the instance an aligned call of the plan runs, whatever the alignment of this call (streams)
+// ntapers > 0: an mt_spectrogram call -- PSD columns summed over the plan's taper rows in one launch (WIN == 2 instances).
 struct StftStreamArgs {
     const void* hist = nullptr; int64_t h = 0, ldh = 0, ldo = 0; const void* seam = nullptr; int64_t lds = 0;
     bool keep_plan = false;
+    int ntapers = 0;
 };
 
 // k segments of each channel's virtual column [history; s], s being the len x nchan chunk (one-shot: the whole matrix).  A
@@ -1341,17 +1430,18 @@ static int launch_stft_fused(SpecPlanImpl* p, const void* s, int64_t len, int64_
     const int64_t upc = CPLX ? k : (k + 1) / 2;
     const int64_t units = upc * nchan;
     if (units < 1) return DSPB200_OK;
-    const SS ss{reinterpret_cast<const In*>(sa.seam), sa.lds, sa.h, sa.ldo, (W1K ? aligned : tma) ? 1 : 0};
+    const SS ss{reinterpret_cast<const In*>(sa.seam), sa.lds, sa.h, sa.ldo, (W1K ? aligned : tma) ? 1 : 0, sa.ntapers};
     const auto* w = reinterpret_cast<const typename win_t<T>::type*>(p->d_window);
+    const bool mt = sa.ntapers > 0;
     if constexpr (W1K) {
         // one warp per unit (stft_w1k_kernel): a one-shot call needs the TMA alignment conditions, a stream those of its plan
         if ((sa.keep_plan ? plan_aligned : aligned) && p->d_t32 != nullptr) {
             constexpr int WARPS = 4;
-            const size_t smem1 = (size_t)w1k::T32_LEN * sizeof(cx<float>) + (w ? (size_t)p->n * sizeof(float2) : 0) +
+            const size_t smem1 = (size_t)w1k::T32_LEN * sizeof(cx<float>) + (w && !mt ? (size_t)p->n * sizeof(float2) : 0) +
                                  (size_t)WARPS * w1k::warp_bytes(CPLX ? p->n : p->hop + p->n, sizeof(In));
             using K1 = void (*)(const void*, int64_t, int64_t, int64_t, int64_t, int64_t, int, const float2*, const cx<float>*, void*, int,
                                 int, int, float, float, SS);
-            K1 k1 = w ? (K1)stft_w1k_kernel<CPLX, 1, WARPS> : (K1)stft_w1k_kernel<CPLX, 0, WARPS>;
+            K1 k1 = mt ? (K1)stft_w1k_kernel<CPLX, 2, WARPS> : w ? (K1)stft_w1k_kernel<CPLX, 1, WARPS> : (K1)stft_w1k_kernel<CPLX, 0, WARPS>;
             if (smem1 <= p->smem_optin) {
                 DSP_TRY(set_smem(k1, smem1));
                 int per = 1;
@@ -1375,7 +1465,10 @@ static int launch_stft_fused(SpecPlanImpl* p, const void* s, int64_t len, int64_
     // window presence is a compile-time property of the Float32 kernels (predicated-off window products still issue)
     constexpr bool SPEC = sizeof(T) == 4;
     Kern kern;
-    if constexpr (W1K) {
+    if (mt) {
+        if constexpr (W1K) kern = (Kern)stft_fused_kernel<T, N, CPLX, false, 2>;
+        else kern = tma ? (Kern)stft_fused_kernel<T, N, CPLX, true, 2> : (Kern)stft_fused_kernel<T, N, CPLX, false, 2>;
+    } else if constexpr (W1K) {
         kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, false, 1> : (Kern)stft_fused_kernel<T, N, CPLX, false, 0>;
     } else if constexpr (SPEC) {
         if (tma) kern = w ? (Kern)stft_fused_kernel<T, N, CPLX, true, 1> : (Kern)stft_fused_kernel<T, N, CPLX, true, 0>;
@@ -1396,7 +1489,7 @@ static int launch_stft_fused(SpecPlanImpl* p, const void* s, int64_t len, int64_
 
 // Pinned Welch launch configuration (dspb200_spec_plan_pin_welch, a testing aid): any instance of welch_candidates.  Fills
 // both alignment classes of the cache: aligned calls get (mode, g), unaligned ones MODE 0, G = 1; both `vctas`.
-template <typename T, int N, bool CPLX, bool BATCH>
+template <typename T, int N, bool CPLX, bool BATCH, bool TAPERS = false>
 static int welch_pin(SpecPlanImpl* p, int mode, int g, int64_t vctas) {
     constexpr int NT = fft_threads<N>::value;
     using Kern = welch_kern_t<T, BATCH>;
@@ -1405,7 +1498,7 @@ static int welch_pin(SpecPlanImpl* p, int mode, int g, int64_t vctas) {
         const int m = a ? mode : 0, gg = a ? g : 1;
         Kern k = nullptr;
         size_t smem = 0;
-        DSP_TRY((welch_candidates<T, N, CPLX, BATCH>(p, true, true, [&](Kern kc, size_t sc, int mc, int gc) -> int {
+        DSP_TRY((welch_candidates<T, N, CPLX, BATCH, TAPERS>(p, true, true, [&](Kern kc, size_t sc, int mc, int gc) -> int {
             if (mc == m && gc == gg) { k = kc; smem = sc; }
             return DSPB200_OK;
         })));
@@ -1430,7 +1523,7 @@ static int welch_pin(SpecPlanImpl* p, int mode, int g, int64_t vctas) {
         pinned[a].kern = reinterpret_cast<void*>(k); pinned[a].smem = smem; pinned[a].g = gg; pinned[a].per_sm = per_sm;
         pinned[a].threads = NT * gg; pinned[a].mode = m; pinned[a].vctas = vctas;
     }
-    SpecPlanImpl::WelchCfg* cfg = BATCH ? p->welch_batch_cfg : p->welch_cfg;
+    SpecPlanImpl::WelchCfg* cfg = TAPERS ? p->welch_mt_cfg : BATCH ? p->welch_batch_cfg : p->welch_cfg;
     cfg[0] = pinned[0];
     cfg[1] = pinned[1];
     return DSPB200_OK;
@@ -1737,6 +1830,64 @@ static int mt_cross_run(dspb200_spec_plan* plan, const void* signal, int64_t nch
     return DSPB200_OK;
 }
 
+// mt_pgram of the nchan columns of a len x nchan matrix (len = n), fused sizes: per channel group, one batched Welch launch
+// whose work items are the channels and whose units are a channel's tapers (welch_fused_kernel<..., TAPERS = true>: the
+// tapers' |X_t|^2 summed in registers in taper order, one partial row per channel -- a channel's tapers are never split, so a
+// column's bits do not depend on the other columns), then welch_finalize_kernel.  The groups follow launch_welch_batch's
+// scratch rule.
+template <typename T, int N, bool CPLX>
+static int launch_mt_pgram(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan, void* out, cudaStream_t st) {
+    using In = typename in_type<T, CPLX>::type;
+    const bool aligned = welch_batch_aligned(p, s, len, nchan, sizeof(In));
+    SpecPlanImpl::WelchCfg& cfg = p->welch_mt_cfg[aligned ? 1 : 0];
+    DSP_TRY((welch_select<T, N, CPLX, true, true>(p, cfg, aligned, 0)));
+    const int64_t rows_cap = (int64_t)(WELCH_BATCH_SCRATCH / ((size_t)N * sizeof(T)));
+    const int64_t gc_max = nchan < rows_cap ? nchan : rows_cap;
+    for (int64_t c0 = 0; c0 < nchan; c0 += gc_max) {
+        WelchBatchWork w;                                // one item per channel: its ntapers units, one segment
+        w.k = 1;
+        w.upc = w.per = p->ntapers;
+        w.slices = 1;
+        w.nitems = nchan - c0 < gc_max ? nchan - c0 : gc_max;
+        DSP_TRY(p->bpartial.reserve((size_t)w.nitems * N * sizeof(T)));
+        DSP_TRY((welch_batch_launch<T, CPLX>(p, cfg, w, (const In*)s + c0 * len, len, p->bpartial.p, st)));
+        welch_finalize_kernel<T, N><<<dim3((unsigned)cdiv(p->nout, 32), (unsigned)w.nitems), 32, 0, st>>>(
+            reinterpret_cast<const T*>(p->bpartial.p), 1, reinterpret_cast<T*>(out) + c0 * p->nout, (int)p->nout, CPLX ? 0 : 1,
+            (int)p->onesided, 1.0, 2.0);
+        DSP_LAUNCH_OK();
+    }
+    return DSPB200_OK;
+}
+
+// mt_pgram, cuFFT sizes: the nchan x ntapers (channel, taper) pairs through the plan's batch -- mt_seg_kernel, cuFFT,
+// mt_pow_acc_kernel: three launches per batch -- into a Float64 nout x nchan accumulator, then the fft2pow! scaling (r = 1)
+// of welch_stream_power_kernel, which rounds as pow_finalize_kernel does.
+template <typename T> static int mt_pgram_generic(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, void* out,
+                                                   cudaStream_t st) {
+    SpecPlanImpl* p = &plan->impl;
+    DSP_TRY(generic_prepare(p));
+    DSP_TRY(p->bacc.reserve((size_t)(p->nout * nchan) * sizeof(double)));
+    double* acc = reinterpret_cast<double*>(p->bacc.p);
+    const auto* rows = reinterpret_cast<const typename win_t<T>::type*>(p->d_window);
+    const int64_t nt = p->ntapers, pairs = nchan * nt;
+    const int threads = 256;
+    for (int64_t f0 = 0; f0 < pairs; f0 += p->batch) {
+        const int64_t nf = pairs - f0 < p->batch ? pairs - f0 : p->batch;
+        const dim3 gseg(stream_generic_cols(p, p->nfft, threads), (unsigned)p->batch);
+        if (p->cplx)
+            mt_seg_kernel<T, true><<<gseg, threads, 0, st>>>(s, len, f0, nf, nt, p->n, p->nfft, rows, p->segbuf.p);
+        else
+            mt_seg_kernel<T, false><<<gseg, threads, 0, st>>>(s, len, f0, nf, nt, p->n, p->nfft, rows, p->segbuf.p);
+        DSP_LAUNCH_OK();
+        DSP_TRY(fft_exec(p->fft, p->cplx, p->f64, CUFFT_FORWARD, p->segbuf.p, p->specbuf.p, st));
+        const int64_t nc = (f0 + nf - 1) / nt - f0 / nt + 1;                 // channels with a pair in this batch
+        mt_pow_acc_kernel<T><<<dim3((unsigned)cdiv(p->nout, 128), (unsigned)nc), 128, 0, st>>>(
+            reinterpret_cast<const cx<T>*>(p->specbuf.p), p->nbins_fft, p->nfft, p->nout, f0, nf, nt, acc);
+        DSP_LAUNCH_OK();
+    }
+    return dspb200_welch_stream_power_dev(plan, acc, nchan, 1.0, out, st);
+}
+
 // periodogram(s::AbstractMatrix; nfft, fs, radialsum, radialavg), src/periodograms.jl:473-509, device pointers: queues the
 // work on st (cached plan + scratch arena: the caller goes through convenience_call)
 template <typename T>
@@ -1929,6 +2080,9 @@ int dspb200_spec_plan_pin_welch(dspb200_spec_plan* plan, int batched, int mode, 
     DSP_REQUIRE(plan != nullptr, "plan is NULL");
     SpecPlanImpl* p = &plan->impl;
     SpecPlanImpl::WelchCfg* cfg = batched ? p->welch_batch_cfg : p->welch_cfg;
+    // batched, multitaper plan: mt_pgram's taper-row instance of MODE 0 / 1 is pinned too (MODE 2 / 3 have none: it selects)
+    const bool mt = batched && p->ntapers >= 1;
+    if (mt) p->welch_mt_cfg[0] = p->welch_mt_cfg[1] = SpecPlanImpl::WelchCfg{};
     if (mode < 0) {                                      // unpin: the next call selects as before
         cfg[0] = SpecPlanImpl::WelchCfg{};
         cfg[1] = SpecPlanImpl::WelchCfg{};
@@ -1945,7 +2099,11 @@ int dspb200_spec_plan_pin_welch(dspb200_spec_plan* plan, int batched, int mode, 
     return fused_dispatch(p, "Welch", [&](auto t, auto nn) {
         using T = decltype(t);
         constexpr int N = decltype(nn)::value;
-        if (batched) return p->cplx ? welch_pin<T, N, true, true>(p, mode, groups, vctas) : welch_pin<T, N, false, true>(p, mode, groups, vctas);
+        if (batched) {
+            DSP_TRY((p->cplx ? welch_pin<T, N, true, true>(p, mode, groups, vctas) : welch_pin<T, N, false, true>(p, mode, groups, vctas)));
+            if (!mt || mode >= 2) return (int)DSPB200_OK;
+            return p->cplx ? welch_pin<T, N, true, true, true>(p, mode, groups, vctas) : welch_pin<T, N, false, true, true>(p, mode, groups, vctas);
+        }
         return p->cplx ? welch_pin<T, N, true, false>(p, mode, groups, vctas) : welch_pin<T, N, false, false>(p, mode, groups, vctas);
     });
 }
@@ -1953,7 +2111,8 @@ int dspb200_spec_plan_pin_welch(dspb200_spec_plan* plan, int batched, int mode, 
 int dspb200_spec_plan_welch_config(const dspb200_spec_plan* plan, int batched, int aligned, int* mode, int* groups,
                                    int64_t* vctas) {
     DSP_REQUIRE(plan != nullptr, "plan is NULL");
-    const SpecPlanImpl::WelchCfg& c = (batched ? plan->impl.welch_batch_cfg : plan->impl.welch_cfg)[aligned ? 1 : 0];
+    const SpecPlanImpl::WelchCfg& c = (batched == 2 ? plan->impl.welch_mt_cfg : batched ? plan->impl.welch_batch_cfg
+                                                                                        : plan->impl.welch_cfg)[aligned ? 1 : 0];
     const bool ran = c.kern != nullptr && c.used > 0;
     if (mode) *mode = ran ? c.mode : -1;
     if (groups) *groups = ran ? c.g : 0;
@@ -2356,75 +2515,127 @@ int dspb200_welch_stream_power(dspb200_spec_plan* plan, const double* acc, int64
 
 // Multitaper (SURVEY.md 8f rank 1; src/multitaper.jl:117-242, 262-404).  The plan's window holds `ntapers` rows of n
 // samples, each PRE-SCALED by 1/sqrt(r_t) (r_t = fs * sum|w_t|^2 / weight_t, :135-139), so that
-//   mt_pgram       = sum_t fft2pow!(FFT(w_t .* s), 1)         (one Welch-style accumulation per taper into one spectrum)
-//   mt_spectrogram = sum_t spectrogram(s; window = w_t, r = 1) (one STFT launch per taper + an accumulate kernel)
-static int mt_pgram_check(dspb200_spec_plan* plan, const void* s, int64_t len, void* out) {
-    DSP_REQUIRE(plan && s && out, "NULL argument");
-    DSP_REQUIRE(plan->impl.ntapers >= 1, "not a multitaper plan");
-    DSP_REQUIRE(len == plan->impl.n, "Expected `signal` to be of length `config.n_samples`");    // DimensionMismatch :226
+//   mt_pgram       = sum_t fft2pow!(FFT(w_t .* s), 1)
+//   mt_spectrogram = sum_t spectrogram(s; window = w_t, r = 1)
+// of each of the nchan columns of a len x nchan matrix, every channel's tapers summed in taper order (the vector forms are
+// nchan = 1).  Fused sizes: mt_pgram is launch_mt_pgram (two launches per channel group), mt_spectrogram ONE launch of the
+// STFT kernels' taper-row instances (WIN == 2).  cuFFT sizes: mt_pgram_generic; mt_spectrogram is one batched STFT over all
+// channels per taper, each after the first followed by acc_add_kernel.
+static size_t mt_out_bytes(const SpecPlanImpl* p, int64_t nchan, int64_t k) {
+    return (size_t)(p->nout * k * nchan) * (p->f64 ? 8 : 4);
+}
+// The checks of every form, before any launch.  *k: columns per channel (mt_pgram: 1); *launch = false when there is nothing
+// to do (no channel, or no segment).
+static int mt_batch_check(const dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, const void* out, bool pgram,
+                          bool dev, int64_t* k, bool* launch) {
+    *launch = false;
+    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+    const SpecPlanImpl* p = &plan->impl;
+    DSP_REQUIRE(p->ntapers >= 1, "not a multitaper plan");
+    DSP_REQUIRE(len >= 0 && nchan >= 0, "negative size");
+    if (pgram) DSP_REQUIRE(len == p->n, "Expected `signal` to be of length `config.n_samples`");    // DimensionMismatch :226
+    *k = pgram ? 1 : nsegments(p, len);
+    if (nchan == 0 || *k == 0) return DSPB200_OK;
+    DSP_REQUIRE(s && out, "NULL argument");
+    // the kernels read every channel's samples while other CTAs write `out`
+    DSP_REQUIRE(!dev || !ranges_overlap(out, mt_out_bytes(p, nchan, *k), s, (size_t)(len * nchan) * dtype_size(p->dtype)),
+                "out overlaps s");
+    *launch = true;
     return DSPB200_OK;
 }
-int dspb200_mt_pgram_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t len, void* d_out, void* stream) {
-    DSP_RANGE("dspb200_mt_pgram_exec_dev");
-    DSP_TRY(mt_pgram_check(plan, d_s, len, d_out));
+
+static int mt_pgram_queue(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, void* out, cudaStream_t st) {
     SpecPlanImpl* p = &plan->impl;
-    DSP_CUDA(cudaSetDevice(p->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    auto queue = [&]() -> int {
-        DSP_TRY(welch_begin(p, st));
-        DSP_TRY(for_each_taper(p, [&](int64_t) { return welch_accumulate(p, d_s, 0, 0, 1, st); }));
-        return welch_finalize(p, 1.0, d_out, st);
-    };
-    return settle(st, queue());
-}
-int dspb200_mt_pgram_exec(dspb200_spec_plan* plan, const void* s, int64_t len, void* out) {
-    DSP_RANGE("dspb200_mt_pgram_exec");
-    DSP_TRY(mt_pgram_check(plan, s, len, out));
-    SpecPlanImpl* p = &plan->impl;
-    DSP_TRY(ensure_streams(p));
-    return run_staged(p->pipe.s_exec, {{s, (size_t)len * dtype_size(p->dtype), &p->pipe.in[0]}}, {{out, (size_t)p->nout * (p->f64 ? 8 : 4), &p->pipe.out[0]}},
-                      [&] { return dspb200_mt_pgram_exec_dev(plan, p->pipe.in[0].p, len, p->pipe.out[0].p, p->pipe.s_exec); });
+    if (p->fused)
+        return fused_dispatch(p, "Welch", [&](auto t, auto nn) {
+            using T = decltype(t);
+            constexpr int N = decltype(nn)::value;
+            return p->cplx ? launch_mt_pgram<T, N, true>(p, s, len, nchan, out, st) : launch_mt_pgram<T, N, false>(p, s, len, nchan, out, st);
+        });
+    return p->f64 ? mt_pgram_generic<double>(plan, s, len, nchan, out, st) : mt_pgram_generic<float>(plan, s, len, nchan, out, st);
 }
 
-int dspb200_mt_spectrogram_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t len, void* d_out, void* stream) {
-    DSP_RANGE("dspb200_mt_spectrogram_exec_dev");
-    DSP_REQUIRE(plan != nullptr, "plan is NULL");
+static int mt_spectrogram_queue(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, int64_t k, void* out,
+                                cudaStream_t st) {
     SpecPlanImpl* p = &plan->impl;
-    DSP_REQUIRE(p->ntapers >= 1, "not a multitaper plan");
-    DSP_CUDA(cudaSetDevice(p->device));
-    const int64_t k = nsegments(p, len);
-    if (k == 0) return DSPB200_OK;
-    DSP_REQUIRE(d_s && d_out, "NULL argument");
-    cudaStream_t st = (cudaStream_t)stream;
-    const size_t oel = p->f64 ? 8 : 4;
-    const int64_t cnt = p->nout * k;
-    auto taper = [&](int64_t t) -> int {
-        if (p->fused)                                    // tapers after the first add their PSD columns inside the emit step
-            return dspb200_stft_exec_dev(plan, d_s, len, 1, 1.0, t == 0 ? 1 : 3, d_out, st);
-        DSP_TRY(dspb200_stft_exec_dev(plan, d_s, len, 1, 1.0, 1, t == 0 ? d_out : p->tmp.p, st));
-        if (t > 0) {
-            const int threads = 256;
-            const int grid = (int)(cdiv(cnt, threads) < device_sm_count() * 32 ? cdiv(cnt, threads) : device_sm_count() * 32);
-            if (p->f64) acc_add_kernel<double><<<grid, threads, 0, st>>>((double*)d_out, (const double*)p->tmp.p, cnt);
-            else acc_add_kernel<float><<<grid, threads, 0, st>>>((float*)d_out, (const float*)p->tmp.p, cnt);
-            DSP_LAUNCH_OK();
-        }
+    if (p->fused) {
+        StftStreamArgs sa;                               // no history; columns k apart; every taper row in the one launch
+        sa.ldo = k;
+        sa.ntapers = (int)p->ntapers;
+        return stft_launch(p, sa, s, len, nchan, k, 1.0, 1, out, st);
+    }
+    const int64_t cnt = p->nout * k * nchan;
+    DSP_TRY(p->tmp.reserve((size_t)cnt * (p->f64 ? 8 : 4)));
+    return for_each_taper(p, [&](int64_t t) -> int {
+        DSP_TRY(dspb200_stft_exec_dev(plan, s, len, nchan, 1.0, 1, t == 0 ? out : p->tmp.p, st));
+        if (t == 0) return DSPB200_OK;
+        const int threads = 256;
+        const int grid = (int)(cdiv(cnt, threads) < device_sm_count() * 32 ? cdiv(cnt, threads) : device_sm_count() * 32);
+        if (p->f64) acc_add_kernel<double><<<grid, threads, 0, st>>>((double*)out, (const double*)p->tmp.p, cnt);
+        else acc_add_kernel<float><<<grid, threads, 0, st>>>((float*)out, (const float*)p->tmp.p, cnt);
+        DSP_LAUNCH_OK();
         return DSPB200_OK;
-    };
-    if (!p->fused) DSP_TRY(p->tmp.reserve((size_t)cnt * oel));
-    return settle(st, for_each_taper(p, taper));
+    });
+}
+
+int dspb200_mt_pgram_batch_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t len, int64_t nchan, void* d_out,
+                                    void* stream) {
+    DSP_RANGE("dspb200_mt_pgram_batch_exec_dev");
+    int64_t k = 0;
+    bool launch = false;
+    DSP_TRY(mt_batch_check(plan, d_s, len, nchan, d_out, true, true, &k, &launch));
+    if (!launch) return DSPB200_OK;
+    DSP_CUDA(cudaSetDevice(plan->impl.device));
+    cudaStream_t st = (cudaStream_t)stream;
+    return settle(st, mt_pgram_queue(plan, d_s, len, nchan, d_out, st));
+}
+int dspb200_mt_pgram_batch_exec(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, void* out) {
+    DSP_RANGE("dspb200_mt_pgram_batch_exec");
+    int64_t k = 0;
+    bool launch = false;
+    DSP_TRY(mt_batch_check(plan, s, len, nchan, out, true, false, &k, &launch));
+    if (!launch) return DSPB200_OK;
+    SpecPlanImpl* p = &plan->impl;
+    DSP_TRY(ensure_streams(p));
+    return run_staged(p->pipe.s_exec, {{s, (size_t)(len * nchan) * dtype_size(p->dtype), &p->pipe.in[0]}},
+                      {{out, mt_out_bytes(p, nchan, k), &p->pipe.out[0]}},
+                      [&] { return dspb200_mt_pgram_batch_exec_dev(plan, p->pipe.in[0].p, len, nchan, p->pipe.out[0].p, p->pipe.s_exec); });
+}
+int dspb200_mt_pgram_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t len, void* d_out, void* stream) {
+    return dspb200_mt_pgram_batch_exec_dev(plan, d_s, len, 1, d_out, stream);
+}
+int dspb200_mt_pgram_exec(dspb200_spec_plan* plan, const void* s, int64_t len, void* out) {
+    return dspb200_mt_pgram_batch_exec(plan, s, len, 1, out);
+}
+
+int dspb200_mt_spectrogram_batch_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t len, int64_t nchan, void* d_out,
+                                          void* stream) {
+    DSP_RANGE("dspb200_mt_spectrogram_batch_exec_dev");
+    int64_t k = 0;
+    bool launch = false;
+    DSP_TRY(mt_batch_check(plan, d_s, len, nchan, d_out, false, true, &k, &launch));
+    if (!launch) return DSPB200_OK;
+    DSP_CUDA(cudaSetDevice(plan->impl.device));
+    cudaStream_t st = (cudaStream_t)stream;
+    return settle(st, mt_spectrogram_queue(plan, d_s, len, nchan, k, d_out, st));
+}
+int dspb200_mt_spectrogram_batch_exec(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, void* out) {
+    DSP_RANGE("dspb200_mt_spectrogram_batch_exec");
+    int64_t k = 0;
+    bool launch = false;
+    DSP_TRY(mt_batch_check(plan, s, len, nchan, out, false, false, &k, &launch));
+    if (!launch) return DSPB200_OK;
+    SpecPlanImpl* p = &plan->impl;
+    DSP_TRY(ensure_streams(p));
+    return run_staged(p->pipe.s_exec, {{s, (size_t)(len * nchan) * dtype_size(p->dtype), &p->pipe.in[0]}},
+                      {{out, mt_out_bytes(p, nchan, k), &p->pipe.out[0]}},
+                      [&] { return dspb200_mt_spectrogram_batch_exec_dev(plan, p->pipe.in[0].p, len, nchan, p->pipe.out[0].p, p->pipe.s_exec); });
+}
+int dspb200_mt_spectrogram_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t len, void* d_out, void* stream) {
+    return dspb200_mt_spectrogram_batch_exec_dev(plan, d_s, len, 1, d_out, stream);
 }
 int dspb200_mt_spectrogram_exec(dspb200_spec_plan* plan, const void* s, int64_t len, void* out) {
-    DSP_RANGE("dspb200_mt_spectrogram_exec");
-    DSP_REQUIRE(plan != nullptr, "plan is NULL");
-    SpecPlanImpl* p = &plan->impl;
-    DSP_REQUIRE(p->ntapers >= 1, "not a multitaper plan");
-    const int64_t k = nsegments(p, len);
-    if (k == 0) return DSPB200_OK;
-    DSP_REQUIRE(s && out, "NULL argument");
-    DSP_TRY(ensure_streams(p));
-    return run_staged(p->pipe.s_exec, {{s, (size_t)len * dtype_size(p->dtype), &p->pipe.in[0]}}, {{out, (size_t)(p->nout * k) * (p->f64 ? 8 : 4), &p->pipe.out[0]}},
-                      [&] { return dspb200_mt_spectrogram_exec_dev(plan, p->pipe.in[0].p, len, p->pipe.out[0].p, p->pipe.s_exec); });
+    return dspb200_mt_spectrogram_batch_exec(plan, s, len, 1, out);
 }
 
 static int mt_cross_check(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int64_t f_lo, int64_t nf, void* out) {

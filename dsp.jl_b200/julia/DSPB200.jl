@@ -359,21 +359,46 @@ function spectrogram(s::Matrix{T}, n::Int=size(s, 1) >> 3, noverlap::Int=n >> 1;
     return out, (onesided ? DSP.rfftfreq(nfft, fs) : DSP.fftfreq(nfft, fs)), (n / 2 : n - noverlap : (k - 1) * (n - noverlap) + n / 2) / fs
 end
 
-# DSP.mt_pgram(s; fs, nfft, nw, ntapers, window): src/multitaper.jl:259-304 -- tapers / weights / validation from DSP.jl's own MTConfig
-function mt_pgram(s::Vector{T}; onesided::Bool=T <: Real, nfft::Int=nextpow(2, length(s)), fs::Real=1, nw::Real=4,
-                  ntapers::Int=ceil(Int, 2nw) - 1, window::Union{AbstractMatrix,Nothing}=nothing) where {T<:GPUNumber}
-    cfg = Periodograms.MTConfig{T}(length(s); fs, nfft, window, nw, ntapers, onesided)
-    tapers = permutedims(cfg.window ./ sqrt.(reshape(cfg.r, 1, :)))        # ntapers x n rows, pre-scaled by 1/sqrt(r_t)
+# A multitaper plan of DSP.jl's own MTConfig: the tapers pre-scaled by 1/sqrt(r_t), as ntapers x n rows
+function mt_plan(cfg, ::Type{T}, n, noverlap, nfft, onesided) where {T}
+    tapers = permutedims(cfg.window ./ sqrt.(reshape(cfg.r, 1, :)))
     h = Ref{Ptr{Cvoid}}(C_NULL)
     GC.@preserve tapers check(ccall((:dspb200_mt_plan_create, libdspb200), Cint,
         (Ref{Ptr{Cvoid}}, Cint, Int64, Int64, Int64, Cint, Ptr{Cdouble}, Int64),
-        h, dtype_code(T), length(s), 0, nfft, onesided, tapers, size(tapers, 1)))
-    plan = Plan(h[], :dspb200_spec_plan_destroy)
-    out = zeros(abs2type(T), length(cfg.freq))
-    GC.@preserve s out check(ccall((:dspb200_mt_pgram_exec, libdspb200), Cint,
-        (Ptr{Cvoid}, Ptr{Cvoid}, Int64, Ptr{Cvoid}), plan.ptr, s, length(s), out))
+        h, dtype_code(T), n, noverlap, nfft, onesided, tapers, size(tapers, 1)))
+    return Plan(h[], :dspb200_spec_plan_destroy)
+end
+
+# DSP.mt_pgram(s; fs, nfft, nw, ntapers, window): src/multitaper.jl:259-304 -- tapers / weights / validation from DSP.jl's own
+# MTConfig.  A matrix is the extension: every column a channel, power length(freq) x size(s, 2).
+function mt_pgram(s::VecOrMat{T}; onesided::Bool=T <: Real, nfft::Int=nextpow(2, size(s, 1)), fs::Real=1, nw::Real=4,
+                  ntapers::Int=ceil(Int, 2nw) - 1, window::Union{AbstractMatrix,Nothing}=nothing) where {T<:GPUNumber}
+    len, nchan = size(s, 1), size(s, 2)
+    cfg = Periodograms.MTConfig{T}(len; fs, nfft, window, nw, ntapers, onesided)
+    plan = mt_plan(cfg, T, len, 0, nfft, onesided)
+    out = zeros(abs2type(T), length(cfg.freq), nchan)
+    GC.@preserve s out check(ccall((:dspb200_mt_pgram_batch_exec, libdspb200), Cint,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Int64, Int64, Ptr{Cvoid}), plan.ptr, s, len, nchan, out))
     close!(plan)
-    return Periodograms.Periodogram(out, cfg.freq)
+    return Periodograms.Periodogram(s isa Vector ? vec(out) : out, cfg.freq)
+end
+
+# DSP.mt_spectrogram(s, n, noverlap; fs, onesided, kwargs...) for a matrix (the extension): src/multitaper.jl:262-404 per
+# column; power length(freq) x k x size(s, 2), the layout of the batched spectrogram
+function mt_spectrogram(s::Matrix{T}, n::Int, noverlap::Int; onesided::Bool=T <: Real, nfft::Int=nextpow(2, n), fs::Real=1,
+                        nw::Real=4, ntapers::Int=ceil(Int, 2nw) - 1, window::Union{AbstractMatrix,Nothing}=nothing) where {T<:GPUNumber}
+    len, nchan = size(s)
+    n > noverlap || throw(ArgumentError("Need `samples_per_window > n_overlap_samples`"))
+    cfg = Periodograms.MTConfig{T}(n; fs, nfft, window, nw, ntapers, onesided)
+    k = len >= n ? div(len - n, n - noverlap) + 1 : 0
+    out = zeros(abs2type(T), length(cfg.freq), k, nchan)
+    if k > 0 && nchan > 0
+        plan = mt_plan(cfg, T, n, noverlap, nfft, onesided)
+        GC.@preserve s out check(ccall((:dspb200_mt_spectrogram_batch_exec, libdspb200), Cint,
+            (Ptr{Cvoid}, Ptr{Cvoid}, Int64, Int64, Ptr{Cvoid}), plan.ptr, s, len, nchan, out))
+        close!(plan)
+    end
+    return out, cfg.freq, (n / 2 : n - noverlap : (k - 1) * (n - noverlap) + n / 2) / fs
 end
 
 # ------------------------------------------------------------------------------------------------ resample
@@ -562,6 +587,8 @@ function install_overlay!()
                 stft(s, n, noverlap, psdonly; kw...)
             DSP.resample(x::Vector{$T}, rate::Union{Integer,Rational}) = resample(x, rate)
             DSP.mt_pgram(s::Vector{$T}; kw...) = mt_pgram(s; kw...)
+            DSP.mt_pgram(s::Matrix{$T}; kw...) = mt_pgram(s; kw...)
+            DSP.mt_spectrogram(s::Matrix{$T}, n::Int, noverlap::Int; kw...) = mt_spectrogram(s, n, noverlap; kw...)
         end
     end
     for T in (Float32, Float64)

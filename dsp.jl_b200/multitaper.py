@@ -79,57 +79,69 @@ class MTConfig:
         self.plan = _lib.MtPlan(self.intype, n_samples, noverlap, nfft, onesided, scaled)
 
 
-def mt_pgram(s, config=None, onesided=None, nfft=None, fs=1, nw=4, ntapers=None, window=None):
-    """mt_pgram(s; onesided, nfft=nextfastfft(length(s)), fs, nw, ntapers, window) / mt_pgram(s, config),
-    src/multitaper.jl:178-242."""
+def _mt_signal(s):
+    """A vector or a len x nchan channel matrix (host array or DeviceArray): (s, device?, nchan or None for a vector)."""
     dev = isinstance(s, DeviceArray)
     if not dev:
         s = np.asarray(s)
-    if s.ndim != 1:
-        raise ArgumentError("expected a vector")
-    if config is None:
-        config = MTConfig(s.dtype, s.size, fs=fs, nfft=nextfastfft(s.size) if nfft is None else nfft, window=window, nw=nw,
-                          ntapers=ntapers, onesided=onesided)
-    if s.size != config.n_samples:
-        raise DimensionMismatch("Expected `signal` to be of length `config.n_samples`")
-    if dev:                                                        # device-resident signal: the spectrum stays in HBM
+    if s.ndim not in (1, 2):
+        raise ArgumentError("expected a vector or a len x nchan matrix")
+    return s, dev, (s.shape[1] if s.ndim == 2 else None)
+
+
+def _mt_run(s, dev, nchan, config, shape, run, run_dev):
+    """Run a multitaper plan over the columns of s (nchan None: a vector) into a result of `shape` + (nchan,)."""
+    shape = shape + ((nchan,) if nchan is not None else ())
+    nc = 1 if nchan is None else nchan
+    odt = fftabs2type(config.intype)
+    launch = all(shape)                                            # no channel or no segment: nothing to compute
+    length = s.shape[0]
+    if dev:                                                        # device-resident signal: the result stays in HBM
         if s.dtype != config.intype:
             raise ArgumentError(f"eltype of the device signal {s.dtype} does not match the config's {config.intype}")
-        dout = DeviceArray((config.plan.nout,), fftabs2type(config.intype))
-        config.plan.mt_pgram_dev(s.ptr, s.size, dout.ptr)
-        return Periodogram(dout, config.freq)
-    sig = np.ascontiguousarray(s, dtype=config.intype)
-    out = np.empty(config.plan.nout, dtype=fftabs2type(config.intype))
-    config.plan.mt_pgram(sig, out)
-    return Periodogram(out, config.freq)
+        dout = DeviceArray(shape, odt)
+        if launch:
+            run_dev(s.ptr, length, nc, dout.ptr)
+        return dout
+    out = np.zeros(shape, dtype=odt, order="F")
+    if launch:
+        run(np.asfortranarray(s.reshape(length, nc), dtype=config.intype), length, nc, out)
+    return out
+
+
+def mt_pgram(s, config=None, onesided=None, nfft=None, fs=1, nw=4, ntapers=None, window=None):
+    """mt_pgram(s; onesided, nfft=nextfastfft(length(s)), fs, nw, ntapers, window) / mt_pgram(s, config),
+    src/multitaper.jl:178-242.  A 2-D `s` (len x nchan) is the batched extension: every column is estimated with the same
+    configuration in one call, power is nout x nchan (a DeviceArray for device input) and the defaults come from
+    len = size(s, 1)."""
+    s, dev, nchan = _mt_signal(s)
+    length = s.shape[0]
+    if config is None:
+        config = MTConfig(s.dtype, length, fs=fs, nfft=nextfastfft(length) if nfft is None else nfft, window=window, nw=nw,
+                          ntapers=ntapers, onesided=onesided)
+    if length != config.n_samples:
+        raise DimensionMismatch("Expected `signal` to be of length `config.n_samples`")
+    plan = config.plan
+    power = _mt_run(s, dev, nchan, config, (plan.nout,), plan.mt_pgram_batch, plan.mt_pgram_batch_dev)
+    return Periodogram(power, config.freq)
 
 
 def mt_spectrogram(s, n=None, n_overlap=None, fs=1, onesided=None, nfft=None, nw=4, ntapers=None, window=None):
-    """mt_spectrogram(signal, n, n_overlap; fs, onesided, kwargs...), src/multitaper.jl:262-404 (default nfft = nextpow(2, n))."""
-    dev = isinstance(s, DeviceArray)
-    if not dev:
-        s = np.asarray(s)
-    if s.ndim != 1:
-        raise ArgumentError("expected a vector")
-    n = s.size >> 3 if n is None else int(n)
+    """mt_spectrogram(signal, n, n_overlap; fs, onesided, kwargs...), src/multitaper.jl:262-404 (default nfft = nextpow(2, n)).
+    A 2-D `s` (len x nchan) is the batched extension: power is nout x k x nchan, the layout of the batched spectrogram, and
+    freq and time come from len = size(s, 1)."""
+    s, dev, nchan = _mt_signal(s)
+    length = s.shape[0]
+    n = length >> 3 if n is None else int(n)
     n_overlap = n >> 1 if n_overlap is None else int(n_overlap)
     if n <= n_overlap:
         raise ArgumentError("Need `samples_per_window > n_overlap_samples`")
     config = MTConfig(s.dtype, n, fs=fs, nfft=nfft, window=window, nw=nw, ntapers=ntapers, onesided=onesided, noverlap=n_overlap)
-    k = arraysplit_count(s.size, n, n_overlap)
+    k = arraysplit_count(length, n, n_overlap)
     t = (n / 2 + (n - n_overlap) * np.arange(k, dtype=np.float64)) / fs
-    if dev:
-        if s.dtype != config.intype:
-            raise ArgumentError(f"eltype of the device signal {s.dtype} does not match the config's {config.intype}")
-        dout = DeviceArray((config.plan.nout, k), fftabs2type(config.intype))
-        if k > 0:
-            config.plan.mt_spectrogram_dev(s.ptr, s.size, dout.ptr)
-        return Spectrogram(dout, config.freq, t)
-    sig = np.ascontiguousarray(s, dtype=config.intype)
-    out = np.zeros((config.plan.nout, k), dtype=fftabs2type(config.intype), order="F")
-    if k > 0:
-        config.plan.mt_spectrogram(sig, out)
-    return Spectrogram(out, config.freq, t)
+    plan = config.plan
+    power = _mt_run(s, dev, nchan, config, (plan.nout, k), plan.mt_spectrogram_batch, plan.mt_spectrogram_batch_dev)
+    return Spectrogram(power, config.freq, t)
 
 
 def dpsseig(A, nw):

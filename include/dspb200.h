@@ -222,9 +222,12 @@ DSPB200_API int dspb200_welch_finalize_dev(dspb200_spec_plan* plan, double r, vo
  * the resident virtual-CTA count the channels are sliced for.  DSPB200_EUNSUPPORTED: not a fused plan, no such instance
  * for the plan's (dtype, nfft), or its shared memory exceeds the opt-in limit for the plan's n and hop.
  * DSPB200_EINVALID: vctas < 0 or not a multiple of groups, or more virtual CTAs than the plan has partial rows
- * (single-signal form).  Pinning does not change what is computed, only which instance and grid compute it. */
+ * (single-signal form).  On a multitaper plan, batched = 1 also pins the taper-row instance of that MODE 0 or 1 and G that
+ * dspb200_mt_pgram(_batch)_exec(_dev) runs at fused sizes (MODE 2 / 3 hold one window and have none: those calls then
+ * select their own).  Pinning does not change what is computed, only which instance and grid compute it. */
 DSPB200_API int dspb200_spec_plan_pin_welch(dspb200_spec_plan* plan, int batched, int mode, int groups, int64_t vctas);
-/* The configuration the last fused Welch call of the given form and alignment class (0 unaligned, 1 aligned) used:
+/* The configuration the last fused Welch call of the given form (batched = 2: the mt_pgram calls of a multitaper plan) and
+ * alignment class (0 unaligned, 1 aligned) used:
  * mode, groups and virtual CTAs of its launch.  *groups = 0 (mode -1, vctas 0) when no such call has run since the plan
  * was created or last pinned / unpinned. */
 DSPB200_API int dspb200_spec_plan_welch_config(const dspb200_spec_plan* plan, int batched, int aligned, int* mode, int* groups,
@@ -241,7 +244,7 @@ DSPB200_API int dspb200_filt_welch_exec(dspb200_os_plan* os, dspb200_spec_plan* 
  * scaled with r = fs*norm2 (:883,890); psd_only == 0: raw spectra (complex eltype), two-sided real input
  * completed by conjugate symmetry (:234-244).  nchan > 1 is the batched form of the per-vector reference
  * signature (SURVEY.md hard part 4).  psd_only == 3 (device form, fused sizes): the PSD columns are ADDED to the contents
- * of `out` -- how mt_spectrogram sums its tapers (src/multitaper.jl:362-377) without a separate pass. */
+ * of `out`. */
 DSPB200_API int dspb200_stft_exec(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, double r, int psd_only,
                       void* out);
 DSPB200_API int dspb200_stft_exec_dev(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, double r, int psd_only,
@@ -303,7 +306,8 @@ DSPB200_API int dspb200_periodogram2_exec_dev(int dtype, const void* d_s, int64_
 /* Multitaper (SURVEY.md 8f, "next" rank 1): mt_pgram / mt_spectrogram, src/multitaper.jl:117-242, 262-404.
  * `tapers` = ntapers rows of n Float64 samples, each pre-scaled by the host with 1/sqrt(r_t),
  * r_t = fs * sum|w_t|^2 / weight_t (:135-139); the library then sums fft2pow!(FFT(w_t .* segment), 1) over tapers.
- * mt_pgram: len must equal n (DimensionMismatch :226); out = nout values.  mt_spectrogram: out = nout x k. */
+ * mt_pgram: len must equal n (DimensionMismatch :226); out = nout values.  mt_spectrogram: out = nout x k.  These are the
+ * nchan = 1 case of the _batch forms below. */
 DSPB200_API int dspb200_mt_plan_create(dspb200_spec_plan** plan, int dtype, int64_t n, int64_t noverlap, int64_t nfft,
                            int onesided, const double* tapers_host, int64_t ntapers);
 DSPB200_API int dspb200_mt_pgram_exec(dspb200_spec_plan* plan, const void* s, int64_t len, void* out);
@@ -311,6 +315,26 @@ DSPB200_API int dspb200_mt_spectrogram_exec(dspb200_spec_plan* plan, const void*
 /* device pointers + cudaStream_t; return after the work on that stream has completed */
 DSPB200_API int dspb200_mt_pgram_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t len, void* d_out, void* stream);
 DSPB200_API int dspb200_mt_spectrogram_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t len, void* d_out, void* stream);
+/* Multitaper of many channels (an extension; the reference's mt_pgram / mt_spectrogram take one vector): `s` holds nchan
+ * columns of len samples (column-major), each estimated with the plan's tapers; column c's result is that of the vector call
+ * on it (fused sizes; the one exception: a Float32 nfft = 1024 mt_spectrogram of a matrix whose channels are not 16-byte
+ * aligned runs the block kernel, while an aligned vector runs the warp-per-unit kernel, which rounds differently).
+ * mt_pgram: len must equal n; out = nout x nchan.  mt_spectrogram: out = nchan matrices of nout x k (column-major,
+ * the layout of the batched spectrogram).  Every channel's tapers are summed in taper order.  nchan == 0, or k == 0,
+ * launches nothing and leaves out as it is.  DSPB200_EINVALID, before any launch: a NULL buffer, len != n (mt_pgram), a
+ * negative size, or (device form) out overlapping s.  Fused sizes: mt_pgram runs two launches per group of channels (the
+ * batched Welch kernel, one work item per channel whose units are its tapers, then the finalize kernel); mt_spectrogram one
+ * launch, which transforms every segment pair under every taper inside one CTA (warp, for Float32 nfft = 1024) and writes
+ * each PSD column once per taper.  cuFFT sizes: mt_pgram three launches per batch of (channel, taper) pairs plus one;
+ * mt_spectrogram one batched STFT over all channels per taper, plus one add per taper after the first.  The _dev forms take
+ * device pointers and a cudaStream_t and return after the work on that stream has completed; the host forms copy `s` in and
+ * `out` back. */
+DSPB200_API int dspb200_mt_pgram_batch_exec(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, void* out);
+DSPB200_API int dspb200_mt_pgram_batch_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t len, int64_t nchan, void* d_out,
+                                                void* stream);
+DSPB200_API int dspb200_mt_spectrogram_batch_exec(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, void* out);
+DSPB200_API int dspb200_mt_spectrogram_batch_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t len, int64_t nchan,
+                                                      void* d_out, void* stream);
 /* mt_cross_power_spectra! / mt_coherence!: src/multitaper.jl:553-616, 672-693, 722-790.  `signal` is the reference's
  * n_channels x n_samples matrix (column-major: channel index fastest), n_samples = the plan's n; the plan must be real and
  * one-sided (:411-416) with noverlap = 0.  demean != 0 subtracts the channel means (:566-570).  [f_lo, f_lo+nf) is the
