@@ -647,6 +647,8 @@ struct RsPlanImpl {
     size_t arb_occ_smem = 0;     // resident resample_arb_batch_kernel CTAs per SM for the last (smem, threads) launched
     int arb_occ_threads = 0, arb_per_sm = 0;
     bool arb_occ_hist = false;
+    bool arb_attr_set[2] = {false, false};  // resample_arb_batch_kernel<.., HIST> opted in to smem_optin bytes (plan's device)
+    int mp2_per_sm = 0;          // resident resample_mp2_kernel CTAs per SM at this plan's shared memory (0: not yet known)
     int64_t tpp8 = 0;
     size_t smem_optin = 0;
     DevBuf in, out;
@@ -750,14 +752,13 @@ static int rs_launch_mp2(RsPlanImpl* p, const RsArgs& a, cudaStream_t st, bool* 
     for (int ph = 0; ph < I; ++ph)
         for (int64_t r = 0; r < p->tpp8; ++r) taps.h[ph][r] = h8[(size_t)(ph * p->tpp8 + r)];
     auto kern = resample_mp2_kernel<EX, TR, EO, I, D, G>;
-    static int per_sm = 0;                                                         // per instantiation: resident CTAs per SM
-    if (per_sm == 0) {
+    if (p->mp2_per_sm == 0) {                                  // a plan runs one mp2 instantiation, at one smem
         DSP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 72 * 1024));
         int n = 0;
         DSP_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, M::NTH, smem));
-        per_sm = n < 1 ? 1 : n;
+        p->mp2_per_sm = n < 1 ? 1 : n;
     }
-    int64_t grid = (int64_t)device_sm_count() * per_sm;
+    int64_t grid = (int64_t)device_sm_count() * p->mp2_per_sm;
     if (grid > total) grid = total;
     kern<<<(unsigned)grid, M::NTH, smem, st>>>(
         (const EX*)a.x, a.x_begin, a.nx_local, a.x_col_stride, taps, (int)p->tpp, (int)(p->tpp8 / 8), a.n0, a.phi0,
@@ -876,10 +877,9 @@ static int rs_arb_launch(RsPlanImpl* p, const void* x, int64_t nx, int64_t ldx, 
     const RsArbTiling t = rs_arb_tiling(p->tpp, p->interp, delta, sizeof(EX), sizeof(TR));
     DSP_REQUIRE(t.smem <= p->smem_optin, "arbitrary-rate tile needs %zu bytes of shared memory", t.smem);
     auto kern = resample_arb_batch_kernel<EX, TR, EO, HIST>;
-    static bool attr_set = false;                                    // per instantiation
-    if (!attr_set) {
+    if (!p->arb_attr_set[HIST]) {
         DSP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_optin));
-        attr_set = true;
+        p->arb_attr_set[HIST] = true;
     }
     if (p->arb_occ_smem != t.smem || p->arb_occ_threads != t.threads || p->arb_occ_hist != HIST) {
         int n = 0;

@@ -16,7 +16,13 @@
  *                   out; synchronous on return.  Pinned host memory (dspb200_host_alloc) is streamed in
  *                   chunks so copies overlap compute.
  *  - `*_exec_dev` : DEVICE pointers; enqueued on `stream` (a cudaStream_t, NULL = default stream);
- *                   asynchronous.
+ *                   asynchronous: every launch and copy goes to `stream`, and the call returns without waiting for it.
+ *                   The plan-less _dev calls (conv_nd, conv_nd_os, hilbert, periodogram2) and the multitaper ones
+ *                   (mt_*) are the exception: they return after the work on that stream has completed.
+ *  - the asynchronous _dev calls may be captured in a CUDA graph (stream capture on `stream`) once a call with the same
+ *    plan, shapes and pointers has run outside the capture, which sizes the plan's scratch; the graph replays the call
+ *    with the arguments it was captured with.  dspb200_welch_begin_dev / _accumulate_dev / _finalize_dev keep host
+ *    state between calls, so the three are captured together, in one graph.
  *  - plans own device scratch, twiddle tables and cuFFT plans; one caller at a time per plan (the
  *    reference's WelchConfig / FIRFilter / ArraySplit scratch is equally non-reentrant:
  *    src/periodograms.jl:88-90,525-526; src/Filters/stream_filt.jl:137-142).
@@ -157,7 +163,8 @@ DSPB200_API int dspb200_conv_nd_exec_dev(int dtype, int rank, const int64_t* usi
  * save_blocksize = nffts - vsize + 1 outputs per dimension (:500-506).  Blocks are gathered (zero outside u), transformed
  * by ONE batched N-D cuFFT plan, multiplied by the filter spectrum and scattered, as many per batch as fit the block-buffer
  * budget (default 1 GiB; dspb200_conv_nd_os_set_budget) -- so arrays whose single transform would not fit are convolved
- * in bounded memory, which is what the reference's blocking is for. */
+ * in bounded memory, which is what the reference's blocking is for.  The _dev form takes device pointers and a cudaStream_t
+ * and returns after the work on that stream has completed. */
 DSPB200_API int dspb200_conv_nd_os_exec(int dtype, int rank, const int64_t* usize, const void* u, const int64_t* vsize, const void* v,
                                         const int64_t* nffts, void* out);
 DSPB200_API int dspb200_conv_nd_os_exec_dev(int dtype, int rank, const int64_t* usize, const void* d_u, const int64_t* vsize,
@@ -339,7 +346,8 @@ DSPB200_API int dspb200_mt_spectrogram_batch_exec_dev(dspb200_spec_plan* plan, c
  * n_channels x n_samples matrix (column-major: channel index fastest), n_samples = the plan's n; the plan must be real and
  * one-sided (:411-416) with noverlap = 0.  demean != 0 subtracts the channel means (:566-570).  [f_lo, f_lo+nf) is the
  * 0-based range of retained frequency bins (freq_range, :497-503).  coherence == 0: out = Complex[n_channels x n_channels
- * x nf] cross power spectra; != 0: out = real[n_channels x n_channels x nf] pairwise coherences. */
+ * x nf] cross power spectra; != 0: out = real[n_channels x n_channels x nf] pairwise coherences.  The _dev form takes
+ * device pointers and a cudaStream_t and returns after the work on that stream has completed. */
 DSPB200_API int dspb200_mt_cross_spectra_exec(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int demean,
                                               int64_t f_lo, int64_t nf, int coherence, void* out);
 DSPB200_API int dspb200_mt_cross_spectra_exec_dev(dspb200_spec_plan* plan, const void* d_signal, int64_t nchan, int demean,
