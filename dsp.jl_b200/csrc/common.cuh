@@ -74,6 +74,10 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line);
         }                                         \
     } while (0)
 
+// A global sample or output index of a range form inside the domain dspb200.h states (|v| <= DSPB200_INDEX_LIMIT): the
+// sum and difference of two such indices cannot overflow int64_t.
+static inline bool index_in_domain(int64_t v) { return v >= -DSPB200_INDEX_LIMIT && v <= DSPB200_INDEX_LIMIT; }
+
 // NVTX range around every C-ABI entry point that does device work (SURVEY.md section 5: the reference has no tracing; this
 // is what makes the library's calls visible on an Nsight timeline).  Header-only NVTX3: a no-op unless a tool is attached.
 struct NvtxRange {

@@ -1066,6 +1066,10 @@ int dspb200_os_exec_range_dev(dspb200_os_plan* plan, const void* u_local, int64_
     DSP_RANGE("dspb200_os_exec_range_dev");
     DSP_REQUIRE(plan != nullptr, "plan is NULL");
     DSP_REQUIRE(nu_local >= 0 && out_count >= 0 && out_begin >= 0, "bad range");
+    DSP_REQUIRE(index_in_domain(u_begin) && index_in_domain(nu_local) && index_in_domain(out_begin) &&
+                    index_in_domain(out_count) && index_in_domain(u_begin + nu_local) && index_in_domain(out_begin + out_count),
+                "range outside the index domain: u_begin %lld, nu_local %lld, out_begin %lld, out_count %lld (limit 2^61)",
+                (long long)u_begin, (long long)nu_local, (long long)out_begin, (long long)out_count);
     if (out_count == 0) return DSPB200_OK;
     DSP_REQUIRE(out_local != nullptr && (u_local != nullptr || nu_local == 0), "NULL argument");
     OsPlanImpl* p = &plan->impl;

@@ -1044,6 +1044,14 @@ int dspb200_resample_exec_range_dev(dspb200_resample_plan* plan, const void* x_l
     RsPlanImpl* p = &plan->impl;
     DSP_REQUIRE(nx_local >= 0 && nout_local >= 0 && j_begin >= 0, "bad range");
     DSP_REQUIRE(n0 >= 0 && phi0 >= 0 && phi0 < p->interp, "bad initial phase");
+    // in the order of the conditions every sum and product stays below 2^63: j_end * decim is bounded by division first
+    DSP_REQUIRE(index_in_domain(j_begin) && index_in_domain(nout_local) && index_in_domain(j_begin + nout_local) &&
+                    j_begin + nout_local <= (DSPB200_PHASE_LIMIT - phi0) / p->decim && index_in_domain(n0) &&
+                    index_in_domain(n0 + (phi0 + (j_begin + nout_local) * p->decim) / p->interp) && index_in_domain(x_begin) &&
+                    index_in_domain(nx_local) && index_in_domain(x_begin + nx_local),
+                "range outside the index domain: x_begin %lld, nx_local %lld, n0 %lld, j_begin %lld, nout_local %lld "
+                "(limits 2^61, phase 2^62)", (long long)x_begin, (long long)nx_local, (long long)n0, (long long)j_begin,
+                (long long)nout_local);
     if (nout_local == 0) return DSPB200_OK;
     DSP_REQUIRE(out_local != nullptr && (x_local != nullptr || nx_local == 0), "NULL argument");
     RsArgs a{x_local, x_begin, nx_local, 0, out_local, j_begin, nout_local, 0, n0, phi0, 1};

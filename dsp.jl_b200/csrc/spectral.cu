@@ -2029,6 +2029,19 @@ int64_t dspb200_spec_nsegments(const dspb200_spec_plan* plan, int64_t len) {
     return nsegments(&plan->impl, len);
 }
 
+// The index domain of the segment-range forms (dspb200.h): every sum and product below stays under 2^63 in this order
+static int welch_range_check(const SpecPlanImpl* p, int64_t len, int64_t sample_offset, int64_t seg_begin, int64_t seg_end) {
+    DSP_REQUIRE(seg_begin >= 0 && seg_end >= seg_begin, "bad segment range");
+    DSP_REQUIRE(len >= 0 && index_in_domain(len) && index_in_domain(sample_offset) && index_in_domain(sample_offset + len) &&
+                    (seg_end == seg_begin || seg_end - 1 <= (DSPB200_INDEX_LIMIT - p->n) / p->hop),
+                "segment range outside the index domain: len %lld, sample_offset %lld, segments [%lld, %lld) (limit 2^61)",
+                (long long)len, (long long)sample_offset, (long long)seg_begin, (long long)seg_end);
+    if (seg_end == seg_begin) return DSPB200_OK;
+    DSP_REQUIRE(seg_begin * p->hop >= sample_offset, "segment range starts before the local buffer");
+    DSP_REQUIRE((seg_end - 1) * p->hop + p->n <= sample_offset + len, "segment range runs past the local buffer");
+    return DSPB200_OK;
+}
+
 int dspb200_welch_exec_range_dev(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t sample_offset,
                                  int64_t seg_begin, int64_t seg_end, double r, void* out, void* stream) {
     DSP_RANGE("dspb200_welch_exec_range_dev");
@@ -2036,12 +2049,8 @@ int dspb200_welch_exec_range_dev(dspb200_spec_plan* plan, const void* s, int64_t
     DSP_REQUIRE(r != 0.0, "r must be nonzero");
     SpecPlanImpl* p = &plan->impl;
     cudaStream_t st = (cudaStream_t)stream;
-    DSP_REQUIRE(seg_begin >= 0 && seg_end >= seg_begin, "bad segment range");
-    if (seg_end > seg_begin) {
-        DSP_REQUIRE(s != nullptr, "s is NULL");
-        DSP_REQUIRE(seg_begin * p->hop >= sample_offset, "segment range starts before the local buffer");
-        DSP_REQUIRE((seg_end - 1) * p->hop + p->n <= sample_offset + len, "segment range runs past the local buffer");
-    }
+    DSP_TRY(welch_range_check(p, len, sample_offset, seg_begin, seg_end));
+    DSP_REQUIRE(seg_end == seg_begin || s != nullptr, "s is NULL");
     DSP_TRY(welch_begin(p, st));
     DSP_TRY(welch_accumulate(p, s, sample_offset, seg_begin, seg_end, st));
     return welch_finalize(p, r, out, st);
@@ -2060,11 +2069,9 @@ int dspb200_welch_accumulate_dev(dspb200_spec_plan* plan, const void* s, int64_t
     DSP_RANGE("dspb200_welch_accumulate_dev");
     DSP_REQUIRE(plan != nullptr, "plan is NULL");
     SpecPlanImpl* p = &plan->impl;
-    DSP_REQUIRE(seg_begin >= 0 && seg_end >= seg_begin, "bad segment range");
+    DSP_TRY(welch_range_check(p, len, sample_offset, seg_begin, seg_end));
     if (seg_end == seg_begin) return DSPB200_OK;
     DSP_REQUIRE(s != nullptr, "s is NULL");
-    DSP_REQUIRE(seg_begin * p->hop >= sample_offset, "segment range starts before the local buffer");
-    DSP_REQUIRE((seg_end - 1) * p->hop + p->n <= sample_offset + len, "segment range runs past the local buffer");
     return welch_accumulate(p, s, sample_offset, seg_begin, seg_end, (cudaStream_t)stream);
 }
 int dspb200_welch_finalize_dev(dspb200_spec_plan* plan, double r, void* out, void* stream) {

@@ -74,6 +74,16 @@ DSPB200_API int dspb200_stream_sync(void* stream);
 /* Number of kernels this library has launched in this process (bench.py's `gpu_launches`). */
 DSPB200_API int64_t dspb200_launch_count(void);
 
+/* Index domain of the range forms (dspb200_os_exec_range_dev, dspb200_resample_exec_range_dev,
+ * dspb200_welch_exec_range_dev, dspb200_welch_accumulate_dev).  Their offsets are global sample indices of one long
+ * stream, so they may be far larger than the buffers passed with them.  The kernels form differences of two such
+ * indices (the local position of a global sample) in int64_t, so every global index a call names must lie within
+ * +-DSPB200_INDEX_LIMIT, and the polyphase phase phi0 + j*decim within DSPB200_PHASE_LIMIT; then every sample, output and
+ * phase index the kernels compute stays representable in int64_t.  (Pointers formed from such an index to a sample that is
+ * not stored are never dereferenced.)  Calls outside return DSPB200_EINVALID before any launch. */
+#define DSPB200_INDEX_LIMIT ((int64_t)1 << 61)
+#define DSPB200_PHASE_LIMIT ((int64_t)1 << 62)
+
 /* ------------------------------------------------------------------------------------------ FIR, time domain
  * filt(b, 1, x) / filt!(out, b, 1, x) / tdfilt(h, x): src/dspbase.jl:14-15, 26-66, 95-154;
  * src/Filters/filt.jl:431-443.  y[i] = sum_k b[k] x[i-k+1] per column, evaluated with the reference's
@@ -119,7 +129,10 @@ DSPB200_API int dspb200_os_exec_dev(dspb200_os_plan* plan, const void* u, int64_
                         void* stream);
 /* Range form for sharding one long column across GPUs (SURVEY.md 8e): compute outputs
  * [out_begin, out_begin+out_count) of the convolution of the virtual signal whose samples
- * [u_begin, u_begin+nu_local) are stored at `u_local` (everything outside is zero).  No collective. */
+ * [u_begin, u_begin+nu_local) are stored at `u_local` (everything outside is zero).  No collective.
+ * Domain (DSPB200_INDEX_LIMIT = 2^61): 0 <= out_begin, 0 <= out_count, 0 <= nu_local, |u_begin| <= 2^61,
+ * out_begin + out_count <= 2^61 and u_begin + nu_local <= 2^61; otherwise DSPB200_EINVALID before any launch.
+ * Outputs that no stored sample reaches are transformed like the others: they are zero, of either sign. */
 DSPB200_API int dspb200_os_exec_range_dev(dspb200_os_plan* plan, const void* u_local, int64_t u_begin, int64_t nu_local,
                               void* out_local, int64_t out_begin, int64_t out_count, void* stream);
 /* Stateful overlap-save: fftfilt(f::DF2TFilter, x) / fftfilt!(out, f::DF2TFilter, x), the overlap-save counterpart of
@@ -208,7 +221,10 @@ DSPB200_API int dspb200_welch_batch_exec(dspb200_spec_plan* plan, const void* s,
 DSPB200_API int dspb200_welch_batch_exec_dev(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, double r,
                                              void* out, void* stream);
 /* Segment-range form for multi-GPU sharding: accumulates only segments [seg_begin, seg_end) of the signal
- * whose sample `sample_offset` is s[0]; the caller sums the partial spectra (NCCL all-reduce, SURVEY.md 8e). */
+ * whose sample `sample_offset` is s[0]; the caller sums the partial spectra (NCCL all-reduce, SURVEY.md 8e).
+ * Domain (also of dspb200_welch_accumulate_dev; DSPB200_INDEX_LIMIT = 2^61): 0 <= len, |sample_offset| <= 2^61,
+ * sample_offset + len <= 2^61, 0 <= seg_begin <= seg_end and, for a non-empty range, (seg_end - 1) * hop + n <= 2^61;
+ * otherwise DSPB200_EINVALID before any launch. */
 DSPB200_API int dspb200_welch_exec_range_dev(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t sample_offset,
                                  int64_t seg_begin, int64_t seg_end, double r, void* out, void* stream);
 
@@ -370,7 +386,11 @@ DSPB200_API int dspb200_resample_exec(dspb200_resample_plan* plan, const void* x
 DSPB200_API int dspb200_resample_exec_dev(dspb200_resample_plan* plan, const void* x, int64_t nx, int64_t ncols, int64_t n0,
                               int64_t phi0, void* out, int64_t nout, void* stream);
 /* Range form: outputs [j_begin, j_begin+nout_local) of the virtual input whose samples
- * [x_begin, x_begin+nx_local) are stored at x_local (zero elsewhere). */
+ * [x_begin, x_begin+nx_local) are stored at x_local (zero elsewhere).
+ * Domain (DSPB200_INDEX_LIMIT = 2^61, DSPB200_PHASE_LIMIT = 2^62), with j_end = j_begin + nout_local:
+ * 0 <= j_begin, 0 <= nout_local, j_end <= 2^61, phi0 + j_end * decim <= 2^62, 0 <= n0 and the newest input sample
+ * n0 + (phi0 + j_end * decim) / interp <= 2^61, 0 <= nx_local, |x_begin| <= 2^61 and x_begin + nx_local <= 2^61;
+ * otherwise DSPB200_EINVALID before any launch. */
 DSPB200_API int dspb200_resample_exec_range_dev(dspb200_resample_plan* plan, const void* x_local, int64_t x_begin,
                                     int64_t nx_local, int64_t n0, int64_t phi0, void* out_local, int64_t j_begin,
                                     int64_t nout_local, void* stream);
