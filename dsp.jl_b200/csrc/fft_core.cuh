@@ -21,7 +21,8 @@
 
 // timing probes (wrong results, never in the shipped library): bit 0 skips the stride-256 passes, bit 1 replaces the
 // first-pass global loads by constants (and turns the overlap-save kernels' TMA staging off: no input is read at all),
-// bit 2 the H loads, bit 3 drops the global stores, bit 4 skips the stride-16 passes
+// bit 2 the H loads, bit 3 drops the global stores, bit 4 skips the stride-16 passes (the 32 · 32 · 16 plan: its stride-32
+// passes)
 #ifndef DSP_PROBE
 #define DSP_PROBE 0
 #endif
@@ -604,6 +605,106 @@ __device__ __forceinline__ void fft_forward(const FftCtx<T>& c, int tid, Ld0 ld0
     }
 }
 
+// ---------------------------------------------------------------------------------------------- 32 · 32 · 16 plan
+// The 16384-point Float32 overlap-save kernels run their transforms in three passes instead of the four of
+// fft_plan_traits<16384> (16 · 16 · 16 · 4), with the same DIT / FMA butterflies:
+//   first pass  plain 32-point DFTs of the residue classes x[c + 512 m], c < 512, written as 32 contiguous slots at block
+//               fft_r32_block_of(c) = 32 (c mod 16) + c / 16;
+//   middle      one twiddled radix-32 pass at stride 32 (sub-transforms of M = 1024 points, w = W_1024^t, t < 32), in place;
+//   last pass   radix 16 at stride 1024 (w = W_16384^t, t < 1024); it leaves X[t + 1024 s], s < 16, natural order, in the
+//               registers of the thread that owns t.
+// A thread of the 512-thread CTA runs one radix-32 butterfly per first / middle pass and the radix-16 butterflies t and
+// t + 512 of the last pass: together those hold X[t + 512 m], m < 32 -- exactly the residue class t of the next first
+// pass, so the overlap-save bracket [last, x H, swap, first] stays in registers.  Each pass reads and writes the data
+// buffer once: 10 sweeps of it per overlap-save unit (TMA staging write included) instead of 14, in five barrier-separated
+// phases instead of seven.
+struct fft_r32 {
+    static constexpr int N = 16384;
+    static constexpr int NT = 512;                 // threads: one radix-32 butterfly each, two radix-16 ones in the last pass
+    static constexpr int Q = N / 32;               // radix-32 butterflies per pass = first-pass residue classes
+    static constexpr int QL = N / 16;              // last-pass butterflies = its stride
+    static constexpr int T32_LEN = 32 * 16;        // radix-32 pass: rows t < 32 of 16 tabulated omegas (fft_tw_count<32>)
+    static constexpr int TL_LEN = 2 * QL;          // last pass: (W_N^4t, W_N^t), t < 1024; the other six omegas are formed
+    static constexpr int TABLE_LEN = T32_LEN + TL_LEN;
+    // Padded slot address p + C10 (p >> 10).  The radix-32 and last-pass lanes read runs of consecutive slots inside one
+    // 1024-slot group, and each 32-slot first-pass run stays 16-byte aligned (C10 even).  The scattered first-pass stores
+    // -- lanes c .. c+7 of a quarter warp write the runs of blocks 32 (c mod 16) + c / 16, 1024 slots apart -- fall on
+    // eight different 16-byte bank groups when 1024 + C10 slots are an odd number of them (smallest C10 of the exhaustive
+    // search in tests/host/fft_r32_host_check.cu, which audits every pass: one wavefront per half / quarter warp).
+    static constexpr int C10 = 2;
+    static constexpr int PADDED_LEN = ((N - 1) + C10 * ((N - 1) >> 10) + 1 + 3) & ~3;
+    static constexpr int SMEM_ELEMS = PADDED_LEN + TABLE_LEN;          // data buffer + tables, Float32 complex elements
+};
+__host__ __device__ __forceinline__ constexpr int fft_r32_padaddr(int p) { return p + fft_r32::C10 * (p >> 10); }
+__host__ __device__ __forceinline__ constexpr int fft_r32_block_of(int c) { return 32 * (c & 15) + (c >> 4); }
+
+template <typename T> struct FftR32Ctx {
+    cx<T>* sm;                      // padded data buffer, fft_r32::PADDED_LEN elements
+    const cx<T>* t32;               // shared: radix-32 pass table (pair-major, fft_tw_index)
+    const cx<T>* tl;                // shared: (W_N^4t, W_N^t), t < 1024: one 16-byte word per row
+};
+// Copy the tables (fft_r32_fill_tables: T32_LEN + TL_LEN elements at g) into shared memory at `tabs`.  Must be followed by a
+// barrier over all NT threads before the middle pass.
+template <typename T>
+__device__ __forceinline__ FftR32Ctx<T> fft_r32_make_ctx(cx<T>* data, cx<T>* tabs, const cx<T>* __restrict__ g, int tid) {
+    for (int i = tid; i < fft_r32::TABLE_LEN; i += fft_r32::NT) tabs[i] = g[i];
+    return FftR32Ctx<T>{data, tabs, tabs + fft_r32::T32_LEN};
+}
+
+// plain 32-point butterfly of residue class c (v[m] = x[c + 512 m]) and its store: 32 contiguous slots at block rho(c)
+template <typename T> __host__ __device__ __forceinline__ void fft_r32_first_bfly(cx<T> (&v)[32]) { fft_bfly<T, 32, true>(v, nullptr); }
+template <typename T> __host__ __device__ __forceinline__ void fft_r32_store_block(cx<T>* sm, int c, const cx<T> (&v)[32]) {
+    cx<T>* p = sm + fft_r32_padaddr(32 * fft_r32_block_of(c));
+#pragma unroll
+    for (int r = 0; r < 32; r += 2) sts2<T>(p + r, v[r], v[r + 1]);
+}
+
+// The twiddled radix-32 pass at stride 32, in place: butterfly tid of group tid / 32 (GATE: load gating, after a CTA-wide
+// barrier only, as fft_pass16)
+template <typename T, bool GATE = false> __host__ __device__ __forceinline__ void fft_r32_middle(const FftR32Ctx<T>& c, int tid) {
+    const int t = tid & 31;
+    cx<T>* p = c.sm + fft_r32_padaddr((tid >> 5) * 1024 + t);      // the 32 operands are 32 slots apart, no padding between
+    cx<T> v[32], w[16];
+    if constexpr (GATE) fft_gate_wait<fft_r32::NT>(tid);
+#pragma unroll
+    for (int i = 0; i < 16; i += 2) lds2<T>(c.t32 + fft_tw_index<T>(i, t, 32), w[i], w[i + 1]);
+#pragma unroll
+    for (int r = 0; r < 32; ++r) v[r] = p[32 * r];
+    if constexpr (GATE) fft_gate_open<fft_r32::NT>(tid);
+    fft_bfly<T, 32, false>(v, w);
+#pragma unroll
+    for (int r = 0; r < 32; ++r) p[32 * r] = v[r];
+}
+
+// Last pass of butterfly t < 1024 in two halves, so that a caller can hand the data buffer on between them: the load
+// reads its 16 operands (slots t + 1024 s), the butterfly leaves v[s] = X[t + 1024 s].  Its omegas (w^8, w^4, w^2, W8 w^2,
+// w, W16 w, W8 w, W16^3 w; fft_bfly's order) come from the tabulated w = W_N^t and w^4: two squarings and four constant
+// products.  (w^4 by squaring as well -- w alone, 8 KB -- put the forward transform's relative error at 2.4e-7 and the
+// overlap-save pipeline's at 3.5e-7 in tests/host/fft_r32_host_check.cu, against 1.6e-7 and 2.4e-7 with w^4 tabulated.)
+template <typename T> __host__ __device__ __forceinline__ void fft_r32_last_load(const FftR32Ctx<T>& c, int t, cx<T> (&v)[16]) {
+    const cx<T>* p = c.sm + fft_r32_padaddr(t);
+#pragma unroll
+    for (int s = 0; s < 16; ++s) v[s] = p[fft_r32_padaddr(s * 1024)];
+}
+template <typename T> __host__ __device__ __forceinline__ cx<T> fft_sq(cx<T> a) {
+    return mkc<T>(fma_(a.x, a.x, -(a.y * a.y)), (a.x + a.x) * a.y);
+}
+template <typename T> __host__ __device__ __forceinline__ cx<T> fft_mul_const(cx<T> a, T cr, T ci) {    // a (cr + i ci)
+    return mkc<T>(fma_(a.x, cr, -(a.y * ci)), fma_(a.x, ci, a.y * cr));
+}
+template <typename T> __host__ __device__ __forceinline__ void fft_r32_last_bfly(const FftR32Ctx<T>& c, int t, cx<T> (&v)[16]) {
+    const T c16 = fft_const<T>::C8, s16 = fft_const<T>::S8;                        // W16 = c16 - i s16, W16^3 = s16 - i c16
+    cx<T> w[8];
+    lds2<T>(c.tl + 2 * t, w[1], w[4]);
+    w[2] = fft_sq(w[4]);
+    w[0] = fft_sq(w[1]);
+    w[3] = mul_w8<T>(w[2]);
+    w[5] = fft_mul_const<T>(w[4], c16, -s16);
+    w[6] = mul_w8<T>(w[4]);
+    w[7] = fft_mul_const<T>(w[4], s16, -c16);
+    fft_bfly<T, 16, false>(v, w);
+}
+
 // ---------------------------------------------------------------------------------------------- host side
 // omega(k, m) rows for w = exp(-2 pi i * num / den), radix R: long-double trig, rounded once
 template <typename T> inline void fft_fill_row(cx<T>* row, int R, long long num, long long den, int limit = 1 << 30) {
@@ -660,6 +761,22 @@ template <typename T> inline void fft_fill_tl(cx<T>* tl, long long n) {
         } else {
             fft_fill_row<T>(tl + t * tlk, rl, t, n);
         }
+    }
+}
+
+// tables of the 32 · 32 · 16 plan (fft_r32::TABLE_LEN elements): the radix-32 rows for w = W_1024^t, t < 32, pair-major,
+// then the last-pass rows (W_16384^4t, W_16384^t), t < 1024
+template <typename T> inline void fft_r32_fill_tables(cx<T>* tab) {
+    cx<T> row[16];
+    for (int t = 0; t < 32; ++t) {
+        fft_fill_row<T>(row, 32, t, 1024);
+        for (int i = 0; i < 16; ++i) tab[fft_tw_index<T>(i, t, 32)] = row[i];
+    }
+    const long double PI2 = 6.283185307179586476925286766559005768L;
+    for (int t = 0; t < fft_r32::QL; ++t) {
+        const long double a = -PI2 * (long double)t / (long double)fft_r32::N;
+        tab[fft_r32::T32_LEN + 2 * t] = mkc<T>((T)cosl(4 * a), (T)sinl(4 * a));
+        tab[fft_r32::T32_LEN + 2 * t + 1] = mkc<T>((T)cosl(a), (T)sinl(a));
     }
 }
 

@@ -15,6 +15,7 @@
 #include <math.h>
 #include <stdlib.h>
 #include <new>
+#include <vector>
 
 namespace dspb200 {
 
@@ -27,6 +28,7 @@ struct OsPlanImpl {
     void* d_tw = nullptr;   // fused: last-pass twiddle table (fft_fill_tl)
     void* d_t16 = nullptr;  // fused: radix-16 twiddle tables
     void* d_t256 = nullptr;
+    void* d_r32 = nullptr;  // fused 16384-point Float32: tables of the 32 · 32 · 16 plan (fft_r32_fill_tables)
     int sm_count = 0;               // device_sm_count() at plan creation
     int fused_per_sm = 0;   // resident CTAs per SM of this plan's fused kernel (occupancy calculator, asked once)
     int fused_state_per_sm = 0;     // the same for its stateful instance
@@ -53,9 +55,9 @@ template <typename T> struct os_elt<T, true> { using type = cx<T>; };
 // [last forward pass -> x H -> swap -> first pass of the second transform] in registers | middle passes | last pass ->
 // global stores (thread t writes y[t + r N/16]: coalesced).  H is in natural order (the forward transform ends in
 // natural order), pre-scaled by 1/N; thread t reads H[t + r N/16]: coalesced, no tiling needed.
-// The 16384-point Float32 kernels (os_threads::staged) read an interior unit's input from shared memory instead: two TMA
-// bulk copies, issued during the previous unit, put the span in natural order in front of and at the head of the data
-// buffer (OsStage).
+// The 16384-point Float32 kernels (os_threads::staged) run the 32 · 32 · 16 plan instead (os_unit_r32: first | radix-32 |
+// [last, x H, swap, first] | radix-32 | last), and read an interior unit's input from shared memory: two TMA bulk copies,
+// issued during the previous unit, put the span in natural order in front of and at the head of the data buffer (OsStage).
 // Probes of that kernel's per-unit transfers (2^26 ComplexF32 samples, 4097 taps, H100 SXM 80 GB at 700 W, before staging):
 // conv 0.660 .. 0.667 ms; without the input loads 0.607 .. 0.614, without the H loads 0.628 .. 0.637, without the output
 // stores 0.543 .. 0.546.
@@ -69,7 +71,11 @@ template <typename T> struct os_elt<T, true> { using type = cx<T>; };
 //  * complex N = 16384 (one CTA per SM: its shared memory holds one block): 512 threads, 128 registers, two butterflies in
 //    flight: on the H100 it is faster than 1024 threads with one butterfly each under a 64-register cap, the earlier
 //    generation's choice (2^26 samples, 4097 taps, H100 80 GB HBM3 at 400 W, alternating: conv 0.695 .. 0.704 against
-//    0.795 .. 0.801 ms).  Splitting the block over a two-CTA cluster so that two 512-thread, 64-register CTAs share each
+//    0.795 .. 0.801 ms).  Its transform runs as 32 · 32 · 16 (fft_r32): one radix-32 butterfly per thread in the first and
+//    middle passes, two radix-16 ones in the last, no spills; against 16 · 16 · 16 · 4 at the same shape (2^26 samples,
+//    4097 taps, H100 80GB HBM3 at 700 W, alternating): conv 0.543 .. 0.548 against 0.589 .. 0.595 ms, and the real
+//    one-shot fftfilt of 64 x 2^20 Float32 with 4097 taps 0.380 .. 0.383 against 0.395 .. 0.399 ms.  Splitting the block
+//    over a two-CTA cluster so that two 512-thread, 64-register CTAs share each
 //    SM does not pay there either: a 512-thread, 64-register 8192-point
 //    kernel at two CTAs per SM costs 0.43 of a 16384-point unit per unit (0.46 with the store count of half a
 //    16384-point block; transform length alone gives 0.46 .. 0.5), which leaves no room for the exchange.  Its next unit's
@@ -96,10 +102,14 @@ template <typename T, int N, bool CPLX> struct os_threads {
 constexpr int OS_STAGE_HEAD = 32768;
 static_assert(OS_STAGE_HEAD % 16 == 0, "TMA copies move multiples of 16 bytes");
 static_assert(OS_STAGE_HEAD < 16384 * 4, "the head region holds less than the shortest staged span (N + 1 floats)");
+// data buffer and twiddle tables of the fused kernel, in elements of cx<T>: the staged kernels run the 32 · 32 · 16 plan
+template <typename T, int N, bool CPLX> __host__ __device__ constexpr int os_fft_elems() {
+    return os_threads<T, N, CPLX>::staged ? fft_r32::SMEM_ELEMS : fft_smem_elems<T, N>();
+}
 // dynamic shared memory of the fused kernel: (staged kernels) head region, data buffer and twiddle tables, then (staged
 // kernels) the copies' mbarrier
 template <typename T, int N, bool CPLX> constexpr size_t os_smem_bytes() {
-    return (size_t)fft_smem_elems<T, N>() * sizeof(cx<T>) + (os_threads<T, N, CPLX>::staged ? OS_STAGE_HEAD + 16 : 0);
+    return (size_t)os_fft_elems<T, N, CPLX>() * sizeof(cx<T>) + (os_threads<T, N, CPLX>::staged ? OS_STAGE_HEAD + 16 : 0);
 }
 
 template <typename T> __device__ __forceinline__ cx<T> ldg_cx(const cx<T>* __restrict__ p) {
@@ -188,48 +198,48 @@ struct OsStage {
     uint32_t parity;     // phase of the next wait
 };
 
-// One unit.  staged: its input span is (being) copied to OsStage::head; next_u: slot 0 of the next unit when that one
-// is to be staged (os_fused_kernel decides), else null.  Both only in staged kernels.  STATE: only the edge units' stores
-// change (os_put_state, with the OsUnitState that state_geometry() returns).
+// Output of slot j of a unit (y: swapped domain, result = (y.y, y.x)).  STATE: only the edge units' stores change
+// (os_put_state, with the OsUnitState that state_geometry() returns).
+template <typename T, bool CPLX, bool INTERIOR, bool STATE, typename SGeom>
+__device__ __forceinline__ void os_put(const OsUnit<typename os_elt<T, CPLX>::type>& g, const SGeom& sg, int j, cx<T> y) {
+#if DSP_PROBE & 8
+    if (y.x != T(123456.75)) return;
+#endif
+    if (j < g.nvm1) return;
+    if constexpr (CPLX) {
+        if constexpr (INTERIOR) g.out[j] = mkc<T>(y.y, y.x);
+        else if constexpr (STATE) { if (j < g.jend) os_put_state(g, sg, j, mkc<T>(y.y, y.x)); }
+        else if (j < g.jend) g.out[j] = (j < g.jzero) ? mkc<T>(y.y, y.x) : mkc<T>(T(0), T(0));
+    } else {
+        const int jb = j + g.L;
+        if constexpr (INTERIOR) {
+            g.out[j] = y.y;
+            g.out[jb] = y.x;
+        } else if constexpr (STATE) {
+            if (j < g.jend) os_put_state(g, sg, j, y.y);
+            if (jb < g.jend) os_put_state(g, sg, jb, y.x);
+        } else {
+            if (j < g.jend) g.out[j] = (j < g.jzero) ? y.y : T(0);
+            if (jb < g.jend) g.out[jb] = (jb < g.jzero) ? y.x : T(0);
+        }
+    }
+}
+template <typename E, bool STATE, bool INTERIOR> using os_sgeom_t = std::conditional_t<STATE && !INTERIOR, OsUnitState<E>, OsNoState>;
+
+// One unit of the kernels that are not staged (fft_plan_traits<N>).
 template <typename T, int N, bool CPLX, int NT, bool INTERIOR, int ITERS, bool STATE, typename SG>
 __device__ __forceinline__ void os_unit(const FftCtx<T>& ctx, int tid, const OsUnit<typename os_elt<T, CPLX>::type>& g,
-                                        const cx<T>* __restrict__ H, OsStage& st, bool staged,
-                                        const typename os_elt<T, CPLX>::type* __restrict__ next_u, const SG& state_geometry) {
+                                        const cx<T>* __restrict__ H, const SG& state_geometry) {
     using E = typename os_elt<T, CPLX>::type;
     constexpr int Q = fft_plan_traits<N>::Q;
-    constexpr bool STAGED = os_threads<T, N, CPLX>::staged;
     static_assert(ITERS == (Q + NT - 1) / NT, "register tile does not match the thread count");
-    static_assert(!STAGED || (ITERS == 2 && Q % NT == 0), "TMA staging is laid out for two butterflies per thread");
-    if (STAGED && INTERIOR && staged) {
-        // the span in natural order from st.head (head region, then the data buffer): every thread reads all of its samples
-        // into registers (lanes read consecutive words), the barrier inside fft_first_pass_regs then orders all reads
-        // before the padded stores that overwrite the data buffer's part
-        mbar_wait(st.bar, st.parity);
-        st.parity ^= 1;
-        const E* s = reinterpret_cast<const E*>(st.head);
-        cx<T> v[ITERS][16];
-#pragma unroll
-        for (int it = 0; it < ITERS; ++it)
-#pragma unroll
-            for (int r = 0; r < 16; ++r) {
-                const int j = tid + it * NT + r * Q;
-                if constexpr (CPLX) v[it][r] = s[j];
-                else v[it][r] = mkc<T>(s[j], s[j + g.L]);
-            }
-        fft_first_pass_regs<T, N, NT, true>(ctx, tid, v);
-    } else {
+    {
         // global loads; the barrier inside (between the first butterfly and its stores) also ends the previous unit's last
         // pass
         auto ld0 = [&](int j, int, int) -> cx<T> { return os_sample<T, CPLX, INTERIOR>(g, j); };
         fft_first_pass<T, N, NT, true>(ctx, tid, ld0);
     }
     __syncthreads();
-    if (STAGED && next_u != nullptr && tid == 0) {
-        // the head region has been read: the next unit's head goes there now, its phase completes with the rest
-        fence_proxy_async_shared();
-        mbar_expect_tx_noarrive(st.bar, OS_STAGE_HEAD);
-        tma_load_1d(st.head, next_u, OS_STAGE_HEAD, st.bar);
-    }
     fft_middle<T, N, NT>(ctx, tid);
     // last forward pass, x H, swap, first pass of the second transform -- in registers
     cx<T> v[ITERS][16];
@@ -256,77 +266,119 @@ __device__ __forceinline__ void os_unit(const FftCtx<T>& ctx, int tid, const OsU
     __syncthreads();
     fft_middle<T, N, NT>(ctx, tid);
     constexpr int RL = fft_plan_traits<N>::RL, NBF = 16 / RL;
-    using SGeom = std::conditional_t<STATE && !INTERIOR, OsUnitState<E>, OsNoState>;
-    SGeom sg{};
+    os_sgeom_t<E, STATE, INTERIOR> sg{};
     if constexpr (STATE && !INTERIOR) sg = state_geometry();
-    // output of slot j (y: swapped domain, result = (y.y, y.x))
-    auto put = [&](int j, cx<T> y) {
-#if DSP_PROBE & 8
-        if (y.x != T(123456.75)) return;
-#endif
-        if (j < g.nvm1) return;
-        if constexpr (CPLX) {
-            if constexpr (INTERIOR) g.out[j] = mkc<T>(y.y, y.x);
-            else if constexpr (STATE) { if (j < g.jend) os_put_state(g, sg, j, mkc<T>(y.y, y.x)); }
-            else if (j < g.jend) g.out[j] = (j < g.jzero) ? mkc<T>(y.y, y.x) : mkc<T>(T(0), T(0));
-        } else {
-            const int jb = j + g.L;
-            if constexpr (INTERIOR) {
-                g.out[j] = y.y;
-                g.out[jb] = y.x;
-            } else if constexpr (STATE) {
-                if (j < g.jend) os_put_state(g, sg, j, y.y);
-                if (jb < g.jend) os_put_state(g, sg, jb, y.x);
-            } else {
-                if (j < g.jend) g.out[j] = (j < g.jzero) ? y.y : T(0);
-                if (jb < g.jend) g.out[jb] = (jb < g.jzero) ? y.x : T(0);
-            }
-        }
+    // last pass, streamed one radix-RL butterfly at a time -- RL live values instead of 16
+    auto chunk = [&](auto a_, int tp) {
+        constexpr int A = decltype(a_)::value;
+        cx<T> u[RL];
+        fft_last_pass_chunk<T, N, A>(ctx, tp, u);
+#pragma unroll
+        for (int jj = 0; jj < RL; ++jj) os_put<T, CPLX, INTERIOR, STATE>(g, sg, tp + (A + NBF * jj) * Q, u[jj]);
     };
-    // Last pass.  Staged kernels: every thread reads the operands of both of its butterflies, then -- one barrier later,
-    // when nobody reads the data buffer any more -- one thread issues the copy of the rest of the next unit's span into it,
-    // and the butterflies and the global stores run while the copy is in flight.  The other kernels stream it one radix-RL
-    // butterfly at a time -- RL live values instead of 16
-    if constexpr (STAGED) {
-        cx<T> w[ITERS][16];
 #pragma unroll
-        for (int it = 0; it < ITERS; ++it) fft_last_pass_load<T, N>(ctx, tid + it * NT, w[it]);
-        if (next_u != nullptr) {
-            __syncthreads();
-            if (tid == 0) {
-                fence_proxy_async_shared();
-                mbar_expect_tx(st.bar, st.bytes - OS_STAGE_HEAD);
-                tma_load_1d(ctx.sm, reinterpret_cast<const unsigned char*>(next_u) + OS_STAGE_HEAD, st.bytes - OS_STAGE_HEAD,
-                            st.bar);
-            }
+    for (int it = 0; it < ITERS; ++it) {
+        const int tp = tid + it * NT;
+        if (Q % NT != 0 && tp >= Q) break;
+        chunk(std::integral_constant<int, 0>{}, tp);
+        if constexpr (NBF >= 2) chunk(std::integral_constant<int, 1>{}, tp);
+        if constexpr (NBF >= 4) { chunk(std::integral_constant<int, 2>{}, tp); chunk(std::integral_constant<int, 3>{}, tp); }
+        if constexpr (NBF >= 8) {
+            chunk(std::integral_constant<int, 4>{}, tp); chunk(std::integral_constant<int, 5>{}, tp);
+            chunk(std::integral_constant<int, 6>{}, tp); chunk(std::integral_constant<int, 7>{}, tp);
         }
+    }
+}
+
+// One unit of the staged kernels (os_threads::staged: the 16384-point Float32 ones), in the 32 · 32 · 16 plan (fft_r32):
+//   first | radix-32 | [last, x H, swap, first] | radix-32 | last
+// Thread tid owns residue class tid of both first passes, butterfly tid of both radix-32 passes and the radix-16
+// butterflies tid, tid + 512 of both last passes, whose outputs X[tid + 512 m], m < 32, are that residue class.
+// staged: the unit's input span is (being) copied to OsStage::head; next_u: slot 0 of the next unit when that one is to be
+// staged (os_fused_kernel decides), else null.
+template <typename T, bool CPLX, bool INTERIOR, bool STATE, typename SG>
+__device__ __forceinline__ void os_unit_r32(const FftR32Ctx<T>& ctx, int tid, const OsUnit<typename os_elt<T, CPLX>::type>& g,
+                                            const cx<T>* __restrict__ H, OsStage& st, bool staged,
+                                            const typename os_elt<T, CPLX>::type* __restrict__ next_u, const SG& state_geometry) {
+    using E = typename os_elt<T, CPLX>::type;
+    constexpr int NT = fft_r32::NT, Q = fft_r32::Q;
+    cx<T> v[32];
+    if (INTERIOR && staged) {
+        // the span in natural order from st.head (head region, then the data buffer): lanes read consecutive words
+        mbar_wait(st.bar, st.parity);
+        st.parity ^= 1;
+        const E* s = reinterpret_cast<const E*>(st.head);
 #pragma unroll
-        for (int it = 0; it < ITERS; ++it) {
-            const int tp = tid + it * NT;
-            fft_last_pass_bfly<T, N>(ctx, tp, w[it]);
-#pragma unroll
-            for (int r = 0; r < 16; ++r) put(tp + r * Q, w[it][r]);
+        for (int m = 0; m < 32; ++m) {
+            const int j = tid + m * Q;
+            if constexpr (CPLX) v[m] = s[j];
+            else v[m] = mkc<T>(s[j], s[j + g.L]);
         }
     } else {
-        auto chunk = [&](auto a_, int tp) {
-            constexpr int A = decltype(a_)::value;
-            cx<T> u[RL];
-            fft_last_pass_chunk<T, N, A>(ctx, tp, u);
 #pragma unroll
-            for (int jj = 0; jj < RL; ++jj) put(tp + (A + NBF * jj) * Q, u[jj]);
-        };
+        for (int m = 0; m < 32; ++m) v[m] = os_sample<T, CPLX, INTERIOR>(g, tid + m * Q);
+    }
+    fft_r32_first_bfly<T>(v);
+    // every thread has read its samples (the staged ones lie in the data buffer's head) and the previous unit's last pass
+    // is over
+    __syncthreads();
+    fft_r32_store_block<T>(ctx.sm, tid, v);
+    __syncthreads();
+    if (next_u != nullptr && tid == 0) {
+        // the head region has been read: the next unit's head goes there now, its phase completes with the rest
+        fence_proxy_async_shared();
+        mbar_expect_tx_noarrive(st.bar, OS_STAGE_HEAD);
+        tma_load_1d(st.head, next_u, OS_STAGE_HEAD, st.bar);
+    }
+#if !(DSP_PROBE & 16)
+    fft_r32_middle<T, true>(ctx, tid);
+#endif
+    __syncthreads();
+    // last forward pass, x H, swap, first pass of the second transform -- in registers
+    {
+        cx<T> u[2][16];
 #pragma unroll
-        for (int it = 0; it < ITERS; ++it) {
-            const int tp = tid + it * NT;
-            if (Q % NT != 0 && tp >= Q) break;
-            chunk(std::integral_constant<int, 0>{}, tp);
-            if constexpr (NBF >= 2) chunk(std::integral_constant<int, 1>{}, tp);
-            if constexpr (NBF >= 4) { chunk(std::integral_constant<int, 2>{}, tp); chunk(std::integral_constant<int, 3>{}, tp); }
-            if constexpr (NBF >= 8) {
-                chunk(std::integral_constant<int, 4>{}, tp); chunk(std::integral_constant<int, 5>{}, tp);
-                chunk(std::integral_constant<int, 6>{}, tp); chunk(std::integral_constant<int, 7>{}, tp);
-            }
+        for (int it = 0; it < 2; ++it) {
+            fft_r32_last_load<T>(ctx, tid + it * NT, u[it]);
+            fft_r32_last_bfly<T>(ctx, tid + it * NT, u[it]);
         }
+#pragma unroll
+#if DSP_PROBE & 4
+        for (int m = 0; m < 32; ++m) v[m] = cswap(cmul(u[m & 1][m >> 1], mkc<T>(T(0.5), T(m))));
+#else
+        for (int m = 0; m < 32; ++m) v[m] = cswap(cmul(u[m & 1][m >> 1], ldg_cx<T>(H + tid + m * Q)));
+#endif
+    }
+    fft_r32_first_bfly<T>(v);
+    __syncthreads();                                   // every thread has read its last-pass inputs
+    fft_r32_store_block<T>(ctx.sm, tid, v);
+    __syncthreads();
+#if !(DSP_PROBE & 16)
+    fft_r32_middle<T, true>(ctx, tid);
+#endif
+    __syncthreads();
+    os_sgeom_t<E, STATE, INTERIOR> sg{};
+    if constexpr (STATE && !INTERIOR) sg = state_geometry();
+    // Last pass: every thread reads the operands of both of its butterflies, then -- one barrier later, when nobody reads
+    // the data buffer any more -- one thread issues the copy of the rest of the next unit's span into it, and the
+    // butterflies and the global stores run while the copy is in flight.
+    cx<T> w[2][16];
+#pragma unroll
+    for (int it = 0; it < 2; ++it) fft_r32_last_load<T>(ctx, tid + it * NT, w[it]);
+    if (next_u != nullptr) {
+        __syncthreads();
+        if (tid == 0) {
+            fence_proxy_async_shared();
+            mbar_expect_tx(st.bar, st.bytes - OS_STAGE_HEAD);
+            tma_load_1d(ctx.sm, reinterpret_cast<const unsigned char*>(next_u) + OS_STAGE_HEAD, st.bytes - OS_STAGE_HEAD, st.bar);
+        }
+    }
+#pragma unroll
+    for (int it = 0; it < 2; ++it) {
+        const int t = tid + it * NT;
+        fft_r32_last_bfly<T>(ctx, t, w[it]);
+#pragma unroll
+        for (int s = 0; s < 16; ++s) os_put<T, CPLX, INTERIOR, STATE>(g, sg, t + s * fft_r32::QL, w[it][s]);
     }
 }
 
@@ -337,6 +389,7 @@ os_fused_kernel(const void* __restrict__ u_, int64_t u_begin, int64_t nu_local, 
                 int64_t zero_from, int nv, int64_t units_per_col, int64_t total_units, const cx<T>* __restrict__ gtl,
                 const cx<T>* __restrict__ g16, const cx<T>* __restrict__ g256, const cx<T>* __restrict__ H,
                 const OsState<typename os_elt<T, CPLX>::type, STATE> sa) {
+    // gtl, g16, g256: the tables of fft_plan_traits<N>; staged kernels: gtl holds those of the 32 · 32 · 16 plan
     constexpr int NT = os_threads<T, N, CPLX>::value;
     constexpr int Q = fft_plan_traits<N>::Q;
     constexpr int ITERS = (Q + NT - 1) / NT;
@@ -347,10 +400,14 @@ os_fused_kernel(const void* __restrict__ u_, int64_t u_begin, int64_t nu_local, 
     using E = typename os_elt<T, CPLX>::type;
     const int tid = threadIdx.x;
     pdl_launch_dependents();
-    const FftCtx<T> ctx = fft_make_ctx<T, N, NT>(sm, g16, g256, gtl, tid);
+    auto make_ctx = [&]() {
+        if constexpr (STAGED) return fft_r32_make_ctx<T>(sm, sm + fft_r32::PADDED_LEN, gtl, tid);
+        else return fft_make_ctx<T, N, NT>(sm, g16, g256, gtl, tid);
+    };
+    const auto ctx = make_ctx();
     OsStage st;
     st.head = smem_raw;
-    st.bar = reinterpret_cast<uint64_t*>(smem_raw + HEAD + (size_t)fft_smem_elems<T, N>() * sizeof(cx<T>));
+    st.bar = reinterpret_cast<uint64_t*>(smem_raw + HEAD + (size_t)os_fft_elems<T, N, CPLX>() * sizeof(cx<T>));
     st.parity = 0;
     if constexpr (STAGED) {
         if (tid == 0) {
@@ -441,8 +498,13 @@ os_fused_kernel(const void* __restrict__ u_, int64_t u_begin, int64_t nu_local, 
         const bool interior = geometry(gu, g);
         const E* next_u = stage_src(gu + gridDim.x);
         auto sgeom = [&]() { return state_geometry(gu); };
-        if (interior) os_unit<T, N, CPLX, NT, true, ITERS, STATE>(ctx, tid, g, H, st, staged, next_u, sgeom);
-        else os_unit<T, N, CPLX, NT, false, ITERS, STATE>(ctx, tid, g, H, st, staged, next_u, sgeom);
+        if constexpr (STAGED) {
+            if (interior) os_unit_r32<T, CPLX, true, STATE>(ctx, tid, g, H, st, staged, next_u, sgeom);
+            else os_unit_r32<T, CPLX, false, STATE>(ctx, tid, g, H, st, staged, next_u, sgeom);
+        } else {
+            if (interior) os_unit<T, N, CPLX, NT, true, ITERS, STATE>(ctx, tid, g, H, sgeom);
+            else os_unit<T, N, CPLX, NT, false, ITERS, STATE>(ctx, tid, g, H, sgeom);
+        }
         staged = next_u != nullptr;
     }
 }
@@ -709,8 +771,9 @@ static int launch_os_fused(OsPlanImpl* p, const OsRange& a, const OsStateArgs& s
     const int64_t blocks = units < cap ? units : cap;
     DSP_CUDA(launch_pdl(kern, (unsigned)blocks, NT, smem, st, a.u, a.u_begin, a.nu_local, a.u_col_stride, a.out, a.out_begin,
                         a.out_count, a.out_col_stride, a.zero_from, (int)p->nv, upc, units,
-                        reinterpret_cast<const cx<T>*>(p->d_tw), reinterpret_cast<const cx<T>*>(p->d_t16),
-                        reinterpret_cast<const cx<T>*>(p->d_t256), reinterpret_cast<const cx<T>*>(p->d_H), sa));
+                        reinterpret_cast<const cx<T>*>(os_threads<T, N, CPLX>::staged ? p->d_r32 : p->d_tw),
+                        reinterpret_cast<const cx<T>*>(p->d_t16), reinterpret_cast<const cx<T>*>(p->d_t256),
+                        reinterpret_cast<const cx<T>*>(p->d_H), sa));
     DSP_LAUNCH_OK();
     return DSPB200_OK;
 }
@@ -987,6 +1050,12 @@ int dspb200_os_plan_create(dspb200_os_plan** plan, int dtype, const void* v_host
             p->sm_count = device_sm_count();
             rc = upload_fft_tables(p->nfft, p->f64, &p->d_tw, &p->d_t16, &p->d_t256);
             if (rc != DSPB200_OK) break;
+            if (!p->f64 && p->nfft == fft_r32::N) {                // the 16384-point Float32 kernels' plan (os_unit_r32)
+                std::vector<cx<float>> tab(fft_r32::TABLE_LEN);
+                fft_r32_fill_tables<float>(tab.data());
+                rc = upload(&p->d_r32, tab.data(), tab.size() * sizeof(cx<float>));
+                if (rc != DSPB200_OK) break;
+            }
             e = cudaMalloc(&p->d_H, (size_t)p->nfft * csz);
             if (e != cudaSuccess) { rc = cuda_fail(e, "cudaMalloc(H)", __FILE__, __LINE__); break; }
             rc = p->f64 ? os_filter_dispatch<double>(p, d_v) : os_filter_dispatch<float>(p, d_v);
@@ -1148,6 +1217,7 @@ int dspb200_os_plan_destroy(dspb200_os_plan* plan) {
     if (p->d_tw) cudaFree(p->d_tw);
     if (p->d_t16) cudaFree(p->d_t16);
     if (p->d_t256) cudaFree(p->d_t256);
+    if (p->d_r32) cudaFree(p->d_r32);
     if (p->d_H) cudaFree(p->d_H);
     if (p->fft_ok) { cufftDestroy(p->fwd); cufftDestroy(p->inv); }
     p->td.release(); p->fd.release();
