@@ -47,6 +47,7 @@ SIGNATURES = {
     "dspb200_host_free": (_int, [_vp]),
     "dspb200_memcpy_h2d": (_int, [_vp, _vp, _sz, _vp]),
     "dspb200_memcpy_d2h": (_int, [_vp, _vp, _sz, _vp]),
+    "dspb200_memcpy2d_d2d": (_int, [_vp, _sz, _vp, _sz, _sz, _sz, _vp]),
     "dspb200_stream_sync": (_int, [_vp]),
     "dspb200_launch_count": (_i64, []),
     "dspb200_fir_plan_create": (_int, [_pp, _int, _vp, _i64]),
@@ -72,6 +73,11 @@ SIGNATURES = {
     "dspb200_conv_nd_os_set_budget": (_int, [C.c_size_t]),
     "dspb200_hilbert_exec": (_int, [_int, _vp, _i64, _i64, _vp]),
     "dspb200_hilbert_exec_dev": (_int, [_int, _vp, _i64, _i64, _vp, _vp]),
+    "dspb200_filtfilt_extend_async": (_int, [_int, _vp, _i64, _i64, _i64, _vp, _vp]),
+    "dspb200_xcorr_peak_async": (_int, [_int, _vp, _i64, _i64, _i64, _int, _vp, _vp, _vp]),
+    "dspb200_shift_async": (_int, [_int, _vp, _i64, _i64, _i64, _vp, _int, _vp, _i64, _vp]),
+    "dspb200_scale_div_async": (_int, [_int, _vp, _i64, _dbl, _vp]),
+    "dspb200_conv_fft_columns": (_int, [_int, _vp, _i64, _i64, _vp, _i64, _i64, _vp, _vp]),
     "dspb200_spec_plan_create": (_int, [_pp, _int, _i64, _i64, _i64, _int, _vp]),
     "dspb200_spec_plan_info": (_int, [_vp, C.POINTER(_i64), C.POINTER(_int)]),
     "dspb200_spec_nsegments": (_i64, [_vp, _i64]),
@@ -512,3 +518,30 @@ def hilbert(x, n, ncols, out):
 
 def hilbert_dev(dtype, x_ptr, n, ncols, out_ptr, stream=0):
     check(lib.dspb200_hilbert_exec_dev(np_dtype_code(np.dtype(dtype)), x_ptr, n, ncols, out_ptr, stream))
+
+
+def memcpy2d_d2d(dst_ptr, dpitch, src_ptr, spitch, width, height, stream=0):
+    check(lib.dspb200_memcpy2d_d2d(dst_ptr, int(dpitch), src_ptr, int(spitch), int(width), int(height), stream))
+
+
+def filtfilt_extend_async(dtype, x_ptr, n, ncols, pad, ext_ptr, stream=0):
+    check(lib.dspb200_filtfilt_extend_async(np_dtype_code(np.dtype(dtype)), x_ptr, int(n), int(ncols), int(pad), ext_ptr, stream))
+
+
+def xcorr_peak_async(dtype, s_ptr, nres, ncols, center, reversed_, delay_ptr, nanflag_ptr, stream=0):
+    check(lib.dspb200_xcorr_peak_async(np_dtype_code(np.dtype(dtype)), s_ptr, int(nres), int(ncols), int(center),
+                                       1 if reversed_ else 0, delay_ptr, nanflag_ptr, stream))
+
+
+def shift_async(dtype, x_ptr, nx, ncols, shift, shifts_ptr, negate, out_ptr, nout, stream=0):
+    check(lib.dspb200_shift_async(np_dtype_code(np.dtype(dtype)), x_ptr, int(nx), int(ncols), int(shift), shifts_ptr,
+                                  1 if negate else 0, out_ptr, int(nout), stream))
+
+
+def scale_div_async(dtype, x_ptr, n, divisor, stream=0):
+    check(lib.dspb200_scale_div_async(np_dtype_code(np.dtype(dtype)), x_ptr, int(n), float(divisor), stream))
+
+
+def conv_fft_columns(dtype, u_ptr, nu, ncols, v_ptr, nv, nfft, out_ptr, stream=0):
+    check(lib.dspb200_conv_fft_columns(np_dtype_code(np.dtype(dtype)), u_ptr, int(nu), int(ncols), v_ptr, int(nv), int(nfft),
+                                       out_ptr, stream))

@@ -209,6 +209,10 @@ int exec_state_host(P* p, const cudaStream_t& s_exec, const void* x, int64_t nx,
 }
 
 int device_sm_count();
+// height rows of width bytes, src + r*spitch -> dst + r*dpitch, device to device on st: one cudaMemcpy2DAsync, or one
+// cudaMemcpyAsync per row where a pitch exceeds the device's cudaDevAttrMaxPitch (columns of more than ~2 GiB) or there is
+// one row.  Copies, no kernel launch.
+int memcpy2d_dd(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t height, cudaStream_t st);
 void count_launch(int n = 1);
 
 // cuFFT plans and device scratch of the plan-less convenience entry points (conv_fft, conv_nd, hilbert, periodogram2) are

@@ -31,6 +31,20 @@ int device_sm_count() {
     return n;
 }
 
+int memcpy2d_dd(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t height, cudaStream_t st) {
+    if (width == 0 || height == 0) return DSPB200_OK;
+    int dev = 0, max_pitch = 0;
+    DSP_CUDA(cudaGetDevice(&dev));
+    DSP_CUDA(cudaDeviceGetAttribute(&max_pitch, cudaDevAttrMaxPitch, dev));
+    if (height > 1 && dpitch <= (size_t)max_pitch && spitch <= (size_t)max_pitch) {
+        DSP_CUDA(cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, height, cudaMemcpyDeviceToDevice, st));
+        return DSPB200_OK;
+    }
+    for (size_t r = 0; r < height; ++r)
+        DSP_CUDA(cudaMemcpyAsync((char*)dst + r * dpitch, (const char*)src + r * spitch, width, cudaMemcpyDeviceToDevice, st));
+    return DSPB200_OK;
+}
+
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
 int cufft_fail(cufftResult r, const char* what) {
@@ -293,6 +307,11 @@ int dspb200_memcpy_d2h(void* dst, const void* src, size_t bytes, void* stream) {
     if (bytes == 0) return DSPB200_OK;
     DSP_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
     return DSPB200_OK;
+}
+int dspb200_memcpy2d_d2d(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t height, void* stream) {
+    if (width == 0 || height == 0) return DSPB200_OK;
+    DSP_REQUIRE(dst && src && dpitch >= width && spitch >= width, "NULL argument or a pitch below the row width");
+    return memcpy2d_dd(dst, dpitch, src, spitch, width, height, (cudaStream_t)stream);
 }
 int dspb200_stream_sync(void* stream) {
     DSP_CUDA(cudaStreamSynchronize((cudaStream_t)stream));

@@ -434,6 +434,27 @@ function hilbert(x::Array{T}) where {T<:GPUReal}
     out
 end
 
+# ---- the device work of filtfilt / finddelay / shiftsignal / alignsignals on device memory (src/Filters/filt.jl:245-259,
+# src/util.jl:360-427).  Raw device pointers and a cudaStream_t (C_NULL: the default stream), as a CuArray binding would
+# pass them; each call enqueues one launch and returns.  Not executed: no `julia` in the build image.
+# extrapolate_signal! of every column: x is n x ncols, ext is (n + 2pad) x ncols, eltype T
+filtfilt_extend!(::Type{T}, ext::Ptr{Cvoid}, x::Ptr{Cvoid}, n::Integer, ncols::Integer, pad::Integer;
+                 stream::Ptr{Cvoid}=C_NULL) where {T<:GPUNumber} =
+    check(ccall((:dspb200_filtfilt_extend_async, libdspb200), Cint, (Cint, Ptr{Cvoid}, Int64, Int64, Int64, Ptr{Cvoid}, Ptr{Cvoid}),
+                dtype_code(T), x, n, ncols, pad, ext, stream))
+# finddelay's peak of every column of the real correlation s (nres x ncols): Int64 delays and Int32 NaN flags per column
+xcorr_peak!(::Type{T}, delay::Ptr{Int64}, nanflag::Ptr{Int32}, s::Ptr{Cvoid}, nres::Integer, ncols::Integer, center::Integer;
+            reversed::Bool=false, stream::Ptr{Cvoid}=C_NULL) where {T<:GPUReal} =
+    check(ccall((:dspb200_xcorr_peak_async, libdspb200), Cint,
+                (Cint, Ptr{Cvoid}, Int64, Int64, Int64, Cint, Ptr{Int64}, Ptr{Int32}, Ptr{Cvoid}),
+                dtype_code(T), s, nres, ncols, center, reversed, delay, nanflag, stream))
+# shiftsignal of every column, zero-filled: by `shift`, or by the device Int64 shifts (negated when `negate`)
+shiftsignal!(::Type{T}, out::Ptr{Cvoid}, x::Ptr{Cvoid}, n::Integer, ncols::Integer; shift::Integer=0,
+             shifts::Ptr{Int64}=Ptr{Int64}(C_NULL), negate::Bool=false, stream::Ptr{Cvoid}=C_NULL) where {T<:GPUNumber} =
+    check(ccall((:dspb200_shift_async, libdspb200), Cint,
+                (Cint, Ptr{Cvoid}, Int64, Int64, Int64, Ptr{Int64}, Cint, Ptr{Cvoid}, Int64, Ptr{Cvoid}),
+                dtype_code(T), x, n, ncols, shift, shifts, negate, out, n, stream))
+
 # ---- mt_cross_power_spectra! / mt_coherence!, src/multitaper.jl:553-603, 722-790.  `plan` is a multitaper plan built
 # with dspb200_mt_plan_create from config.mt_config (tapers pre-scaled by 1/sqrt(r_t)); validation stays in DSP.jl.
 function mt_cross!(output::Array, signal::Matrix{T}, plan::Ptr{Cvoid}, demean::Bool, freq_inds::UnitRange{Int},

@@ -69,6 +69,11 @@ DSPB200_API int dspb200_host_alloc(void** hptr, size_t bytes);  /* pinned host m
 DSPB200_API int dspb200_host_free(void* hptr);
 DSPB200_API int dspb200_memcpy_h2d(void* dst, const void* src, size_t bytes, void* stream);
 DSPB200_API int dspb200_memcpy_d2h(void* dst, const void* src, size_t bytes, void* stream);
+/* height rows of width bytes, row r at src + r*spitch -> dst + r*dpitch, device to device, enqueued on `stream` (cropping
+ * the columns of a column-major matrix: one row per column).  Pitches past the device's limit for 2-D copies (about 2 GiB)
+ * are copied row by row, so any column length within DSPB200_INDEX_LIMIT works. */
+DSPB200_API int dspb200_memcpy2d_d2d(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t height,
+                                     void* stream);
 DSPB200_API int dspb200_stream_sync(void* stream);
 
 /* Number of kernels this library has launched in this process (bench.py's `gpu_launches`). */
@@ -189,6 +194,41 @@ DSPB200_API int dspb200_conv_nd_os_set_budget(size_t bytes);
  * pointers and a cudaStream_t and returns after the work on that stream has completed. */
 DSPB200_API int dspb200_hilbert_exec(int dtype, const void* x, int64_t n, int64_t ncols, void* out);
 DSPB200_API int dspb200_hilbert_exec_dev(int dtype, const void* d_x, int64_t n, int64_t ncols, void* d_out, void* stream);
+
+/* ------------------------------------------------------------------------------------------ xcorr / filtfilt / finddelay
+ * The device work of xcorr, FIR filtfilt, finddelay, shiftsignal and alignsignals (src/dspbase.jl:867-898,
+ * src/util.jl:336-427, src/Filters/filt.jl:245-259, 301-337) that surrounds the filter and correlation calls above.  The
+ * *_async calls follow the conventions of the asynchronous _dev calls: device pointers, every launch on `stream`, no
+ * synchronisation, capturable in a CUDA graph.  Matrices are column-major, one channel per column.  DSPB200_EINVALID,
+ * before any launch: a NULL buffer, a negative size, an output overlapping an input, a size past DSPB200_INDEX_LIMIT.
+ * ncols == 0 (and nout == 0, n == 0 where they are sizes of the output) launches nothing.  Each call is one launch. */
+/* extrapolate_signal! (src/Filters/filt.jl:245-259): column c of ext ((n + 2 pad) x ncols) is the odd-symmetric extension
+ * [2x[0] - x[pad..1]; x; 2x[n-1] - x[n-2..n-1-pad]] of column c of x (n x ncols), each sample rounded in dtype as the
+ * host computes it.  pad >= n gives DSPB200_EINVALID. */
+DSPB200_API int dspb200_filtfilt_extend_async(int dtype, const void* x, int64_t n, int64_t ncols, int64_t pad, void* ext,
+                                              void* stream);
+/* finddelay's peak (src/util.jl:360-368) of every column of the real correlation s (nres x ncols, F32 or F64): among the
+ * samples of largest |s| the one closest to `center` (1-based index), the lower one on a tie; delay[c] = center - index.
+ * Exact comparisons, no floating-point atomics: the result does not depend on the launch.  nanflag[c] = 1 when the column
+ * holds a NaN (the reference throws; delay[c] is then meaningless), else 0.  reversed != 0: sample p of a column stands at
+ * index nres - 1 - p (xcorr(y, x) stored as xcorr(x, y)).  One cluster of up to 8 CTAs per column.  Complex dtypes give
+ * DSPB200_EINVALID; nres == 0 with ncols > 0 too. */
+DSPB200_API int dspb200_xcorr_peak_async(int dtype, const void* s, int64_t nres, int64_t ncols, int64_t center, int reversed,
+                                         int64_t* delay, int* nanflag, void* stream);
+/* shiftsignal (src/util.jl:379-412), out of place: out[i, c] = x[i - s_c, c] where 0 <= i - s_c < nx, else zero, for
+ * i < nout (nout == nx: shiftsignal; nout > nx with s = 0: zero padding).  s_c = shifts[c] (device int64, negated when
+ * negate != 0: alignsignals' -delay) when shifts != NULL, else `shift`, which must satisfy |shift| <= nx. */
+DSPB200_API int dspb200_shift_async(int dtype, const void* x, int64_t nx, int64_t ncols, int64_t shift, const int64_t* shifts,
+                                    int negate, void* out, int64_t nout, void* stream);
+/* xcorr's :biased scaling, in place: x[i] / divisor in dtype for i < n, as numpy divides by a Python integer (a complex
+ * sample times the rounded reciprocal of divisor + 0im, as Smith's division does with a zero imaginary part). */
+DSPB200_API int dspb200_scale_div_async(int dtype, void* x, int64_t n, double divisor, void* stream);
+/* conv(u[:, c], v; algorithm=:fft_simple) for every column of u (nu x ncols) with one vector v (nv): one batched 1-D transform
+ * pair of nfft >= nu + nv - 1 points over the columns (no transform along the channels); out is (nu + nv - 1) x ncols.  Device
+ * pointers; like the plan-less _dev calls it uses the cached plans and returns after the work on `stream` has completed.
+ * Five launches whatever ncols. */
+DSPB200_API int dspb200_conv_fft_columns(int dtype, const void* d_u, int64_t nu, int64_t ncols, const void* d_v, int64_t nv,
+                                         int64_t nfft, void* d_out, void* stream);
 
 /* ------------------------------------------------------------------------------------------ Welch / STFT
  * One plan per (dtype, n, noverlap, nfft, onesided, window): the analogue of WelchConfig
