@@ -10,6 +10,9 @@ the same thin layer over the same C ABI, include/dspb200.h):
     STFTStream (an extension: stft / spectrogram of a chunked multichannel stream)
     WelchStream (an extension: welch_pgram of a chunked multichannel stream)
                                                                        (src/periodograms.jl)
+    MTConfig, MTSpectrogramConfig, mt_pgram, mt_spectrogram, mt_spectrogram_, allocate_output, MTSpectrogramStream (an
+    extension: mt_spectrogram of a chunked multichannel stream), mt_cross_power_spectra, mt_coherence
+                                                                       (src/multitaper.jl)
     hanning, hamming, rect, bartlett, kaiser, nextfastfft              (src/windows.jl, src/util.jl)
 
 All numerics run in hand-written CUDA kernels inside libdspb200.so; there is no CPU fallback.
@@ -30,8 +33,9 @@ from .filters import filt_ as filt_hx_
 from .periodograms import (Periodogram, Periodogram2, Spectrogram, STFTStream, WelchConfig, WelchStream, arraysplit, arraysplit_count, compute_window, fftshift,
                            filt_welch, freq, periodogram, power, spectrogram, stft, time, welch_pgram, welch_pgram_)
 
-from .multitaper import (Coherence, CrossPowerSpectra, MTConfig, MTCrossSpectraConfig, dpss, dpss_config, dpsseig,
-                         mt_coherence, mt_cross_power_spectra, mt_pgram, mt_spectrogram)
+from .multitaper import (Coherence, CrossPowerSpectra, MTConfig, MTCrossSpectraConfig, MTSpectrogramConfig, MTSpectrogramStream,
+                         allocate_output, dpss, dpss_config, dpsseig, mt_coherence, mt_cross_power_spectra, mt_pgram,
+                         mt_spectrogram, mt_spectrogram_)
 from .clients import alignsignals, filtfilt, finddelay, hilbert, shiftsignal, xcorr
 from . import device, filters, sharding
 

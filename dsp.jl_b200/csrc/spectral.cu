@@ -2364,11 +2364,49 @@ static int stft_stream_check(const SpecPlanImpl* p, const void* hist_in, int64_t
     DSP_REQUIRE(nhist >= 0 && nx >= 0 && nchan >= 0 && nseg >= 0 && ldh >= 0, "negative size");
     DSP_REQUIRE(psd_only == 0 || psd_only == 1, "psd_only must be 0 (raw spectra) or 1 (PSD columns)");
     DSP_REQUIRE(r != 0.0 || !psd_only, "r must be nonzero");
+    // a multitaper plan's rows carry 1/sqrt(r_t): PSD columns with r = 1 only (raw spectra of a taper sum are not defined)
+    DSP_REQUIRE(p->ntapers == 0 || (psd_only == 1 && r == 1.0), "a multitaper plan streams PSD columns (psd_only = 1) with r = 1");
     DSP_REQUIRE(ldo >= nseg, "output column stride ldo < nseg");
     const size_t oel = (psd_only ? 1 : 2) * (p->f64 ? 8 : 4);
     const size_t obytes = (nchan && nseg) ? (size_t)(((nchan - 1) * ldo + nseg) * p->nout) * oel : 0;
     return stream_check(p, hist_in, nhist, hist_out, ldh, x, nx, nchan, nseg, out, obytes, "out", dev, newh, launch);
 }
+
+extern "C++" {
+// out[c ldc + i] + add[c per + i], rounded once, for i < per and c < nchan: the taper add of a streaming mt_spectrogram, whose
+// channels are ldc values apart in `out` (ldo columns) and per apart in the plan's scratch (nseg columns)
+template <typename T>
+__global__ void acc_add_cols_kernel(T* __restrict__ out, int64_t ldc, const T* __restrict__ add, int64_t per, int64_t nchan) {
+    const int64_t total = per * nchan;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t c = i / per;
+        T* o = out + c * ldc + (i - c * per);
+        *o = add_rn(*o, add[i]);
+    }
+}
+
+// Streaming mt_spectrogram, cuFFT sizes, in the order of the one-shot call (mt_spectrogram_queue): taper 0's PSD columns
+// into out, every later taper's into the plan's scratch and then added to out, each through the generic stream STFT
+template <typename T>
+static int mt_stream_generic(SpecPlanImpl* p, const StftStreamArgs& sa, const void* x, int64_t nx, int64_t nchan, int64_t nseg,
+                             void* out, cudaStream_t st) {
+    DSP_TRY(generic_prepare(p));
+    const int64_t per = p->nout * nseg;
+    DSP_TRY(p->tmp.reserve((size_t)(per * nchan) * sizeof(T)));
+    StftStreamArgs st_tmp = sa;
+    st_tmp.ldo = nseg;
+    return for_each_taper(p, [&](int64_t t) -> int {
+        DSP_TRY(stft_generic<T>(p, t == 0 ? sa : st_tmp, x, nx, nchan, nseg, 1.0, 1, t == 0 ? out : p->tmp.p, st));
+        if (t == 0) return DSPB200_OK;
+        const int threads = 256;
+        const int64_t want = cdiv(per * nchan, threads), cap = (int64_t)p->sm_count * 32;
+        acc_add_cols_kernel<T><<<(unsigned)(want < cap ? want : cap), threads, 0, st>>>((T*)out, sa.ldo * p->nout,
+                                                                                       (const T*)p->tmp.p, per, nchan);
+        DSP_LAUNCH_OK();
+        return DSPB200_OK;
+    });
+}
+}  // extern "C++"
 
 // Segments 0 .. nseg - 1 of every channel's virtual column [hist_in (nhist); x (nx)] into out (column s of channel c at
 // out + (c ldo + s) nout), then the new history v[nseg hop, nhist + nx) into hist_out.  Fused sizes: at most two launches.
@@ -2393,7 +2431,14 @@ int dspb200_stft_stream_exec_dev(dspb200_spec_plan* plan, const void* hist_in, i
     sa.seam = p->seam.p;
     sa.lds = sm.lds;
     if (nseg == 0) return DSPB200_OK;
-    // launch 2 (fused sizes; cuFFT sizes: three per batch): the transforms
+    // launch 2 (fused sizes; cuFFT sizes: three per batch): the transforms -- a multitaper plan's every taper row in the one
+    // fused launch, or its tapers one after another through cuFFT
+    if (p->ntapers >= 1) {
+        if (!p->fused)
+            return p->f64 ? mt_stream_generic<double>(p, sa, x, nx, nchan, nseg, out, st)
+                          : mt_stream_generic<float>(p, sa, x, nx, nchan, nseg, out, st);
+        sa.ntapers = (int)p->ntapers;
+    }
     return stft_launch(p, sa, x, nx, nchan, nseg, r, psd_only, out, st);
 }
 
@@ -2527,7 +2572,8 @@ int dspb200_welch_stream_power(dspb200_spec_plan* plan, const double* acc, int64
 // of each of the nchan columns of a len x nchan matrix, every channel's tapers summed in taper order (the vector forms are
 // nchan = 1).  Fused sizes: mt_pgram is launch_mt_pgram (two launches per channel group), mt_spectrogram ONE launch of the
 // STFT kernels' taper-row instances (WIN == 2).  cuFFT sizes: mt_pgram_generic; mt_spectrogram is one batched STFT over all
-// channels per taper, each after the first followed by acc_add_kernel.
+// channels per taper, each after the first followed by acc_add_kernel.  A stream of mt_spectrogram is the STFT stream call on
+// a multitaper plan (dspb200_stft_stream_exec_dev: the same WIN == 2 launch, or mt_stream_generic).
 static size_t mt_out_bytes(const SpecPlanImpl* p, int64_t nchan, int64_t k) {
     return (size_t)(p->nout * k * nchan) * (p->f64 ? 8 : 4);
 }

@@ -1,6 +1,6 @@
 """Multitaper spectral estimation front ends (SURVEY.md 8f rank 1; reference src/multitaper.jl:5-790), backed by
-libdspb200: `dpss`, `dpsseig`, `MTConfig`, `dpss_config`, `mt_pgram`, `mt_spectrogram`, `mt_cross_power_spectra`,
-`mt_coherence`."""
+libdspb200: `dpss`, `dpsseig`, `MTConfig`, `dpss_config`, `mt_pgram`, `MTSpectrogramConfig`, `mt_spectrogram`,
+`mt_spectrogram_` (`mt_spectrogram!`), `allocate_output`, `MTSpectrogramStream`, `mt_cross_power_spectra`, `mt_coherence`."""
 import math
 
 import numpy as np
@@ -8,7 +8,7 @@ import numpy as np
 from . import _lib
 from .device import DeviceArray
 from .errors import ArgumentError, DimensionMismatch, DomainError
-from .periodograms import Periodogram, Spectrogram, arraysplit_count
+from .periodograms import Periodogram, Spectrogram, STFTStream, arraysplit_count
 from .util import fftabs2type, fftfreq, fftintype, fftouttype, nextfastfft, rfftfreq
 
 
@@ -75,8 +75,19 @@ class MTConfig:
         self.r = fs * norm2 / w                                                      # :135-139
         self.freq = rfftfreq(nfft, fs) if onesided else fftfreq(nfft, fs)
         self.intype = fftintype(eltype)
-        scaled = (win / np.sqrt(self.r)[None, :]).T                                  # rows pre-scaled by 1/sqrt(r_t)
-        self.plan = _lib.MtPlan(self.intype, n_samples, noverlap, nfft, onesided, scaled)
+        self._rows = (win / np.sqrt(self.r)[None, :]).T                              # rows pre-scaled by 1/sqrt(r_t)
+        self.plan = _lib.MtPlan(self.intype, n_samples, noverlap, nfft, onesided, self._rows)
+        self._spectrogram_plans = {int(noverlap): self.plan}
+
+    def spectrogram_plan(self, n_overlap):
+        """The plan of these taper rows with segments n_samples - n_overlap apart (a plan fixes its overlap): `plan` itself
+        for the overlap it was built with, otherwise one more plan of the same rows, built on first use and kept."""
+        n_overlap = int(n_overlap)
+        plan = self._spectrogram_plans.get(n_overlap)
+        if plan is None:
+            plan = self._spectrogram_plans[n_overlap] = _lib.MtPlan(self.intype, self.n_samples, n_overlap, self.nfft,
+                                                                     self.onesided, self._rows)
+        return plan
 
 
 def _mt_signal(s):
@@ -89,8 +100,9 @@ def _mt_signal(s):
     return s, dev, (s.shape[1] if s.ndim == 2 else None)
 
 
-def _mt_run(s, dev, nchan, config, shape, run, run_dev):
-    """Run a multitaper plan over the columns of s (nchan None: a vector) into a result of `shape` + (nchan,)."""
+def _mt_run(s, dev, nchan, config, shape, run, run_dev, out=None):
+    """Run a multitaper plan over the columns of s (nchan None: a vector) into a result of `shape` + (nchan,): a new array,
+    or `out` (checked by the caller: that shape and the real eltype of the config, a DeviceArray for a device signal)."""
     shape = shape + ((nchan,) if nchan is not None else ())
     nc = 1 if nchan is None else nchan
     odt = fftabs2type(config.intype)
@@ -99,14 +111,16 @@ def _mt_run(s, dev, nchan, config, shape, run, run_dev):
     if dev:                                                        # device-resident signal: the result stays in HBM
         if s.dtype != config.intype:
             raise ArgumentError(f"eltype of the device signal {s.dtype} does not match the config's {config.intype}")
-        dout = DeviceArray(shape, odt)
+        dout = DeviceArray(shape, odt) if out is None else out
         if launch:
             run_dev(s.ptr, length, nc, dout.ptr)
         return dout
-    out = np.zeros(shape, dtype=odt, order="F")
+    res = np.zeros(shape, dtype=odt, order="F") if out is None or not out.flags.f_contiguous else out
     if launch:
-        run(np.asfortranarray(s.reshape(length, nc), dtype=config.intype), length, nc, out)
-    return out
+        run(np.asfortranarray(s.reshape(length, nc), dtype=config.intype), length, nc, res)
+    if out is not None and res is not out:
+        out[...] = res
+    return res if out is None else out
 
 
 def mt_pgram(s, config=None, onesided=None, nfft=None, fs=1, nw=4, ntapers=None, window=None):
@@ -126,10 +140,89 @@ def mt_pgram(s, config=None, onesided=None, nfft=None, fs=1, nw=4, ntapers=None,
     return Periodogram(power, config.freq)
 
 
+class MTSpectrogramConfig:
+    """MTSpectrogramConfig(n_samples, mt_config, n_overlap_samples) /
+    MTSpectrogramConfig{T}(n_samples, samples_per_window, n_overlap_samples; fs, kwargs...), src/multitaper.jl:248-285:
+    segments of mt_config.n_samples samples, n_overlap_samples apart, of a signal of n_samples; `time` holds the segment
+    centres (samples_per_window/2 + hop*i)/fs.  Keyword settings (those of MTConfig) build the MTConfig of `eltype`."""
+
+    def __init__(self, n_samples, mt_config_or_samples_per_window, n_overlap_samples, eltype=np.float64, fs=1, **kw):
+        if isinstance(mt_config_or_samples_per_window, MTConfig):
+            if kw:
+                raise ArgumentError("pass either an MTConfig or keyword settings")
+            mt = mt_config_or_samples_per_window
+        else:
+            mt = MTConfig(eltype, int(mt_config_or_samples_per_window), fs=fs, **kw)
+        spw, n_overlap_samples = mt.n_samples, int(n_overlap_samples)
+        if spw <= n_overlap_samples:
+            raise ArgumentError("Need `samples_per_window > n_overlap_samples`; got `samples_per_window` = "
+                                f"{spw} and `n_overlap_samples` = {n_overlap_samples}.")
+        if n_overlap_samples < 0:
+            raise DomainError("noverlap must be between zero and n")                  # ArraySplit, src/periodograms.jl:44
+        hop = spw - n_overlap_samples
+        k = arraysplit_count(int(n_samples), spw, n_overlap_samples)
+        self.n_samples, self.n_overlap_samples, self.mt_config = int(n_samples), n_overlap_samples, mt
+        self.time = (spw / 2 + hop * np.arange(k, dtype=np.float64)) / mt.fs
+
+
+def allocate_output(config):
+    """allocate_output(config::MTSpectrogramConfig), src/multitaper.jl:326-328: an uninitialised
+    length(freq) x length(time) matrix of the real eltype of the config, column-major."""
+    if not isinstance(config, MTSpectrogramConfig):
+        raise ArgumentError("allocate_output takes an MTSpectrogramConfig")
+    mt = config.mt_config
+    return np.empty((mt.freq.size, config.time.size), dtype=fftabs2type(mt.intype), order="F")
+
+
+def _mt_spectrogram_config(s, config, out):
+    """mt_spectrogram(s, config) / mt_spectrogram!(out, s, config) (out None: a new array), src/multitaper.jl:308-338."""
+    s, dev, nchan = _mt_signal(s)
+    mt = config.mt_config
+    shape = (mt.freq.size, config.time.size)
+    if out is not None:
+        want = shape + ((nchan,) if nchan is not None else ())
+        if tuple(out.shape) != want:
+            raise DimensionMismatch(f"Expected `destination` to be of size `(length(config.mt_config.freq), "
+                                    f"length(config.time))` = {want}; got {tuple(out.shape)}")
+    if s.shape[0] != config.n_samples:
+        raise DimensionMismatch(f"Expected `signal` to be of length `config.n_samples`; got {s.shape[0]} and "
+                                f"{config.n_samples}")
+    if out is not None:
+        if dev != isinstance(out, DeviceArray):
+            raise ArgumentError("the destination of a device signal is a DeviceArray, that of a host signal a host array")
+        if out.dtype != fftabs2type(mt.intype):
+            raise ArgumentError(f"Eltype of output ({out.dtype}) doesn't match the expected type: {fftabs2type(mt.intype)}.")
+        if dev and out.overlaps(s):
+            raise ArgumentError("the destination must not overlap the signal")
+    plan = mt.spectrogram_plan(config.n_overlap_samples)
+    power = _mt_run(s, dev, nchan, mt, (plan.nout, config.time.size), plan.mt_spectrogram_batch,
+                    plan.mt_spectrogram_batch_dev, out)
+    return Spectrogram(power, mt.freq, config.time)
+
+
+def mt_spectrogram_(out, s, config):
+    """mt_spectrogram!(destination, signal, config::MTSpectrogramConfig), src/multitaper.jl:308-324: the multitaper
+    spectrogram into `out`, length(freq) x length(time) (x nchan for a len x nchan signal; a DeviceArray for a device
+    signal, which may not overlap it).  Returns the Spectrogram, whose power is `out`."""
+    if not isinstance(config, MTSpectrogramConfig):
+        raise ArgumentError("mt_spectrogram_ takes an MTSpectrogramConfig")
+    return _mt_spectrogram_config(s, config, out)
+
+
 def mt_spectrogram(s, n=None, n_overlap=None, fs=1, onesided=None, nfft=None, nw=4, ntapers=None, window=None):
-    """mt_spectrogram(signal, n, n_overlap; fs, onesided, kwargs...), src/multitaper.jl:262-404 (default nfft = nextpow(2, n)).
+    """mt_spectrogram(signal, n, n_overlap; fs, onesided, kwargs...), src/multitaper.jl:262-404 (default nfft = nextpow(2, n)),
+    mt_spectrogram(signal, config::MTSpectrogramConfig) and mt_spectrogram(signal, mt_config::MTConfig,
+    n_overlap=mt_config.n_samples >> 1) (:330-391; the settings are then those of the config).
     A 2-D `s` (len x nchan) is the batched extension: power is nout x k x nchan, the layout of the batched spectrogram, and
     freq and time come from len = size(s, 1)."""
+    if isinstance(n, MTSpectrogramConfig):
+        if n_overlap is not None:
+            raise ArgumentError("an MTSpectrogramConfig fixes the overlap")
+        return _mt_spectrogram_config(s, n, None)
+    if isinstance(n, MTConfig):
+        s = _mt_signal(s)[0]
+        config = MTSpectrogramConfig(s.shape[0], n, n.n_samples >> 1 if n_overlap is None else n_overlap)
+        return _mt_spectrogram_config(s, config, None)
     s, dev, nchan = _mt_signal(s)
     length = s.shape[0]
     n = length >> 3 if n is None else int(n)
@@ -142,6 +235,73 @@ def mt_spectrogram(s, n=None, n_overlap=None, fs=1, onesided=None, nfft=None, nw
     plan = config.plan
     power = _mt_run(s, dev, nchan, config, (plan.nout, k), plan.mt_spectrogram_batch, plan.mt_spectrogram_batch_dev)
     return Spectrogram(power, config.freq, t)
+
+
+class MTSpectrogramStream(STFTStream):
+    """mt_spectrogram of a signal that arrives in chunks (an extension: the reference's mt_spectrogram takes one vector).
+
+    MTSpectrogramStream(mt_config, n_overlap=n>>1, device=False) streams with the tapers, weights, nfft, fs and sidedness of
+    an MTConfig, whose eltype every chunk must have; MTSpectrogramStream(n, n_overlap=n>>1, fs=1, onesided=None,
+    nfft=nextpow(2, n), nw=4, ntapers=None, window=None, taper_weights=None, device=False) builds the MTConfig from those
+    settings and the first chunk's eltype.  It is a psdonly STFTStream whose plan holds the config's pre-scaled taper rows
+    (r = 1): the chunk rules, `history`, `history_len`, `nsegments`, reset(), the pairing of real segments and the launch
+    counts are those of STFTStream, and the columns a chunk completes are exactly (bit for bit) the columns of
+    mt_spectrogram(concatenation of all chunks so far, mt_config, n_overlap) at the global segment indices.
+    `mt_spectrogram(x)` returns their Spectrogram, `mt_spectrogram_(out, x)` writes them into `out` and returns their
+    number, and `finish()` returns the Spectrogram of the held-back last segment of a real stream."""
+
+    _a_name = "an MTSpectrogramStream"
+
+    def __init__(self, config_or_n, n_overlap=None, fs=1, onesided=None, nfft=None, nw=4, ntapers=None, window=None,
+                 taper_weights=None, device=False):
+        self._given = config_or_n if isinstance(config_or_n, MTConfig) else None
+        if self._given is not None:
+            mt = self._given
+            n, fs, nfft, onesided = mt.n_samples, mt.fs, mt.nfft, mt.onesided
+        else:
+            n = int(config_or_n)
+            if n <= 0:
+                raise ArgumentError("`n_samples` must be positive")
+            nfft = (1 << (n - 1).bit_length()) if nfft is None else int(nfft)                   # nextpow(2, n)
+            self._mt_kw = dict(fs=fs, nfft=nfft, window=window, nw=nw, ntapers=ntapers, taper_weights=taper_weights,
+                               onesided=onesided)
+        super().__init__(n, n_overlap, psdonly=True, onesided=onesided, nfft=nfft, fs=fs, device=device)
+        self.r = 1.0                                        # the taper rows carry 1/sqrt(r_t)
+        self._configs = {}
+        self.mt_config = self._given
+
+    def _setup(self, dt, chan_shape):
+        mt = self._configs.get(dt)
+        if mt is None:
+            if self._given is not None:
+                if dt != self._given.intype:
+                    raise ArgumentError(f"this MTSpectrogramStream's MTConfig takes {self._given.intype} chunks; got {dt}")
+                mt = self._given
+            else:
+                mt = MTConfig(dt, self.n, noverlap=self.noverlap, **self._mt_kw)
+            self._configs[dt] = mt
+            self._plans[dt] = mt.spectrogram_plan(self.noverlap)
+        super()._setup(dt, chan_shape)
+        self.mt_config = mt
+
+    def _freq(self):
+        return rfftfreq(self.nfft, self.fs) if self.onesided else fftfreq(self.nfft, self.fs)
+
+    def mt_spectrogram(self, x):
+        """Spectrogram(power, freq, time) of the columns chunk x completes: power is (nout, kc) for a vector chunk,
+        (nout, kc, nchan) for a matrix chunk; the time of global segment g is (n/2 + g*hop)/fs."""
+        return self.spectrogram(x)
+
+    def mt_spectrogram_(self, out, x):
+        """The columns chunk x completes into `out`, whose second dimension holds at least kc columns; returns kc."""
+        return self.stft_(out, x)
+
+    def finish(self):
+        """Spectrogram of the held-back last segment of a real stream (0 or 1 column per channel); None before the first
+        chunk.  Ends the stream until reset()."""
+        g0 = self.nsegments
+        p = super().finish()
+        return None if p is None else Spectrogram(p, self._freq(), self._times(g0, p.shape[1]))
 
 
 def dpsseig(A, nw):

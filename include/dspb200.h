@@ -323,7 +323,14 @@ DSPB200_API int dspb200_stft_exec_dev(dspb200_spec_plan* plan, const void* s, in
  * any launch, when hist_out overlaps hist_in, x or out, when out overlaps x or a history buffer, when ldo < nseg, when
  * (nseg-1)*hop + n > nhist + nx, or when the new history would exceed ldh.  nx == 0 with nseg == 0 launches nothing and
  * leaves hist_out as it was (the history is still hist_in).  Fused sizes: at most two launches; cuFFT sizes: three per
- * batch of (channel, segment) pairs plus the history. */
+ * batch of (channel, segment) pairs plus the history.
+ * A multitaper plan (dspb200_mt_plan_create) streams mt_spectrogram: psd_only must be 1 and r 1.0 (the taper rows carry
+ * 1/sqrt(r_t)), otherwise DSPB200_EINVALID before any launch.  Column s of channel c is then the PSD of that segment summed
+ * over the plan's taper rows in taper order, the bits of column s of dspb200_mt_spectrogram_batch_exec_dev over the
+ * concatenated signal; the virtual columns, pairing, plan and refusals are those above, and the call is queued on the
+ * caller's stream like every other call of this form.  Fused sizes: at most two launches (the history, then every taper row
+ * of every segment in one launch); cuFFT sizes: per taper three launches per batch of (channel, segment) pairs, one add per
+ * taper after the first, plus the history. */
 DSPB200_API int dspb200_stft_stream_exec_dev(dspb200_spec_plan* plan, const void* hist_in, int64_t nhist, void* hist_out, int64_t ldh,
                                              const void* x, int64_t nx, int64_t nchan, int64_t nseg, double r, int psd_only,
                                              void* out, int64_t ldo, void* stream);
