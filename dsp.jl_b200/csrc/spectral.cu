@@ -13,10 +13,12 @@
 //     finalize kernel reduces the rows of each channel.
 //   * STFT / spectrogram: the spectrum is parked in shared memory (natural order), un-mixed per bin and
 //     stored column by column, coalesced along frequency.
-// Generic path (any other nfft): segment/window kernel -> batched cuFFT -> power / store kernels.
+// Generic path (any other nfft): seg_window_kernel -> batched cuFFT -> power / store kernels.  Every cuFFT-size Welch and
+// mt_pgram is one segment list per channel through seg_window_kernel, cuFFT and a Float64 accumulate kernel, then
+// welch_stream_power_kernel.
 // STFT: one-shot and streaming calls (dspb200_stft_stream_exec(_dev)) run the same kernels over each channel's virtual column
 // [history; chunk] (StftStream; a one-shot call has no history), a stream after stft_stream_edge_kernel has copied the seam
-// samples and written the new history; cuFFT sizes run a call's (channel, segment) pairs through stft_seg_kernel -> cuFFT ->
+// samples and written the new history; cuFFT sizes run a call's (channel, segment) pairs through seg_window_kernel -> cuFFT ->
 // stft_store_kernel.
 #include "fft_core.cuh"
 #include "async_copy.cuh"
@@ -59,13 +61,13 @@ struct SpecPlanImpl {
     WelchCfg welch_batch_cfg[2];
     WelchCfg welch_mt_cfg[2];     // the batched kernel's taper-row instances (mt_pgram), which share `bpartial`
     DevBuf bpartial;              // fused: one row of nfft real T per (channel, slice), at most WELCH_BATCH_SCRATCH bytes
-    DevBuf bacc;                  // generic: double[nbins_fft], one channel at a time
+    DevBuf bacc;                  // generic: double[nout], one channel at a time (mt_pgram: double[nout][nchan])
     // generic path
     cufftHandle fft = 0;
     bool fft_ok = false;
     int64_t batch = 0;            // segments per cuFFT call
     int64_t nbins_fft = 0;        // nfft/2+1 (real) or nfft (complex)
-    DevBuf segbuf, specbuf, acc;  // acc: double[nbins_fft]
+    DevBuf segbuf, specbuf, acc;  // acc: double[nout], the accumulation open since welch_begin
     // host-pointer path
     HostPipe pipe;
     DevBuf hin, hout;             // dspb200_stft_stream_exec: the staged histories
@@ -817,54 +819,6 @@ stft_w1k_kernel(const void* __restrict__ s_, int64_t chan_stride, int64_t k, int
     }
 }
 
-// ---------------------------------------------------------------------------------------------- generic kernels
-// buf[b][j] = window[j] * s[(seg0+b)*hop + j] (j < n), 0 for n <= j < nfft and for b >= nseg.
-template <typename T, bool CPLX>
-__global__ void seg_window_kernel(const void* __restrict__ s_, int64_t first_sample, int64_t hop, int64_t n,
-                                  int64_t nfft, int64_t nseg, int64_t batch, const typename win_t<T>::type* __restrict__ win,
-                                  void* __restrict__ buf_) {
-    using In = typename in_type<T, CPLX>::type;
-    const In* s = reinterpret_cast<const In*>(s_);
-    In* buf = reinterpret_cast<In*>(buf_);
-    const int64_t total = batch * nfft;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t b = i / nfft, j = i - b * nfft;
-        In v;
-        if constexpr (CPLX) v = mkc<T>(T(0), T(0)); else v = T(0);
-        if (b < nseg && j < n) {
-            v = s[first_sample + b * hop + j];
-            if (win) {
-                const auto w = win[j];
-                if constexpr (CPLX) v = mkc<T>(win_mul(v.x, w), win_mul(v.y, w)); else v = win_mul(v, w);
-            }
-        }
-        buf[i] = v;
-    }
-}
-
-// acc[k] += sum_b |X[b][k]|^2  (thread per bin, coalesced along k)
-template <typename T>
-__global__ void pow_acc_kernel(const cx<T>* __restrict__ X, int64_t nbins, int64_t nseg, double* __restrict__ acc) {
-    const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (k >= nbins) return;
-    double sum = 0.0;
-    for (int64_t b = 0; b < nseg; ++b) sum += (double)cabs2(X[b * nbins + k]);
-    acc[k] += sum;
-}
-
-// out[k] from acc (fft2pow! scaling and the real two-sided mirror, :142-172)
-template <typename T>
-__global__ void pow_finalize_kernel(const double* __restrict__ acc, int64_t nbins_fft, int64_t nfft, int64_t nout,
-                                    int onesided, double m1, double m2, T* __restrict__ out) {
-    const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (k >= nout) return;
-    int64_t src = k;
-    if (k >= nbins_fft) src = nfft - k;   // mirror of a real FFT
-    double m = m1;
-    if (onesided && k != 0 && !(k == nbins_fft - 1 && (nfft % 2 == 0))) m = m2;
-    out[k] = (T)(acc[src] * m);
-}
-
 // ---------------------------------------------------------------------------------------------- STFT, small kernels
 // Launch 1 of a streaming call, one grid-stride pass over nchan x (ls + hn) items: (a) seam[c lds + i] = v_c[i], i < ls --
 // the samples of the units that start in the history, contiguous, so that the transform reads every unit from one range;
@@ -883,20 +837,22 @@ __global__ void stft_stream_edge_kernel(const E* __restrict__ hist_in, int64_t h
     }
 }
 
-// STFT calls, cuFFT sizes: the call's nchan x k (channel c, segment j) pairs, f = c k + j, fill the cuFFT batch in
-// order.  Slot b = blockIdx.y holds pair f0 + b: buf[b][i] = window[i] * v_c[j hop + i] (i < n), 0 for n <= i < nfft and
-// for slots past the list -- seg_window_kernel's values, read from the virtual column.  One slot per grid row: the pair is
-// resolved once per block, not per element.
+// cuFFT sizes (STFT, Welch, multitaper, arraysplit): the call's nchan x k (channel c, segment j) pairs, f = c k + j, fill
+// the cuFFT batch in order.  Slot b = blockIdx.y holds pair f0 + b: buf[b][i] = w_j[i] * v_c[j hop + i] (i < n), 0 for
+// n <= i < nfft and for slots past the list, read from the virtual column v_c = [history (h samples); x_c].  The window
+// of segment j is win + j wstride: the plan's one window (wstride = 0), or taper row j of a multitaper plan (hop = 0,
+// wstride = n: every taper of a channel reads the same n samples).  One slot per grid row: the pair is resolved once per
+// block, not per element.
 template <typename T, bool CPLX>
-__global__ void stft_seg_kernel(const void* __restrict__ hist_, int64_t h, int64_t ldh, const void* __restrict__ x_,
-                                int64_t nx, int64_t f0, int64_t nf, int64_t k, int64_t hop, int64_t n, int64_t nfft,
-                                const typename win_t<T>::type* __restrict__ win, void* __restrict__ buf_) {
+__global__ void seg_window_kernel(const void* __restrict__ hist_, int64_t h, int64_t ldh, const void* __restrict__ x_,
+                                  int64_t nx, int64_t f0, int64_t nf, int64_t k, int64_t hop, int64_t n, int64_t nfft,
+                                  const typename win_t<T>::type* __restrict__ win, int64_t wstride, void* __restrict__ buf_) {
     using In = typename in_type<T, CPLX>::type;
     const In* hist = reinterpret_cast<const In*>(hist_);
     const In* x = reinterpret_cast<const In*>(x_);
     const int64_t b = blockIdx.y;
     In* buf = reinterpret_cast<In*>(buf_) + b * nfft;
-    const int64_t f = f0 + b, c = f / k, t0 = (f - c * k) * hop - h;        // index in x of the segment's first sample
+    const int64_t f = f0 + b, c = f / k, j = f - c * k, t0 = j * hop - h;  // index in x of the segment's first sample
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nfft; i += (int64_t)gridDim.x * blockDim.x) {
         In v;
         if constexpr (CPLX) v = mkc<T>(T(0), T(0)); else v = T(0);
@@ -904,7 +860,7 @@ __global__ void stft_seg_kernel(const void* __restrict__ hist_, int64_t h, int64
             const int64_t t = t0 + i;
             v = t < 0 ? hist[c * ldh + h + t] : x[c * nx + t];
             if (win) {
-                const auto w = win[i];
+                const auto w = win[j * wstride + i];
                 if constexpr (CPLX) v = mkc<T>(win_mul(v.x, w), win_mul(v.y, w)); else v = win_mul(v, w);
             }
         }
@@ -932,39 +888,11 @@ __global__ void stft_store_kernel(const cx<T>* __restrict__ X, int64_t nbins_fft
     }
 }
 
-// out[i] += add[i]
-template <typename T>
-__global__ void acc_add_kernel(T* __restrict__ out, const T* __restrict__ add, int64_t n) {
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] += add[i];
-}
-
-// mt_pgram, cuFFT sizes: the (channel, taper) pairs f0 .. f0 + nf - 1 (f = c ntapers + t) fill the cuFFT batch in order.
-// Slot b = blockIdx.y holds pair f0 + b: buf[b][i] = taper row t [i] * s[c len + i] (i < n), 0 for n <= i < nfft and for slots
-// past the list -- seg_window_kernel's values under row t.
-template <typename T, bool CPLX>
-__global__ void mt_seg_kernel(const void* __restrict__ s_, int64_t len, int64_t f0, int64_t nf, int64_t ntapers, int64_t n,
-                              int64_t nfft, const typename win_t<T>::type* __restrict__ rows, void* __restrict__ buf_) {
-    using In = typename in_type<T, CPLX>::type;
-    const In* s = reinterpret_cast<const In*>(s_);
-    const int64_t b = blockIdx.y;
-    In* buf = reinterpret_cast<In*>(buf_) + b * nfft;
-    const int64_t f = f0 + b, c = f / ntapers, t = f - c * ntapers;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nfft; i += (int64_t)gridDim.x * blockDim.x) {
-        In v;
-        if constexpr (CPLX) v = mkc<T>(T(0), T(0)); else v = T(0);
-        if (b < nf && i < n) {
-            v = s[c * len + i];
-            const auto w = rows[t * n + i];
-            if constexpr (CPLX) v = mkc<T>(win_mul(v.x, w), win_mul(v.y, w)); else v = win_mul(v, w);
-        }
-        buf[i] = v;
-    }
-}
-
 // mt_pgram, cuFFT sizes: thread (bin kk, channel f0 / ntapers + blockIdx.y) adds (double)|X|^2 of its channel's slots to
 // acc (nout x nchan) one taper at a time, in taper order -- continuing the channel's sum when its first tapers were in an
-// earlier batch -- so that every channel gets pow_acc_kernel's sum over its tapers whatever the batch boundaries.  Two-sided
-// real output: bin kk >= nbins_fft reads nfft - kk.
+// earlier batch -- so that every channel gets one running sum over its tapers whatever the batch boundaries
+// (welch_stream_acc_kernel instead adds each batch's partial sum, which rounds differently).  Two-sided real output: bin
+// kk >= nbins_fft reads nfft - kk.
 template <typename T>
 __global__ void mt_pow_acc_kernel(const cx<T>* __restrict__ X, int64_t nbins_fft, int64_t nfft, int64_t nout, int64_t f0,
                                   int64_t nf, int64_t ntapers, double* __restrict__ acc) {
@@ -1143,8 +1071,8 @@ __global__ void welch_stream_acc_kernel(const cx<T>* __restrict__ X, int64_t nbi
     *q = (add || a > c * k) ? *q + sum : sum;
 }
 
-// Power of a streaming accumulation, column blockIdx.y: the fft2pow! scale (m1 = 1/r, m2 = 2/r; :142-172) of welch_finalize_kernel
-// (half: fused real plans, whose acc holds twice the power) and pow_finalize_kernel
+// Power of a Float64 accumulation, column blockIdx.y: the fft2pow! scale (m1 = 1/r, m2 = 2/r; :142-172) of welch_finalize_kernel
+// (half: fused real plans, whose acc holds twice the power); every cuFFT-size Welch and mt_pgram ends here
 template <typename T>
 __global__ void welch_stream_power_kernel(const double* __restrict__ acc, int64_t nout, int64_t nfft, int onesided, int half,
                                           double m1, double m2, T* __restrict__ out) {
@@ -1541,33 +1469,7 @@ static int generic_prepare(SpecPlanImpl* p) {
     const size_t esz = dtype_size(p->dtype);
     DSP_TRY(p->segbuf.reserve((size_t)(b * p->nfft) * esz));
     DSP_TRY(p->specbuf.reserve((size_t)(b * p->nbins_fft) * (p->f64 ? 16 : 8)));
-    DSP_TRY(p->acc.reserve((size_t)p->nbins_fft * sizeof(double)));
-    return DSPB200_OK;
-}
-
-template <typename T> static int generic_segments(SpecPlanImpl* p, const void* s, int64_t first_sample, int64_t nseg,
-                                                   cudaStream_t st) {
-    const int64_t total = p->batch * p->nfft;
-    const int threads = 256;
-    const int grid = (int)(cdiv(total, threads) < 65535 * 8 ? cdiv(total, threads) : 65535 * 8);
-    if (p->cplx)
-        seg_window_kernel<T, true><<<grid, threads, 0, st>>>(s, first_sample, p->hop, p->n, p->nfft, nseg, p->batch, reinterpret_cast<const typename win_t<T>::type*>(p->d_window), p->segbuf.p);
-    else
-        seg_window_kernel<T, false><<<grid, threads, 0, st>>>(s, first_sample, p->hop, p->n, p->nfft, nseg, p->batch, reinterpret_cast<const typename win_t<T>::type*>(p->d_window), p->segbuf.p);
-    DSP_LAUNCH_OK();
-    return fft_exec(p->fft, p->cplx, p->f64, CUFFT_FORWARD, p->segbuf.p, p->specbuf.p, st);
-}
-
-template <typename T> static int welch_generic_acc(SpecPlanImpl* p, const void* s, int64_t sample_offset,
-                                                    int64_t seg_begin, int64_t seg_end, cudaStream_t st) {
-    for (int64_t b0 = seg_begin; b0 < seg_end; b0 += p->batch) {
-        const int64_t nseg = seg_end - b0 < p->batch ? seg_end - b0 : p->batch;
-        DSP_TRY(generic_segments<T>(p, s, b0 * p->hop - sample_offset, nseg, st));
-        const int threads = 128;
-        pow_acc_kernel<T><<<(int)cdiv(p->nbins_fft, threads), threads, 0, st>>>(
-            reinterpret_cast<const cx<T>*>(p->specbuf.p), p->nbins_fft, nseg, reinterpret_cast<double*>(p->acc.p));
-        DSP_LAUNCH_OK();
-    }
+    DSP_TRY(p->acc.reserve((size_t)p->nout * sizeof(double)));
     return DSPB200_OK;
 }
 
@@ -1577,18 +1479,26 @@ static unsigned stream_generic_cols(const SpecPlanImpl* p, int64_t len, int thre
     return (unsigned)(want < cap ? want : cap);
 }
 
-// The spectra of (channel, segment) pairs f0 .. f0 + nf - 1 of the virtual columns [hist; x] (f = c k + j) in the plan's
-// batch buffer: stft_seg_kernel, then the plan's cuFFT transform
-template <typename T> static int stream_generic_fft(SpecPlanImpl* p, const void* hist, int64_t h, int64_t ldh, const void* x,
-                                                     int64_t nx, int64_t f0, int64_t nf, int64_t k, cudaStream_t st) {
-    const int threads = 256;
+// seg_window_kernel of the plan's element type (T: its real type) into buf, 256 threads per block
+template <typename T> static int seg_window_launch(const SpecPlanImpl* p, dim3 grid, const void* hist, int64_t h, int64_t ldh,
+                                                    const void* x, int64_t nx, int64_t f0, int64_t nf, int64_t k, int64_t hop,
+                                                    int64_t wstride, void* buf, cudaStream_t st) {
     const auto* w = reinterpret_cast<const typename win_t<T>::type*>(p->d_window);
-    const dim3 gseg(stream_generic_cols(p, p->nfft, threads), (unsigned)p->batch);
     if (p->cplx)
-        stft_seg_kernel<T, true><<<gseg, threads, 0, st>>>(hist, h, ldh, x, nx, f0, nf, k, p->hop, p->n, p->nfft, w, p->segbuf.p);
+        seg_window_kernel<T, true><<<grid, 256, 0, st>>>(hist, h, ldh, x, nx, f0, nf, k, hop, p->n, p->nfft, w, wstride, buf);
     else
-        stft_seg_kernel<T, false><<<gseg, threads, 0, st>>>(hist, h, ldh, x, nx, f0, nf, k, p->hop, p->n, p->nfft, w, p->segbuf.p);
+        seg_window_kernel<T, false><<<grid, 256, 0, st>>>(hist, h, ldh, x, nx, f0, nf, k, hop, p->n, p->nfft, w, wstride, buf);
     DSP_LAUNCH_OK();
+    return DSPB200_OK;
+}
+
+// The spectra of (channel, segment) pairs f0 .. f0 + nf - 1 of the virtual columns [hist; x] (f = c k + j) in the plan's
+// batch buffer: seg_window_kernel (segments hop samples apart, windows wstride values apart), then the plan's cuFFT transform
+template <typename T> static int stream_generic_fft(SpecPlanImpl* p, const void* hist, int64_t h, int64_t ldh, const void* x,
+                                                     int64_t nx, int64_t f0, int64_t nf, int64_t k, int64_t hop,
+                                                     int64_t wstride, cudaStream_t st) {
+    const dim3 gseg(stream_generic_cols(p, p->nfft, 256), (unsigned)p->batch);
+    DSP_TRY(seg_window_launch<T>(p, gseg, hist, h, ldh, x, nx, f0, nf, k, hop, wstride, p->segbuf.p, st));
     return fft_exec(p->fft, p->cplx, p->f64, CUFFT_FORWARD, p->segbuf.p, p->specbuf.p, st);
 }
 
@@ -1599,35 +1509,11 @@ template <typename T> static int stft_generic(SpecPlanImpl* p, const StftStreamA
     const int threads = 256;
     for (int64_t f0 = 0; f0 < pairs; f0 += p->batch) {
         const int64_t nf = pairs - f0 < p->batch ? pairs - f0 : p->batch;
-        DSP_TRY(stream_generic_fft<T>(p, sa.hist, sa.h, sa.ldh, x, nx, f0, nf, k, st));
+        DSP_TRY(stream_generic_fft<T>(p, sa.hist, sa.h, sa.ldh, x, nx, f0, nf, k, p->hop, 0, st));
         const dim3 gout(stream_generic_cols(p, p->nout, threads), (unsigned)nf);
         stft_store_kernel<T><<<gout, threads, 0, st>>>(reinterpret_cast<const cx<T>*>(p->specbuf.p), p->nbins_fft, p->nfft,
                                                        p->nout, f0, k, sa.ldo, psd_only, p->onesided, (T)(1.0 / r), (T)(2.0 / r),
                                                        out);
-        DSP_LAUNCH_OK();
-    }
-    return DSPB200_OK;
-}
-
-// cuFFT sizes of the batched Welch: one channel after another through the generic segment / FFT / power kernels, into the
-// batch's own Float64 accumulator
-template <typename T> static int welch_batch_generic(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan, int64_t k,
-                                                      double r, void* out, cudaStream_t st) {
-    DSP_TRY(p->bacc.reserve((size_t)p->nbins_fft * sizeof(double)));
-    double* acc = reinterpret_cast<double*>(p->bacc.p);
-    for (int64_t c = 0; c < nchan; ++c) {
-        DSP_CUDA(cudaMemsetAsync(acc, 0, (size_t)p->nbins_fft * sizeof(double), st));
-        for (int64_t b0 = 0; b0 < k; b0 += p->batch) {
-            const int64_t nseg = k - b0 < p->batch ? k - b0 : p->batch;
-            DSP_TRY(generic_segments<T>(p, s, c * len + b0 * p->hop, nseg, st));
-            const int threads = 128;
-            pow_acc_kernel<T><<<(int)cdiv(p->nbins_fft, threads), threads, 0, st>>>(
-                reinterpret_cast<const cx<T>*>(p->specbuf.p), p->nbins_fft, nseg, acc);
-            DSP_LAUNCH_OK();
-        }
-        const int threads = 128;
-        pow_finalize_kernel<T><<<(int)cdiv(p->nout, threads), threads, 0, st>>>(acc, p->nbins_fft, p->nfft, p->nout, p->onesided,
-                                                                                1.0 / r, 2.0 / r, reinterpret_cast<T*>(out) + c * p->nout);
         DSP_LAUNCH_OK();
     }
     return DSPB200_OK;
@@ -1714,8 +1600,8 @@ static int welch_stream_fused(SpecPlanImpl* p, const StreamSeam& sm, const void*
     return DSPB200_OK;
 }
 
-// Streaming Welch, cuFFT sizes: the nchan x k (channel, segment) pairs of the virtual columns through the plan's batch, three
-// launches per batch
+// Welch, cuFFT sizes: the nchan x k (channel, segment) pairs of the virtual columns through the plan's batch, three launches
+// per batch.  Streaming calls, and every other Welch form as one channel with no history.
 template <typename T> static int welch_stream_generic(SpecPlanImpl* p, const void* hist, int64_t h, int64_t ldh, const void* x,
                                                        int64_t nx, int64_t nchan, int64_t k, double* acc, int add,
                                                        cudaStream_t st) {
@@ -1723,11 +1609,52 @@ template <typename T> static int welch_stream_generic(SpecPlanImpl* p, const voi
     const int threads = 128;
     for (int64_t f0 = 0; f0 < pairs; f0 += p->batch) {
         const int64_t nf = pairs - f0 < p->batch ? pairs - f0 : p->batch;
-        DSP_TRY(stream_generic_fft<T>(p, hist, h, ldh, x, nx, f0, nf, k, st));
+        DSP_TRY(stream_generic_fft<T>(p, hist, h, ldh, x, nx, f0, nf, k, p->hop, 0, st));
         const int64_t nc = (f0 + nf - 1) / k - f0 / k + 1;                  // channels with a pair in this batch
         welch_stream_acc_kernel<T><<<dim3((unsigned)cdiv(p->nout, threads), (unsigned)nc), threads, 0, st>>>(
             reinterpret_cast<const cx<T>*>(p->specbuf.p), p->nbins_fft, p->nfft, p->nout, f0, nf, k, add, acc);
         DSP_LAUNCH_OK();
+    }
+    return DSPB200_OK;
+}
+
+static int welch_generic(SpecPlanImpl* p, const void* hist, int64_t h, int64_t ldh, const void* x, int64_t nx, int64_t nchan,
+                         int64_t k, double* acc, int add, cudaStream_t st) {
+    DSP_TRY(generic_prepare(p));
+    return p->f64 ? welch_stream_generic<double>(p, hist, h, ldh, x, nx, nchan, k, acc, add, st)
+                  : welch_stream_generic<float>(p, hist, h, ldh, x, nx, nchan, k, acc, add, st);
+}
+
+// The PSD of the nout x nchan Float64 accumulator acc (welch_stream_power_kernel, up to 65535 channels per launch)
+static int welch_power(const SpecPlanImpl* p, const double* acc, int64_t nchan, double r, void* out, cudaStream_t st) {
+    const int threads = 128;
+    const int half = p->fused && !p->cplx;
+    for (int64_t c0 = 0; c0 < nchan; c0 += 65535) {
+        const int64_t gc = nchan - c0 < 65535 ? nchan - c0 : 65535;
+        const dim3 grid((unsigned)cdiv(p->nout, threads), (unsigned)gc);
+        if (p->f64)
+            welch_stream_power_kernel<double><<<grid, threads, 0, st>>>(acc + c0 * p->nout, p->nout, p->nfft, p->onesided, half,
+                                                                       1.0 / r, 2.0 / r, (double*)out + c0 * p->nout);
+        else
+            welch_stream_power_kernel<float><<<grid, threads, 0, st>>>(acc + c0 * p->nout, p->nout, p->nfft, p->onesided, half,
+                                                                      1.0 / r, 2.0 / r, (float*)out + c0 * p->nout);
+        DSP_LAUNCH_OK();
+    }
+    return DSPB200_OK;
+}
+
+// Batched Welch, cuFFT sizes: channel after channel, each written (add = 0) into the batch's own accumulator -- an
+// accumulation open on the plan (acc) is left as it was -- and scaled into its column.  The channels are not packed into
+// shared cuFFT batches (as a stream packs them): a channel's batch boundaries would then depend on the channels before it,
+// and its sum would round differently from the vector call's.
+static int welch_batch_generic(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan, int64_t k, double r, void* out,
+                               cudaStream_t st) {
+    DSP_TRY(p->bacc.reserve((size_t)p->nout * sizeof(double)));
+    double* acc = reinterpret_cast<double*>(p->bacc.p);
+    const size_t esz = dtype_size(p->dtype), osz = p->f64 ? 8 : 4;
+    for (int64_t c = 0; c < nchan; ++c) {
+        DSP_TRY(welch_generic(p, nullptr, 0, 0, (const char*)s + (size_t)(c * len) * esz, len, 1, k, acc, 0, st));
+        DSP_TRY(welch_power(p, acc, 1, r, (char*)out + (size_t)(c * p->nout) * osz, st));
     }
     return DSPB200_OK;
 }
@@ -1738,7 +1665,7 @@ static int welch_begin(SpecPlanImpl* p, cudaStream_t st) {
         p->rows_used = 0;            // the first launch writes its rows, later ones add (welch_fused_kernel, `fresh_from`)
     } else {
         DSP_TRY(generic_prepare(p));
-        DSP_CUDA(cudaMemsetAsync(p->acc.p, 0, (size_t)p->nbins_fft * sizeof(double), st));
+        DSP_CUDA(cudaMemsetAsync(p->acc.p, 0, (size_t)p->nout * sizeof(double), st));
     }
     return DSPB200_OK;
 }
@@ -1754,21 +1681,17 @@ static int welch_accumulate(SpecPlanImpl* p, const void* s, int64_t sample_offse
                            : launch_welch_fused<T, N, false>(p, s, seg_begin, seg_end - seg_begin, sample_offset, st);
         });
     }
-    return p->f64 ? welch_generic_acc<double>(p, s, sample_offset, seg_begin, seg_end, st)
-                  : welch_generic_acc<float>(p, s, sample_offset, seg_begin, seg_end, st);
+    // one channel, no history, its first segment at x[0] (welch_range_check: seg_begin hop >= sample_offset), added to acc;
+    // the channel's column stride is never read
+    const int64_t first = seg_begin * p->hop - sample_offset;
+    return welch_generic(p, nullptr, 0, 0, (const char*)s + (size_t)first * dtype_size(p->dtype), 0, 1, seg_end - seg_begin,
+                         reinterpret_cast<double*>(p->acc.p), 1, st);
 }
 
 static int welch_finalize(SpecPlanImpl* p, double r, void* out, cudaStream_t st) {
     if (p->fused)
         return fused_dispatch(p, "Welch", [&](auto t, auto nn) { return launch_welch_finalize<decltype(t), decltype(nn)::value>(p, r, out, st); });
-    const int threads = 128;
-    const int grid = (int)cdiv(p->nout, threads);
-    if (p->f64)
-        pow_finalize_kernel<double><<<grid, threads, 0, st>>>((const double*)p->acc.p, p->nbins_fft, p->nfft, p->nout, p->onesided, 1.0 / r, 2.0 / r, (double*)out);
-    else
-        pow_finalize_kernel<float><<<grid, threads, 0, st>>>((const double*)p->acc.p, p->nbins_fft, p->nfft, p->nout, p->onesided, 1.0 / r, 2.0 / r, (float*)out);
-    DSP_LAUNCH_OK();
-    return DSPB200_OK;
+    return welch_power(p, reinterpret_cast<const double*>(p->acc.p), 1, r, out, st);
 }
 
 static int64_t nsegments(const SpecPlanImpl* p, int64_t len) {
@@ -1859,33 +1782,24 @@ static int launch_mt_pgram(SpecPlanImpl* p, const void* s, int64_t len, int64_t 
     return DSPB200_OK;
 }
 
-// mt_pgram, cuFFT sizes: the nchan x ntapers (channel, taper) pairs through the plan's batch -- mt_seg_kernel, cuFFT,
-// mt_pow_acc_kernel: three launches per batch -- into a Float64 nout x nchan accumulator, then the fft2pow! scaling (r = 1)
-// of welch_stream_power_kernel, which rounds as pow_finalize_kernel does.
-template <typename T> static int mt_pgram_generic(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, void* out,
+// mt_pgram, cuFFT sizes: the nchan x ntapers (channel, taper) pairs through the plan's batch -- seg_window_kernel (pair
+// (c, t): channel c's n samples under taper row t), cuFFT, mt_pow_acc_kernel: three launches per batch -- into a Float64
+// nout x nchan accumulator, then the fft2pow! scaling (r = 1) of welch_power.
+template <typename T> static int mt_pgram_generic(SpecPlanImpl* p, const void* s, int64_t len, int64_t nchan, void* out,
                                                    cudaStream_t st) {
-    SpecPlanImpl* p = &plan->impl;
     DSP_TRY(generic_prepare(p));
     DSP_TRY(p->bacc.reserve((size_t)(p->nout * nchan) * sizeof(double)));
     double* acc = reinterpret_cast<double*>(p->bacc.p);
-    const auto* rows = reinterpret_cast<const typename win_t<T>::type*>(p->d_window);
     const int64_t nt = p->ntapers, pairs = nchan * nt;
-    const int threads = 256;
     for (int64_t f0 = 0; f0 < pairs; f0 += p->batch) {
         const int64_t nf = pairs - f0 < p->batch ? pairs - f0 : p->batch;
-        const dim3 gseg(stream_generic_cols(p, p->nfft, threads), (unsigned)p->batch);
-        if (p->cplx)
-            mt_seg_kernel<T, true><<<gseg, threads, 0, st>>>(s, len, f0, nf, nt, p->n, p->nfft, rows, p->segbuf.p);
-        else
-            mt_seg_kernel<T, false><<<gseg, threads, 0, st>>>(s, len, f0, nf, nt, p->n, p->nfft, rows, p->segbuf.p);
-        DSP_LAUNCH_OK();
-        DSP_TRY(fft_exec(p->fft, p->cplx, p->f64, CUFFT_FORWARD, p->segbuf.p, p->specbuf.p, st));
+        DSP_TRY(stream_generic_fft<T>(p, nullptr, 0, 0, s, len, f0, nf, nt, 0, p->n, st));
         const int64_t nc = (f0 + nf - 1) / nt - f0 / nt + 1;                 // channels with a pair in this batch
         mt_pow_acc_kernel<T><<<dim3((unsigned)cdiv(p->nout, 128), (unsigned)nc), 128, 0, st>>>(
             reinterpret_cast<const cx<T>*>(p->specbuf.p), p->nbins_fft, p->nfft, p->nout, f0, nf, nt, acc);
         DSP_LAUNCH_OK();
     }
-    return dspb200_welch_stream_power_dev(plan, acc, nchan, 1.0, out, st);
+    return welch_power(p, acc, nchan, 1.0, out, st);
 }
 
 // periodogram(s::AbstractMatrix; nfft, fs, radialsum, radialavg), src/periodograms.jl:473-509, device pointers: queues the
@@ -2160,9 +2074,7 @@ int dspb200_welch_batch_exec_dev(dspb200_spec_plan* plan, const void* s, int64_t
             return p->cplx ? launch_welch_batch<T, N, true>(p, s, len, nchan, k, r, out, st)
                            : launch_welch_batch<T, N, false>(p, s, len, nchan, k, r, out, st);
         });
-    DSP_TRY(generic_prepare(p));
-    return p->f64 ? welch_batch_generic<double>(p, s, len, nchan, k, r, out, st)
-                  : welch_batch_generic<float>(p, s, len, nchan, k, r, out, st);
+    return welch_batch_generic(p, s, len, nchan, k, r, out, st);
 }
 
 int dspb200_welch_batch_exec(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, double r, void* out) {
@@ -2270,15 +2182,14 @@ int dspb200_arraysplit_exec(dspb200_spec_plan* plan, const void* s, int64_t len,
     DSP_TRY(ensure_streams(p));
     const size_t esz = dtype_size(p->dtype);
     return run_staged(p->pipe.s_exec, {{s, (size_t)len * esz, &p->pipe.in[0]}}, {{out, (size_t)(k * p->nfft) * esz, &p->pipe.out[0]}}, [&]() -> int {
-        const int64_t total = k * p->nfft;
-        const int threads = 256;
-        const int grid = (int)(cdiv(total, threads) < 65535 * 8 ? cdiv(total, threads) : 65535 * 8);
-#define SEGK(T_, C_) seg_window_kernel<T_, C_><<<grid, threads, 0, p->pipe.s_exec>>>(p->pipe.in[0].p, 0, p->hop, p->n, p->nfft, k, k, \
-        reinterpret_cast<const typename win_t<T_>::type*>(p->d_window), p->pipe.out[0].p)
-        if (p->f64) { if (p->cplx) SEGK(double, true); else SEGK(double, false); }
-        else { if (p->cplx) SEGK(float, true); else SEGK(float, false); }
-#undef SEGK
-        DSP_LAUNCH_OK();
+        // one channel, no history; segment f in row f - f0 of a launch of at most 65535 grid rows
+        for (int64_t f0 = 0; f0 < k; f0 += 65535) {
+            const int64_t nf = k - f0 < 65535 ? k - f0 : 65535;
+            const dim3 grid((unsigned)cdiv(p->nfft, 256), (unsigned)nf);
+            void* buf = (char*)p->pipe.out[0].p + (size_t)(f0 * p->nfft) * esz;
+            DSP_TRY(p->f64 ? seg_window_launch<double>(p, grid, nullptr, 0, 0, p->pipe.in[0].p, len, f0, nf, k, p->hop, 0, buf, p->pipe.s_exec)
+                           : seg_window_launch<float>(p, grid, nullptr, 0, 0, p->pipe.in[0].p, len, f0, nf, k, p->hop, 0, buf, p->pipe.s_exec));
+        }
         return DSPB200_OK;
     });
 }
@@ -2385,8 +2296,8 @@ __global__ void acc_add_cols_kernel(T* __restrict__ out, int64_t ldc, const T* _
     }
 }
 
-// Streaming mt_spectrogram, cuFFT sizes, in the order of the one-shot call (mt_spectrogram_queue): taper 0's PSD columns
-// into out, every later taper's into the plan's scratch and then added to out, each through the generic stream STFT
+// mt_spectrogram, cuFFT sizes, one-shot (no history in sa) or streaming: taper 0's PSD columns into out, every later taper's
+// into the plan's scratch and then added to out, each through the generic stream STFT
 template <typename T>
 static int mt_stream_generic(SpecPlanImpl* p, const StftStreamArgs& sa, const void* x, int64_t nx, int64_t nchan, int64_t nseg,
                              void* out, cudaStream_t st) {
@@ -2498,9 +2409,7 @@ int dspb200_welch_stream_exec_dev(dspb200_spec_plan* plan, const void* hist_in, 
             return p->cplx ? welch_stream_fused<T, N, true>(p, sm, x, nx, nhist, nchan, nseg, acc, add, st)
                            : welch_stream_fused<T, N, false>(p, sm, x, nx, nhist, nchan, nseg, acc, add, st);
         });
-    DSP_TRY(generic_prepare(p));
-    return p->f64 ? welch_stream_generic<double>(p, hist_in, nhist, ldh, x, nx, nchan, nseg, acc, add, st)
-                  : welch_stream_generic<float>(p, hist_in, nhist, ldh, x, nx, nchan, nseg, acc, add, st);
+    return welch_generic(p, hist_in, nhist, ldh, x, nx, nchan, nseg, acc, add, st);
 }
 
 // Host twin (returns when the work is done): the chunk, the histories and acc are staged
@@ -2533,21 +2442,7 @@ int dspb200_welch_stream_power_dev(dspb200_spec_plan* plan, const double* acc, i
     DSP_REQUIRE(acc && out, "NULL argument");
     DSP_REQUIRE(!ranges_overlap(out, (size_t)(p->nout * nchan) * (p->f64 ? 8 : 4), acc, (size_t)(p->nout * nchan) * sizeof(double)),
                 "out overlaps acc");
-    cudaStream_t st = (cudaStream_t)stream;
-    const int threads = 128;
-    const int half = p->fused && !p->cplx;
-    for (int64_t c0 = 0; c0 < nchan; c0 += 65535) {
-        const int64_t gc = nchan - c0 < 65535 ? nchan - c0 : 65535;
-        const dim3 grid((unsigned)cdiv(p->nout, threads), (unsigned)gc);
-        if (p->f64)
-            welch_stream_power_kernel<double><<<grid, threads, 0, st>>>(acc + c0 * p->nout, p->nout, p->nfft, p->onesided, half,
-                                                                       1.0 / r, 2.0 / r, (double*)out + c0 * p->nout);
-        else
-            welch_stream_power_kernel<float><<<grid, threads, 0, st>>>(acc + c0 * p->nout, p->nout, p->nfft, p->onesided, half,
-                                                                      1.0 / r, 2.0 / r, (float*)out + c0 * p->nout);
-        DSP_LAUNCH_OK();
-    }
-    return DSPB200_OK;
+    return welch_power(p, acc, nchan, r, out, (cudaStream_t)stream);
 }
 
 int dspb200_welch_stream_power(dspb200_spec_plan* plan, const double* acc, int64_t nchan, double r, void* out) {
@@ -2571,9 +2466,10 @@ int dspb200_welch_stream_power(dspb200_spec_plan* plan, const double* acc, int64
 //   mt_spectrogram = sum_t spectrogram(s; window = w_t, r = 1)
 // of each of the nchan columns of a len x nchan matrix, every channel's tapers summed in taper order (the vector forms are
 // nchan = 1).  Fused sizes: mt_pgram is launch_mt_pgram (two launches per channel group), mt_spectrogram ONE launch of the
-// STFT kernels' taper-row instances (WIN == 2).  cuFFT sizes: mt_pgram_generic; mt_spectrogram is one batched STFT over all
-// channels per taper, each after the first followed by acc_add_kernel.  A stream of mt_spectrogram is the STFT stream call on
-// a multitaper plan (dspb200_stft_stream_exec_dev: the same WIN == 2 launch, or mt_stream_generic).
+// STFT kernels' taper-row instances (WIN == 2).  cuFFT sizes: mt_pgram_generic; mt_spectrogram is mt_stream_generic with no
+// history (one batched STFT over all channels per taper, each after the first followed by acc_add_cols_kernel).  A stream of
+// mt_spectrogram is the STFT stream call on a multitaper plan (dspb200_stft_stream_exec_dev: the same WIN == 2 launch, or
+// mt_stream_generic).
 static size_t mt_out_bytes(const SpecPlanImpl* p, int64_t nchan, int64_t k) {
     return (size_t)(p->nout * k * nchan) * (p->f64 ? 8 : 4);
 }
@@ -2605,30 +2501,19 @@ static int mt_pgram_queue(dspb200_spec_plan* plan, const void* s, int64_t len, i
             constexpr int N = decltype(nn)::value;
             return p->cplx ? launch_mt_pgram<T, N, true>(p, s, len, nchan, out, st) : launch_mt_pgram<T, N, false>(p, s, len, nchan, out, st);
         });
-    return p->f64 ? mt_pgram_generic<double>(plan, s, len, nchan, out, st) : mt_pgram_generic<float>(plan, s, len, nchan, out, st);
+    return p->f64 ? mt_pgram_generic<double>(p, s, len, nchan, out, st) : mt_pgram_generic<float>(p, s, len, nchan, out, st);
 }
 
 static int mt_spectrogram_queue(dspb200_spec_plan* plan, const void* s, int64_t len, int64_t nchan, int64_t k, void* out,
                                 cudaStream_t st) {
     SpecPlanImpl* p = &plan->impl;
-    if (p->fused) {
-        StftStreamArgs sa;                               // no history; columns k apart; every taper row in the one launch
-        sa.ldo = k;
-        sa.ntapers = (int)p->ntapers;
-        return stft_launch(p, sa, s, len, nchan, k, 1.0, 1, out, st);
-    }
-    const int64_t cnt = p->nout * k * nchan;
-    DSP_TRY(p->tmp.reserve((size_t)cnt * (p->f64 ? 8 : 4)));
-    return for_each_taper(p, [&](int64_t t) -> int {
-        DSP_TRY(dspb200_stft_exec_dev(plan, s, len, nchan, 1.0, 1, t == 0 ? out : p->tmp.p, st));
-        if (t == 0) return DSPB200_OK;
-        const int threads = 256;
-        const int grid = (int)(cdiv(cnt, threads) < device_sm_count() * 32 ? cdiv(cnt, threads) : device_sm_count() * 32);
-        if (p->f64) acc_add_kernel<double><<<grid, threads, 0, st>>>((double*)out, (const double*)p->tmp.p, cnt);
-        else acc_add_kernel<float><<<grid, threads, 0, st>>>((float*)out, (const float*)p->tmp.p, cnt);
-        DSP_LAUNCH_OK();
-        return DSPB200_OK;
-    });
+    StftStreamArgs sa;                                   // no history; columns k apart
+    sa.ldo = k;
+    if (!p->fused)
+        return p->f64 ? mt_stream_generic<double>(p, sa, s, len, nchan, k, out, st)
+                      : mt_stream_generic<float>(p, sa, s, len, nchan, k, out, st);
+    sa.ntapers = (int)p->ntapers;                        // every taper row in the one launch
+    return stft_launch(p, sa, s, len, nchan, k, 1.0, 1, out, st);
 }
 
 int dspb200_mt_pgram_batch_exec_dev(dspb200_spec_plan* plan, const void* d_s, int64_t len, int64_t nchan, void* d_out,

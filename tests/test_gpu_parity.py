@@ -533,6 +533,13 @@ def test_arraysplit_and_fftshift():
         relerr(dsp.arraysplit(x, 512, 384, 1024, w), op.arraysplit(x, 512, 384, 1024, w)) < 1e-7
     with pytest.raises(dsp.DomainError):
         dsp.arraysplit(np.ones(10), 4, 4)
+    # more than 65535 segments: several launches of up to 65535 segments each, on a cuFFT-size and a fused plan.  The
+    # window is exact in Float32, so the oracle's Float64 product rounded once is the kernel's product.
+    x = randn(600000, np.float32)
+    for n, noverlap, nfft in ((16, 8, None), (64, 56, 256)):
+        w = dsp.hanning(n).astype(np.float32).astype(np.float64)
+        q = dsp.arraysplit(x, n, noverlap, nfft, w)
+        assert q.shape[0] > 65535 and np.array_equal(q, op.arraysplit(x, n, noverlap, nfft, w, f64=False))
     # test/periodograms.jl:239-248
     p = dsp.periodogram(DATA)
     ps = dsp.fftshift(p)

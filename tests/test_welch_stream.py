@@ -285,6 +285,30 @@ def test_one_chunk_in_channel_groups():
     check_welch(got, x, N, N // 2, N, True, dsp.hanning, 3, "groups")
 
 
+CUFFT_ONE = [(F32, 1000, 1000), (F64, 300, 320), (C128, 20000, 24000)]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("dt,n,nfft", CUFFT_ONE, ids=[f"{d.name}-{n}-{N}" for d, n, N in CUFFT_ONE])
+def test_one_chunk_is_bit_identical_to_welch_pgram_at_cufft_sizes(dt, n, nfft):
+    # one channel, more segments than one cuFFT batch: the stream and welch_pgram of the device vector (and of the one-column
+    # matrix) run the same segment list through the same batches.  Not so for several channels: the stream packs the
+    # channels' segments into shared batches.
+    from test_spectral_kernel_paths import generic_batch
+    rng = np.random.default_rng(nfft)
+    hop = n - n // 2
+    k = generic_batch(nfft) + 3
+    length = (k - 1) * hop + n + 7
+    x = _signal(rng, (length, 1), dt)
+    for onesided in ((None, False) if dt.kind == "f" else (None,)):
+        kw = dict(n=n, noverlap=n // 2, nfft=nfft, window=dsp.hanning, onesided=onesided)
+        got, s, _ = _stream(x, [length], **kw)
+        assert s.nsegments == k
+        vec = dsp.welch_pgram(dsp.to_device(np.ascontiguousarray(x[:, 0])), **kw).power
+        assert _same(got[:, 0], vec), (dt, n, nfft, onesided)
+        assert _same(got, _oneshot(x, **kw)), (dt, n, nfft, onesided)
+
+
 # =============================================================================== GPU: many chunks, within the bound
 
 def _units(kc, dt):
