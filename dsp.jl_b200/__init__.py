@@ -11,7 +11,9 @@ the same thin layer over the same C ABI, include/dspb200.h):
     WelchStream (an extension: welch_pgram of a chunked multichannel stream)
                                                                        (src/periodograms.jl)
     MTConfig, MTSpectrogramConfig, mt_pgram, mt_spectrogram, mt_spectrogram_, allocate_output, MTSpectrogramStream (an
-    extension: mt_spectrogram of a chunked multichannel stream), mt_cross_power_spectra, mt_coherence
+    extension: mt_spectrogram of a chunked multichannel stream), MTCrossSpectraConfig, MTCoherenceConfig,
+    mt_cross_power_spectra, mt_cross_power_spectra_, mt_coherence, mt_coherence_ (and, an extension, their epoch means
+    over an n_channels x n_samples x n_epochs signal)
                                                                        (src/multitaper.jl)
     hanning, hamming, rect, bartlett, kaiser, nextfastfft              (src/windows.jl, src/util.jl)
 
@@ -33,9 +35,9 @@ from .filters import filt_ as filt_hx_
 from .periodograms import (Periodogram, Periodogram2, Spectrogram, STFTStream, WelchConfig, WelchStream, arraysplit, arraysplit_count, compute_window, fftshift,
                            filt_welch, freq, periodogram, power, spectrogram, stft, time, welch_pgram, welch_pgram_)
 
-from .multitaper import (Coherence, CrossPowerSpectra, MTConfig, MTCrossSpectraConfig, MTSpectrogramConfig, MTSpectrogramStream,
-                         allocate_output, dpss, dpss_config, dpsseig, mt_coherence, mt_cross_power_spectra, mt_pgram,
-                         mt_spectrogram, mt_spectrogram_)
+from .multitaper import (Coherence, CrossPowerSpectra, MTCoherenceConfig, MTConfig, MTCrossSpectraConfig, MTSpectrogramConfig,
+                         MTSpectrogramStream, allocate_output, dpss, dpss_config, dpsseig, mt_coherence, mt_coherence_,
+                         mt_cross_power_spectra, mt_cross_power_spectra_, mt_pgram, mt_spectrogram, mt_spectrogram_)
 from .clients import alignsignals, filtfilt, finddelay, hilbert, shiftsignal, xcorr
 from . import device, filters, sharding
 

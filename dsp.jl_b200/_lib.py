@@ -116,6 +116,8 @@ SIGNATURES = {
     "dspb200_mt_spectrogram_batch_exec_dev": (_int, [_vp, _vp, _i64, _i64, _vp, _vp]),
     "dspb200_mt_cross_spectra_exec": (_int, [_vp, _vp, _i64, _int, _i64, _i64, _int, _vp]),
     "dspb200_mt_cross_spectra_exec_dev": (_int, [_vp, _vp, _i64, _int, _i64, _i64, _int, _vp, _vp]),
+    "dspb200_mt_cross_spectra_epochs": (_int, [_vp, _vp, _i64, _i64, _int, _i64, _i64, _int, _vp, _vp]),
+    "dspb200_mt_cross_spectra_epochs_exec": (_int, [_vp, _vp, _i64, _i64, _int, _i64, _i64, _int, _vp]),
     "dspb200_spec_plan_destroy": (_int, [_vp]),
     "dspb200_resample_plan_create": (_int, [_pp, _int, _int, _vp, _i64, _i64, _i64]),
     "dspb200_resample_out_dtype": (_int, [_vp, C.POINTER(_int)]),
@@ -398,6 +400,14 @@ class MtPlan(SpecPlan):
     def cross_spectra(self, signal, nchan, demean, f_lo, nf, coherence, out):
         check(lib.dspb200_mt_cross_spectra_exec(self.handle, ptr(signal), int(nchan), 1 if demean else 0, int(f_lo), int(nf),
                                                 1 if coherence else 0, ptr(out)))
+
+    def cross_spectra_epochs_dev(self, signal_ptr, nchan, nepochs, demean, f_lo, nf, coherence, out_ptr, stream=0):
+        check(lib.dspb200_mt_cross_spectra_epochs(self.handle, signal_ptr, int(nchan), int(nepochs), 1 if demean else 0, int(f_lo),
+                                                  int(nf), 1 if coherence else 0, out_ptr, stream))
+
+    def cross_spectra_epochs(self, signal, nchan, nepochs, demean, f_lo, nf, coherence, out):
+        check(lib.dspb200_mt_cross_spectra_epochs_exec(self.handle, ptr(signal), int(nchan), int(nepochs), 1 if demean else 0,
+                                                       int(f_lo), int(nf), 1 if coherence else 0, ptr(out)))
 
 
 class ResamplePlan(_Plan):

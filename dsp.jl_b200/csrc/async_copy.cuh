@@ -1,5 +1,5 @@
-// dspb200 -- TMA bulk (1-D) global -> shared copies completed through an mbarrier (sm_90a PTX).
-// SASS: UBLKCP (cp.async.bulk), SYNCS.ARRIVE.TRANS64 (expect_tx), SYNCS.PHASECHK.TRANS64.TRYWAIT (try_wait).
+// dspb200 -- TMA bulk (1-D) global -> shared copies completed through an mbarrier, and per-thread cp.async copies (sm_90a
+// PTX).  SASS: UBLKCP (cp.async.bulk), SYNCS.ARRIVE.TRANS64 (expect_tx), SYNCS.PHASECHK.TRANS64.TRYWAIT (try_wait), LDGSTS.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -38,6 +38,16 @@ __device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gmem_src
 __device__ __forceinline__ void tma_prefetch_l2(const void* gmem_src, uint32_t bytes) {
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gmem_src), "r"(bytes) : "memory");
 }
+
+// Per-thread asynchronous copies (cp.async, LDGSTS) of one naturally aligned 8- or 16-byte element: for staging tiles whose
+// rows start at any element, where a bulk copy's 16-byte alignment does not hold.  cp_async_commit closes the calling
+// thread's group of copies; cp_async_wait<N> waits until at most N of its groups are still in flight.
+template <int BYTES> __device__ __forceinline__ void cp_async(void* smem_dst, const void* gmem_src) {
+    static_assert(BYTES == 8 || BYTES == 16, "cp.async.ca copies 4, 8 or 16 bytes");
+    asm volatile("cp.async.ca.shared.global [%0], [%1], %2;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "n"(BYTES) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     asm volatile(

@@ -908,11 +908,14 @@ __global__ void mt_pow_acc_kernel(const cx<T>* __restrict__ X, int64_t nbins_fft
 }
 
 // Multitaper cross spectra (src/multitaper.jl:553-616).
-// signal is the reference's n_channels x n_samples matrix (channel index fastest); xs gets one contiguous column per
-// channel, minus the channel mean when `demean` (:566-570).  One block per channel.
+// signal is an n_channels x n_samples x n_epochs array (channel index fastest; one epoch: the reference's matrix); xs gets
+// one contiguous column per (channel, epoch), column e nchan + c, minus that column's mean when `demean` (:566-570).  One
+// block per column.
 template <typename T>
 __global__ void cs_prep_kernel(const T* __restrict__ signal, int64_t nchan, int64_t n, int demean, T* __restrict__ xs) {
-    const int64_t c = blockIdx.x;
+    const int64_t col = blockIdx.x, c = col % nchan;
+    signal += (col / nchan) * nchan * n;
+    xs += col * n;
     __shared__ double red[32];
     __shared__ T mean_s;
     double acc = 0.0;
@@ -930,22 +933,130 @@ __global__ void cs_prep_kernel(const T* __restrict__ signal, int64_t nchan, int6
         __syncthreads();
     }
     const T mu = demean ? mean_s : T(0);
-    for (int64_t i = threadIdx.x; i < n; i += blockDim.x) xs[i + n * c] = signal[c + nchan * i] - mu;
+    for (int64_t i = threadIdx.x; i < n; i += blockDim.x) xs[i] = signal[c + nchan * i] - mu;
 }
 
-// out[l, m, fi] += c_f * x[f, l] * conj(x[f, m]), f = f_lo + fi; x = spectra of ONE taper (rows pre-scaled by
-// 1/sqrt(r_t), so the reference's weight 2/r_t and its 1/sqrt(2) on the DC / Nyquist rows become c_f = 2, or 1 there)
+__device__ __forceinline__ float fma_rn(float a, float b, float c) { return __fmaf_rn(a, b, c); }
+__device__ __forceinline__ double fma_rn(double a, double b, double c) { return __fma_rn(a, b, c); }
+__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
+
+// Tile of cs_acc_kernel<T>: F consecutive frequencies x CS_C channels l x CS_C channels m per CTA of CS_THREADS threads;
+// thread (fi, tl, tm) owns the RL x RM outputs l = l0 + tl + (CS_C / RL) i, m = m0 + tm + (CS_C / RM) j (strided, so that a
+// warp's shared-memory reads hit distinct banks).  Float64 owns half as many outputs per thread as Float32: its 16 complex
+// accumulators (partial and epoch sum of 4 x 2 outputs) and 6 operands fit the register file without spills.  The slabs of
+// CS_STAGES consecutive (epoch, taper) steps are in flight at once.
+constexpr int CS_C = 16, CS_THREADS = 256, CS_STAGES = 4;
+template <typename T> struct CsTile {
+    static constexpr int RL = 4, RM = sizeof(T) == 4 ? 4 : 2, TL = CS_C / RL, TM = CS_C / RM, F = CS_THREADS / (TL * TM);
+};
+
+// out[l, m, fi] over the g epochs of one group whose raw spectra x hold, for taper t, channel c of epoch e at column
+// e nchan + c of the t-th nout x (nchan g) slab.  With f = f_lo + fi, each taper adds the term c_f * x[f, l] * conj(x[f, m])
+// (rows pre-scaled by 1/sqrt(r_t), so the reference's weight 2/r_t and its 1/sqrt(2) on the DC / Nyquist rows become c_f =
+// 2, or 1 there), with the FMA placement of re = fma(a.x, b.x, a.y b.y), im = fma(a.y, b.x, -(a.x b.y)), tapers 0 .. K-1 in
+// order into the epoch's partial (the first assigns c_f (re, im), later ones add fma(c_f, re, p.x), fma(c_f, im, p.y)), and
+// the partials of the epochs in order into the epoch sum (in the output eltype).  fresh: the first epoch's partial is the
+// sum; else the sum continues from out.  divisor > 1: the sum's parts are then divided by it (the last group of E > 1
+// epochs).  Every (l, m) is computed: a mirrored triangle would carry the other FMA placement in its imaginary part.
+// The two frequency-by-channel slabs of each (epoch, taper) are loaded by cp.async, coalesced along frequency, into a ring of
+// CS_STAGES buffers, CS_STAGES - 1 steps ahead of the one being summed; each output is written once.  Block b: l tile b % ct, m tile (b / ct) % ct, frequency tile
+// b / ct^2 (ct = ceil(nchan / CS_C)), so the CTAs that share a slab run side by side.
 template <typename T>
-__global__ void cs_acc_kernel(cx<T>* __restrict__ out, const cx<T>* __restrict__ x, int64_t nout, int64_t nchan, int64_t f_lo,
-                              int64_t nf, int nyquist_row, int first) {
-    const int64_t total = nf * nchan * nchan;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t l = i % nchan, m = (i / nchan) % nchan, f = f_lo + i / (nchan * nchan);
-        const T c = (f == 0 || (nyquist_row && f == nout - 1)) ? T(1) : T(2);
-        const cx<T> a = x[f + l * nout], b = x[f + m * nout];
-        const cx<T> v = mkc<T>(c * (a.x * b.x + a.y * b.y), c * (a.y * b.x - a.x * b.y));
-        out[i] = first ? v : mkc<T>(out[i].x + v.x, out[i].y + v.y);
+__global__ void __launch_bounds__(CS_THREADS) cs_acc_kernel(cx<T>* __restrict__ out, const cx<T>* __restrict__ x, int64_t nout,
+                                                            int64_t nchan, int64_t g, int64_t ntapers, int64_t f_lo, int64_t nf,
+                                                            int nyquist_row, int fresh, int64_t divisor) {
+    using Tile = CsTile<T>;
+    constexpr int RL = Tile::RL, RM = Tile::RM, TL = Tile::TL, TM = Tile::TM, F = Tile::F, LD = F + 1;
+    __shared__ cx<T> slab[CS_STAGES][2][CS_C][LD];            // [buffer][l slab, m slab][channel][frequency], padded rows
+    const int64_t ct = (nchan + CS_C - 1) / CS_C, b = blockIdx.x;
+    const int64_t l0 = (b % ct) * CS_C, m0 = ((b / ct) % ct) * CS_C, fi0 = (b / (ct * ct)) * F;
+    const int tid = threadIdx.x, fi = tid / (TL * TM), tl = tid % TL, tm = (tid / TL) % TM;
+    // loads: thread tid copies frequency tid % F of channels tid / F (+ CS_THREADS / F) of both slabs
+    constexpr int LROWS = CS_THREADS / F;                     // channels per copy pass: CS_C (Float32) or 2 CS_C / 2 (Float64)
+    const int lf = tid % F, lc = tid / F;
+    const bool fin = fi0 + lf < nf;
+    const cx<T>* const src = x + (f_lo + fi0 + lf);
+    const int64_t tstride = nout * nchan * g;
+    int64_t ne = 0, nt = 0;                                   // the next (epoch, taper) to stage
+    auto stage = [&](int buf) {                               // one commit group per step, empty past the last step
+        if (ne < g) {
+            const int64_t off = nout * nchan * ne + tstride * nt;
+#pragma unroll
+            for (int c = lc; c < CS_C; c += LROWS) {
+                if (fin && l0 + c < nchan) cp_async<sizeof(cx<T>)>(&slab[buf][0][c][lf], src + off + nout * (l0 + c));
+                if (fin && m0 + c < nchan) cp_async<sizeof(cx<T>)>(&slab[buf][1][c][lf], src + off + nout * (m0 + c));
+            }
+            if (++nt == ntapers) { nt = 0; ++ne; }
+        }
+        cp_async_commit();
+    };
+    const int64_t f = f_lo + fi0 + fi;
+    const T cf = (f == 0 || (nyquist_row && f == nout - 1)) ? T(1) : T(2);
+    const bool fout = fi0 + fi < nf;
+    cx<T>* const o = out + nchan * nchan * (fi0 + fi);
+    cx<T> p[RL][RM], sum[RL][RM];
+    if (!fresh && fout) {
+#pragma unroll
+        for (int i = 0; i < RL; ++i)
+#pragma unroll
+            for (int j = 0; j < RM; ++j) {
+                const int64_t l = l0 + tl + TL * i, m = m0 + tm + TM * j;
+                if (l < nchan && m < nchan) sum[i][j] = o[l + nchan * m];
+            }
     }
+#pragma unroll
+    for (int k = 0; k < CS_STAGES - 1; ++k) stage(k);
+    int buf = 0;
+    for (int64_t e = 0; e < g; ++e) {
+        for (int64_t t = 0; t < ntapers; ++t) {
+            cp_async_wait<CS_STAGES - 2>();                   // this step's group has landed (this thread's copies) ...
+            __syncthreads();                                  // ... everyone's; and the buffer of the last step is free
+            stage(buf == 0 ? CS_STAGES - 1 : buf - 1);
+            cx<T> a[RL], bb[RM];
+#pragma unroll
+            for (int i = 0; i < RL; ++i) a[i] = slab[buf][0][tl + TL * i][fi];
+#pragma unroll
+            for (int j = 0; j < RM; ++j) bb[j] = slab[buf][1][tm + TM * j][fi];
+            if (t == 0) {
+#pragma unroll
+                for (int i = 0; i < RL; ++i)
+#pragma unroll
+                    for (int j = 0; j < RM; ++j) {
+                        const T re = fma_rn(a[i].x, bb[j].x, mul_rn(a[i].y, bb[j].y));
+                        const T im = fma_rn(a[i].y, bb[j].x, -mul_rn(a[i].x, bb[j].y));
+                        p[i][j] = mkc<T>(mul_rn(cf, re), mul_rn(cf, im));
+                    }
+            } else {
+#pragma unroll
+                for (int i = 0; i < RL; ++i)
+#pragma unroll
+                    for (int j = 0; j < RM; ++j) {
+                        const T re = fma_rn(a[i].x, bb[j].x, mul_rn(a[i].y, bb[j].y));
+                        const T im = fma_rn(a[i].y, bb[j].x, -mul_rn(a[i].x, bb[j].y));
+                        p[i][j] = mkc<T>(fma_rn(cf, re, p[i][j].x), fma_rn(cf, im, p[i][j].y));
+                    }
+            }
+            if (t + 1 == ntapers) {
+                const bool first = fresh && e == 0;
+#pragma unroll
+                for (int i = 0; i < RL; ++i)
+#pragma unroll
+                    for (int j = 0; j < RM; ++j)
+                        sum[i][j] = first ? p[i][j] : mkc<T>(sum[i][j].x + p[i][j].x, sum[i][j].y + p[i][j].y);
+            }
+            buf = buf + 1 == CS_STAGES ? 0 : buf + 1;
+        }
+    }
+    if (!fout) return;
+    const T d = (T)divisor;
+#pragma unroll
+    for (int i = 0; i < RL; ++i)
+#pragma unroll
+        for (int j = 0; j < RM; ++j) {
+            const int64_t l = l0 + tl + TL * i, m = m0 + tm + TM * j;
+            if (l < nchan && m < nchan) o[l + nchan * m] = divisor > 1 ? mkc<T>(sum[i][j].x / d, sum[i][j].y / d) : sum[i][j];
+        }
 }
 
 // coherence_from_cs!, src/multitaper.jl:672-693: |S_lm| / sqrt(real(S_ll * S_mm)) from the lower triangle, unit diagonal
@@ -1723,30 +1834,62 @@ template <class F> static int for_each_taper(SpecPlanImpl* p, F&& f) {
     return rc;
 }
 
-// mt_cross_power_spectra! / mt_coherence!, src/multitaper.jl:553-603, 722-790, device pointers; queues the work on st (the
-// caller waits for it: the plan's scratch is reused by the next call).  The spectra accumulate in `out`, or, for
-// coherence, in pipe.out[0], from which coherence_kernel writes `out`.
+static bool smooth7(int64_t v) {
+    for (int64_t q : {2, 3, 5, 7})
+        while (v % q == 0) v /= q;
+    return v == 1;
+}
+
+// Epochs per group of a multitaper cross-spectra call: the raw spectra of all tapers of a group's epochs (nout x nchan x K
+// per epoch) stay within MT_CROSS_SCRATCH bytes, and a group holds at least one epoch.
+static constexpr size_t MT_CROSS_SCRATCH = (size_t)1 << 30;
+static int64_t mt_cross_group(const SpecPlanImpl* p, int64_t nchan, int64_t nepochs) {
+    const size_t per_epoch = (size_t)(p->nout * nchan * p->ntapers) * (p->f64 ? 16 : 8);
+    const int64_t g = (int64_t)(MT_CROSS_SCRATCH / per_epoch);
+    return g < 1 ? 1 : (g < nepochs ? g : nepochs);
+}
+
+// mt_cross_power_spectra! / mt_coherence! of the epoch mean, src/multitaper.jl:553-603, 722-790, device pointers; queues the
+// work on st (the caller waits for it: the plan's scratch is reused by the next call).  signal is n_channels x n x nepochs.
+// Per group of epochs (mt_cross_group): cs_prep_kernel over its (channel, epoch) columns, one raw-spectra STFT call per
+// taper over those columns into the taper's slab of p->tmp (per_epoch: one per taper and epoch), and one cs_acc_kernel
+// launch, which sums every taper and epoch of the group into the spectra.  The spectra are written to `out`, or, for
+// coherence, to pipe.out[0], from which coherence_kernel writes `out`.
 template <typename T>
-static int mt_cross_run(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int demean, int64_t f_lo, int64_t nf,
-                        int coherence, void* out, cudaStream_t st) {
+static int mt_cross_run(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int64_t nepochs, int demean, int64_t f_lo,
+                        int64_t nf, int coherence, void* out, cudaStream_t st) {
     SpecPlanImpl* p = &plan->impl;
-    const int64_t n = p->n, cnt = nchan * nchan * nf;
-    DSP_TRY(p->pipe.in[1].reserve((size_t)(n * nchan) * sizeof(T)));
-    DSP_TRY(p->tmp.reserve((size_t)(p->nout * nchan) * sizeof(cx<T>)));
+    const int64_t n = p->n, cnt = nchan * nchan * nf, G = mt_cross_group(p, nchan, nepochs);
+    const int64_t ctiles = cdiv(nchan, CS_C), ctas = ctiles * ctiles * cdiv(nf, CsTile<T>::F);
+    // At odd or non-7-smooth cuFFT sizes a column's transform is not independent of its neighbours in the cuFFT batch (a
+    // 3-channel Float32 nfft 1031 call differed from the matrix calls when two epochs shared a batch), so each epoch is
+    // transformed by a call of its own, in the batch slots the matrix call gives it.
+    const bool per_epoch = !p->fused && (p->nfft % 2 != 0 || !smooth7(p->nfft));
+    DSP_REQUIRE(ctas <= INT32_MAX, "too many output tiles (%lld)", (long long)ctas);
+    DSP_TRY(p->pipe.in[1].reserve((size_t)(n * nchan * G) * sizeof(T)));
+    DSP_TRY(p->tmp.reserve((size_t)(p->nout * nchan * G * p->ntapers) * sizeof(cx<T>)));
     if (coherence) DSP_TRY(p->pipe.out[0].reserve((size_t)cnt * sizeof(cx<T>)));
     cx<T>* const cs = (cx<T>*)(coherence ? p->pipe.out[0].p : out);
-    cs_prep_kernel<T><<<(unsigned)nchan, 256, 0, st>>>((const T*)signal, nchan, n, demean, (T*)p->pipe.in[1].p);
-    DSP_LAUNCH_OK();
-    const int threads = 256;
-    const int grid = (int)(cdiv(cnt, threads) < device_sm_count() * 32 ? cdiv(cnt, threads) : device_sm_count() * 32);
-    DSP_TRY(for_each_taper(p, [&](int64_t t) -> int {
-        DSP_TRY(dspb200_stft_exec_dev(plan, p->pipe.in[1].p, n, nchan, 1.0, 0, p->tmp.p, st));     // raw spectra, nout x nchan
-        cs_acc_kernel<T><<<grid, threads, 0, st>>>(cs, (const cx<T>*)p->tmp.p, p->nout, nchan, f_lo, nf, (p->nfft % 2 == 0) ? 1 : 0,
-                                                   t == 0 ? 1 : 0);
+    for (int64_t e0 = 0; e0 < nepochs; e0 += G) {
+        const int64_t g = nepochs - e0 < G ? nepochs - e0 : G, cols = nchan * g;
+        cs_prep_kernel<T><<<(unsigned)cols, 256, 0, st>>>((const T*)signal + e0 * nchan * n, nchan, n, demean, (T*)p->pipe.in[1].p);
         DSP_LAUNCH_OK();
-        return DSPB200_OK;
-    }));
+        DSP_TRY(for_each_taper(p, [&](int64_t t) -> int {                  // raw spectra of taper t, nout x cols
+            cx<T>* const slab = (cx<T>*)p->tmp.p + t * p->nout * cols;
+            if (!per_epoch) return dspb200_stft_exec_dev(plan, p->pipe.in[1].p, n, cols, 1.0, 0, slab, st);
+            for (int64_t e = 0; e < g; ++e)
+                DSP_TRY(dspb200_stft_exec_dev(plan, (const T*)p->pipe.in[1].p + e * nchan * n, n, nchan, 1.0, 0,
+                                              slab + e * nchan * p->nout, st));
+            return DSPB200_OK;
+        }));
+        cs_acc_kernel<T><<<(unsigned)ctas, CS_THREADS, 0, st>>>(cs, (const cx<T>*)p->tmp.p, p->nout, nchan, g, p->ntapers, f_lo, nf,
+                                                               (p->nfft % 2 == 0) ? 1 : 0, e0 == 0 ? 1 : 0,
+                                                               e0 + g == nepochs ? nepochs : 1);
+        DSP_LAUNCH_OK();
+    }
     if (coherence) {
+        const int threads = 256;
+        const int grid = (int)(cdiv(cnt, threads) < device_sm_count() * 32 ? cdiv(cnt, threads) : device_sm_count() * 32);
         coherence_kernel<T><<<grid, threads, 0, st>>>((T*)out, cs, nchan, nf);
         DSP_LAUNCH_OK();
     }
@@ -2587,16 +2730,57 @@ static int mt_cross_check(dspb200_spec_plan* plan, const void* signal, int64_t n
     DSP_REQUIRE(nf == 0 || (signal && out), "NULL argument");
     return DSPB200_OK;
 }
-int dspb200_mt_cross_spectra_exec_dev(dspb200_spec_plan* plan, const void* d_signal, int64_t nchan, int demean, int64_t f_lo,
-                                      int64_t nf, int coherence, void* d_out, void* stream) {
-    DSP_RANGE("dspb200_mt_cross_spectra_exec_dev");
-    DSP_TRY(mt_cross_check(plan, d_signal, nchan, f_lo, nf, d_out));
+// The epoch form's checks on top of mt_cross_check: nepochs >= 1, every index and byte count of the signal and the output
+// inside DSPB200_INDEX_LIMIT, and (device form) an output that does not overlap the signal
+static int mt_cross_epochs_check(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int64_t nepochs, int64_t f_lo,
+                                 int64_t nf, int coherence, void* out, bool dev) {
+    DSP_TRY(mt_cross_check(plan, signal, nchan, f_lo, nf, out));
+    DSP_REQUIRE(nepochs >= 1, "n_epochs must be positive");
+    const SpecPlanImpl* p = &plan->impl;
+    const int64_t lim = DSPB200_INDEX_LIMIT / 16, esz = p->f64 ? 8 : 4;
+    DSP_REQUIRE(nchan <= INT32_MAX && p->n <= lim / nchan && nepochs <= lim / (nchan * p->n) &&
+                (nf == 0 || nchan <= lim / nchan / nf), "signal or output past DSPB200_INDEX_LIMIT");
+    if (dev) {
+        const size_t sbytes = (size_t)(nchan * p->n * nepochs * esz);
+        const size_t obytes = (size_t)(nchan * nchan * nf * esz * (coherence ? 1 : 2));
+        DSP_REQUIRE(!ranges_overlap(signal, sbytes, out, obytes), "out overlaps the signal");
+    }
+    return DSPB200_OK;
+}
+static int mt_cross_dev(dspb200_spec_plan* plan, const void* d_signal, int64_t nchan, int64_t nepochs, int demean, int64_t f_lo,
+                        int64_t nf, int coherence, void* d_out, void* stream) {
     if (nf == 0) return DSPB200_OK;
     SpecPlanImpl* p = &plan->impl;
     DSP_TRY(ensure_streams(p));
     cudaStream_t st = (cudaStream_t)stream;
-    return settle(st, p->f64 ? mt_cross_run<double>(plan, d_signal, nchan, demean, f_lo, nf, coherence, d_out, st)
-                             : mt_cross_run<float>(plan, d_signal, nchan, demean, f_lo, nf, coherence, d_out, st));
+    return settle(st, p->f64 ? mt_cross_run<double>(plan, d_signal, nchan, nepochs, demean, f_lo, nf, coherence, d_out, st)
+                             : mt_cross_run<float>(plan, d_signal, nchan, nepochs, demean, f_lo, nf, coherence, d_out, st));
+}
+int dspb200_mt_cross_spectra_exec_dev(dspb200_spec_plan* plan, const void* d_signal, int64_t nchan, int demean, int64_t f_lo,
+                                      int64_t nf, int coherence, void* d_out, void* stream) {
+    DSP_RANGE("dspb200_mt_cross_spectra_exec_dev");
+    DSP_TRY(mt_cross_check(plan, d_signal, nchan, f_lo, nf, d_out));
+    return mt_cross_dev(plan, d_signal, nchan, 1, demean, f_lo, nf, coherence, d_out, stream);
+}
+int dspb200_mt_cross_spectra_epochs(dspb200_spec_plan* plan, const void* d_signal, int64_t nchan, int64_t nepochs, int demean,
+                                    int64_t f_lo, int64_t nf, int coherence, void* d_out, void* stream) {
+    DSP_RANGE("dspb200_mt_cross_spectra_epochs");
+    DSP_TRY(mt_cross_epochs_check(plan, d_signal, nchan, nepochs, f_lo, nf, coherence, d_out, true));
+    return mt_cross_dev(plan, d_signal, nchan, nepochs, demean, f_lo, nf, coherence, d_out, stream);
+}
+// Host pointers: the signal is staged in pipe.in[0] and the result in pipe.out[1], which the device form does not use.
+int dspb200_mt_cross_spectra_epochs_exec(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int64_t nepochs, int demean,
+                                         int64_t f_lo, int64_t nf, int coherence, void* out) {
+    DSP_RANGE("dspb200_mt_cross_spectra_epochs_exec");
+    DSP_TRY(mt_cross_epochs_check(plan, signal, nchan, nepochs, f_lo, nf, coherence, out, false));
+    if (nf == 0) return DSPB200_OK;
+    SpecPlanImpl* p = &plan->impl;
+    DSP_TRY(ensure_streams(p));
+    HostPipe& hp = p->pipe;
+    const size_t esz = p->f64 ? 8 : 4, out_bytes = (size_t)(nchan * nchan * nf) * esz * (coherence ? 1 : 2);
+    return run_staged(hp.s_exec, {{signal, (size_t)(p->n * nchan * nepochs) * esz, &hp.in[0]}}, {{out, out_bytes, &hp.out[1]}}, [&] {
+        return dspb200_mt_cross_spectra_epochs(plan, hp.in[0].p, nchan, nepochs, demean, f_lo, nf, coherence, hp.out[1].p, hp.s_exec);
+    });
 }
 // Host pointers: the signal is staged in pipe.in[0] and the result in pipe.out[1], which the device form does not use.
 int dspb200_mt_cross_spectra_exec(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int demean, int64_t f_lo,

@@ -464,6 +464,15 @@ function mt_cross!(output::Array, signal::Matrix{T}, plan::Ptr{Cvoid}, demean::B
         plan, signal, size(signal, 1), demean, first(freq_inds) - 1, length(freq_inds), coherence, output))
     output
 end
+# An extension: the epoch mean over an n_channels x n_samples x n_epochs array (signal[:, :, e] is epoch e's matrix),
+# summed in epoch order in the output eltype and divided by n_epochs part by part.
+function mt_cross!(output::Array, signal::Array{T,3}, plan::Ptr{Cvoid}, demean::Bool, freq_inds::UnitRange{Int},
+                   coherence::Bool) where {T<:GPUReal}
+    GC.@preserve signal output check(ccall((:dspb200_mt_cross_spectra_epochs_exec, libdspb200), Cint,
+        (Ptr{Cvoid}, Ptr{Cvoid}, Int64, Int64, Cint, Int64, Int64, Cint, Ptr{Cvoid}),
+        plan, signal, size(signal, 1), size(signal, 3), demean, first(freq_inds) - 1, length(freq_inds), coherence, output))
+    output
+end
 
 # ---- filt!(buffer, ::FIRFilter{FIRArbitrary}, x), src/Filters/stream_filt.jl:579-625.  Output j of a call sits at total
 # phase acc + j*delta; the number of outputs and the carried state are computed in exact rational arithmetic

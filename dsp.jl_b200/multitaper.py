@@ -1,6 +1,7 @@
 """Multitaper spectral estimation front ends (SURVEY.md 8f rank 1; reference src/multitaper.jl:5-790), backed by
 libdspb200: `dpss`, `dpsseig`, `MTConfig`, `dpss_config`, `mt_pgram`, `MTSpectrogramConfig`, `mt_spectrogram`,
-`mt_spectrogram_` (`mt_spectrogram!`), `allocate_output`, `MTSpectrogramStream`, `mt_cross_power_spectra`, `mt_coherence`."""
+`mt_spectrogram_` (`mt_spectrogram!`), `allocate_output`, `MTSpectrogramStream`, `MTCrossSpectraConfig`, `MTCoherenceConfig`,
+`mt_cross_power_spectra`, `mt_cross_power_spectra_` (`mt_cross_power_spectra!`), `mt_coherence`, `mt_coherence_`."""
 import math
 
 import numpy as np
@@ -163,15 +164,6 @@ class MTSpectrogramConfig:
         k = arraysplit_count(int(n_samples), spw, n_overlap_samples)
         self.n_samples, self.n_overlap_samples, self.mt_config = int(n_samples), n_overlap_samples, mt
         self.time = (spw / 2 + hop * np.arange(k, dtype=np.float64)) / mt.fs
-
-
-def allocate_output(config):
-    """allocate_output(config::MTSpectrogramConfig), src/multitaper.jl:326-328: an uninitialised
-    length(freq) x length(time) matrix of the real eltype of the config, column-major."""
-    if not isinstance(config, MTSpectrogramConfig):
-        raise ArgumentError("allocate_output takes an MTSpectrogramConfig")
-    mt = config.mt_config
-    return np.empty((mt.freq.size, config.time.size), dtype=fftabs2type(mt.intype), order="F")
 
 
 def _mt_spectrogram_config(s, config, out):
@@ -377,42 +369,125 @@ class MTCrossSpectraConfig:
         self.freq = mt.freq[idx]
 
 
-def _cross(signal, config, kw, coherence):
+class MTCoherenceConfig:
+    """MTCoherenceConfig(cs_config::MTCrossSpectraConfig) / MTCoherenceConfig(n_channels, n_samples_or_mt_config; eltype,
+    fs, demean, freq_range, kwargs...), src/multitaper.jl:656-697: the coherence settings are those of the cross spectra
+    config `cs_config` (built from the arguments of MTCrossSpectraConfig when none is given)."""
+
+    def __init__(self, cs_config_or_n_channels, mt_config_or_n_samples=None, **kw):
+        if isinstance(cs_config_or_n_channels, MTCrossSpectraConfig):
+            if mt_config_or_n_samples is not None or kw:
+                raise ArgumentError("pass either an MTCrossSpectraConfig or the arguments of one")
+            self.cs_config = cs_config_or_n_channels
+        else:
+            self.cs_config = MTCrossSpectraConfig(cs_config_or_n_channels, mt_config_or_n_samples, **kw)
+
+    @property
+    def freq(self):
+        return self.cs_config.freq
+
+
+def allocate_output(config):
+    """allocate_output(config), src/multitaper.jl:326-328, 506-511, 682-686: an uninitialised column-major array of the
+    config's result: length(freq) x length(time) of the real eltype for an MTSpectrogramConfig, n_channels x n_channels x
+    length(freq) of the complex eltype for an MTCrossSpectraConfig and of the real eltype for an MTCoherenceConfig."""
+    if isinstance(config, MTSpectrogramConfig):
+        mt = config.mt_config
+        return np.empty((mt.freq.size, config.time.size), dtype=fftabs2type(mt.intype), order="F")
+    if isinstance(config, (MTCrossSpectraConfig, MTCoherenceConfig)):
+        cs = config if isinstance(config, MTCrossSpectraConfig) else config.cs_config
+        t = fftouttype(cs.mt_config.intype) if isinstance(config, MTCrossSpectraConfig) else fftabs2type(cs.mt_config.intype)
+        return np.empty((cs.n_channels, cs.n_channels, cs.nfreq), dtype=t, order="F")
+    raise ArgumentError("allocate_output takes an MTSpectrogramConfig, an MTCrossSpectraConfig or an MTCoherenceConfig")
+
+
+def _cross(signal, config, kw, coherence, out=None):
+    """Cross spectra (coherence False) or coherence of an n_channels x n_samples matrix or, an extension, of the epoch mean
+    of an n_channels x n_samples x n_epochs array (host or DeviceArray), into `out` (None: a new array; a DeviceArray for a
+    device signal, which it may not overlap).  Returns (result, freq)."""
     dev = isinstance(signal, DeviceArray)
     if not dev:
         signal = np.asarray(signal)
-    if signal.ndim != 2:
-        raise ArgumentError("expected an n_channels x n_samples matrix")
+    if signal.ndim not in (2, 3):
+        raise ArgumentError("expected an n_channels x n_samples matrix or an n_channels x n_samples x n_epochs array")
+    if isinstance(config, MTCoherenceConfig):
+        config = config.cs_config
     if config is None:
         config = MTCrossSpectraConfig(signal.shape[0], signal.shape[1], eltype=signal.dtype, **kw)
     elif kw:
         raise ArgumentError("pass either a config or keyword settings")
     mt = config.mt_config
-    if tuple(signal.shape) != (config.n_channels, mt.n_samples):
-        raise DimensionMismatch("Size of `signal` does not match `(config.n_channels, config.mt_config.n_samples)`")
+    if tuple(signal.shape[:2]) != (config.n_channels, mt.n_samples):
+        raise DimensionMismatch("Size of `signal` does not match `(config.n_channels, config.mt_config.n_samples)`; got "
+                                f"`size(signal)`={tuple(signal.shape)} but `(config.n_channels, config.mt_config.n_samples)`="
+                                f"{(config.n_channels, mt.n_samples)}")
+    shape = (config.n_channels, config.n_channels, config.nfreq)
+    if out is not None and tuple(out.shape) != shape:
+        raise DimensionMismatch(f"Size of `output` does not match `(config.n_channels, config.n_channels, "
+                                f"length(config.freq_inds))`; got `size(output)`={tuple(out.shape)} but {shape}")
+    nepochs = signal.shape[2] if signal.ndim == 3 else None
+    if nepochs == 0:
+        raise ArgumentError("n_epochs must be positive")
     if signal.dtype.kind == "c":
         raise ArgumentError("Only real data is supported (with the default choice of `onesided=true`) for this operation.")
     tout = fftabs2type(mt.intype) if coherence else fftouttype(mt.intype)
-    if dev:                                                           # device-resident (column-major) matrix: result stays in HBM
+    if out is not None:
+        if dev != isinstance(out, DeviceArray):
+            raise ArgumentError("the destination of a device signal is a DeviceArray, that of a host signal a host array")
+        if out.dtype != tout:
+            raise ArgumentError(f"Eltype of output ({out.dtype}) doesn't match the expected type: {tout}.")
+        if dev and out.overlaps(signal):
+            raise ArgumentError("the destination must not overlap the signal")
+    plan, args = mt.plan, (config.n_channels, config.demean, config.freq_lo, config.nfreq, coherence)
+    if dev:                                                           # device-resident (column-major) array: result stays in HBM
         if signal.dtype != mt.intype:
             raise ArgumentError(f"eltype of the device signal {signal.dtype} does not match the config's {mt.intype}")
-        dout = DeviceArray((config.n_channels, config.n_channels, config.nfreq), tout)
+        dout = DeviceArray(shape, tout) if out is None else out
         if config.nfreq:
-            mt.plan.cross_spectra_dev(signal.ptr, config.n_channels, config.demean, config.freq_lo, config.nfreq, coherence, dout.ptr)
+            if nepochs is None:
+                plan.cross_spectra_dev(signal.ptr, *args, dout.ptr)
+            else:
+                plan.cross_spectra_epochs_dev(signal.ptr, args[0], nepochs, *args[1:], dout.ptr)
         return dout, config.freq
     sig = np.asfortranarray(signal, dtype=mt.intype)                  # the reference's layout: channel index fastest
-    out = np.zeros((config.n_channels, config.n_channels, config.nfreq), dtype=tout, order="F")
+    res = np.zeros(shape, dtype=tout, order="F") if out is None or not out.flags.f_contiguous else out
     if config.nfreq:
-        mt.plan.cross_spectra(sig, config.n_channels, config.demean, config.freq_lo, config.nfreq, coherence, out)
-    return out, config.freq
+        if nepochs is None:
+            plan.cross_spectra(sig, *args, res)
+        else:
+            plan.cross_spectra_epochs(sig, args[0], nepochs, *args[1:], res)
+    if out is not None and res is not out:
+        out[...] = res
+    return (res if out is None else out), config.freq
 
 
 def mt_cross_power_spectra(signal, config=None, **kw):
     """mt_cross_power_spectra(signal; fs, demean, freq_range, kwargs...) / (signal, config), src/multitaper.jl:518-640;
-    signal is n_channels x n_samples."""
+    signal is n_channels x n_samples.  An extension: an n_channels x n_samples x n_epochs signal gives the mean over the
+    epochs of the cross spectra of its matrices signal[:, :, e] (demeaned per channel per epoch), summed in epoch order in
+    the output eltype and divided by n_epochs part by part; one epoch gives the matrix result bit for bit."""
     return CrossPowerSpectra(*_cross(signal, config, kw, False))
 
 
+def mt_cross_power_spectra_(out, signal, config=None, **kw):
+    """mt_cross_power_spectra!(output, signal; kwargs...) / (output, signal, config), src/multitaper.jl:551-585: the cross
+    spectra of a matrix or the epoch mean of a 3-D signal (see mt_cross_power_spectra) into `out`, n_channels x n_channels
+    x length(config.freq) (a DeviceArray for a device signal).  Returns the CrossPowerSpectra, whose power is `out`."""
+    if isinstance(config, MTCoherenceConfig):
+        raise ArgumentError("mt_cross_power_spectra_ takes an MTCrossSpectraConfig")
+    return CrossPowerSpectra(*_cross(signal, config, kw, False, out))
+
+
 def mt_coherence(signal, config=None, **kw):
-    """mt_coherence(signal; fs, demean, freq_range, kwargs...) / (signal, config), src/multitaper.jl:722-790."""
+    """mt_coherence(signal; fs, demean, freq_range, kwargs...) / (signal, config), src/multitaper.jl:722-790; config is an
+    MTCoherenceConfig or an MTCrossSpectraConfig.  A 3-D signal gives the coherence of the epoch-mean cross spectra."""
     return Coherence(*_cross(signal, config, kw, True))
+
+
+def mt_coherence_(out, signal, config=None, **kw):
+    """mt_coherence!(output, signal; kwargs...) / (output, signal, config::MTCoherenceConfig), src/multitaper.jl:756-778: the
+    coherences of a matrix or of the epoch mean of a 3-D signal into `out`, n_channels x n_channels x length(freq) of the
+    real eltype (a DeviceArray for a device signal).  Returns the Coherence, whose coherence is `out`."""
+    if config is not None and not isinstance(config, MTCoherenceConfig):
+        raise ArgumentError("mt_coherence_ takes an MTCoherenceConfig")
+    return Coherence(*_cross(signal, config, kw, True, out))

@@ -415,6 +415,25 @@ DSPB200_API int dspb200_mt_cross_spectra_exec(dspb200_spec_plan* plan, const voi
                                               int64_t f_lo, int64_t nf, int coherence, void* out);
 DSPB200_API int dspb200_mt_cross_spectra_exec_dev(dspb200_spec_plan* plan, const void* d_signal, int64_t nchan, int demean,
                                                   int64_t f_lo, int64_t nf, int coherence, void* d_out, void* stream);
+/* The same estimate over many epochs (trials), an extension: `signal` is n_channels x n_samples x nepochs (column-major:
+ * signal[:, :, e] is epoch e's matrix).  With M_e the cross spectra of dspb200_mt_cross_spectra_exec on epoch e (same plan,
+ * demean per channel per epoch, same [f_lo, f_lo+nf)), the cross spectra are S / nepochs with S = ((M_0 + M_1) + M_2) + ...
+ * summed in epoch order in the output eltype and each of its real and imaginary parts divided by nepochs (nepochs == 1: M_0,
+ * bit for bit the matrix call's result); coherence != 0 gives the coherence of that epoch-mean cross spectrum.  Each M_e is
+ * the taper sum of the matrix call, term for term.  Work: the epochs run in groups whose raw spectra (nout x n_channels x
+ * ntapers per epoch) fit 1 GiB, at least one epoch per group; per group one mean-removal launch, one raw-spectra STFT call
+ * per taper over all the group's (channel, epoch) columns (fused sizes: one launch; even 7-smooth cuFFT sizes: three launches
+ * per batch of the plan's cuFFT batch size; other cuFFT sizes, whose batched transforms couple neighbouring columns: one such
+ * call per taper and epoch, over that epoch's channels), and one accumulate launch that sums every taper and epoch of the
+ * group into each output element and writes it once; coherence adds one launch.  The matrix call is the nepochs == 1 case of this path.
+ * DSPB200_EINVALID before any launch: the matrix call's refusals, nepochs < 1, a signal or output past
+ * DSPB200_INDEX_LIMIT, and (device form) an output overlapping the signal.  nf == 0 launches nothing.
+ * dspb200_mt_cross_spectra_epochs takes device pointers and a cudaStream_t and returns after the work on that stream has
+ * completed; the _exec form copies `signal` in and `out` back. */
+DSPB200_API int dspb200_mt_cross_spectra_epochs(dspb200_spec_plan* plan, const void* d_signal, int64_t nchan, int64_t nepochs,
+                                                int demean, int64_t f_lo, int64_t nf, int coherence, void* d_out, void* stream);
+DSPB200_API int dspb200_mt_cross_spectra_epochs_exec(dspb200_spec_plan* plan, const void* signal, int64_t nchan, int64_t nepochs,
+                                                     int demean, int64_t f_lo, int64_t nf, int coherence, void* out);
 DSPB200_API int dspb200_spec_plan_destroy(dspb200_spec_plan* plan);
 
 /* ------------------------------------------------------------------------------------------ polyphase resample
