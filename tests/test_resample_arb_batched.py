@@ -8,7 +8,11 @@ A second CPU test replaces the device plan with a numpy model and checks the arg
 The main GPU check is exact.  Taps are integers in [-4, 4], samples integers in [-8, 8] (both parts for complex input),
 acc0 = 0 and delta a dyadic rational with two fractional bits, so every phase fraction alpha has two bits.  Each dot product
 is then an integer below 2^24 in magnitude and each output yu*alpha + yl a multiple of 1/4 below 2^22: exact in Float32.
-Every output must equal the float64 closed form bit for bit, whatever the tile, span or bank placement."""
+Every output must equal the float64 closed form bit for bit, whatever the tile, span or bank placement.
+
+These exact checks cover only acc0 = 0 and dyadic phases.  tests/test_resample_arb_kernel_paths.py checks every instance
+and entry point against exact phases for any acc0 and delta (non-dyadic rates, phases on and beside phase boundaries,
+j*delta past 2^31), within a proven phase bound; the checks here stay as the bit-exact special case."""
 import math
 from fractions import Fraction
 
