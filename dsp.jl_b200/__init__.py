@@ -16,6 +16,7 @@ the same thin layer over the same C ABI, include/dspb200.h):
     over an n_channels x n_samples x n_epochs signal)
                                                                        (src/multitaper.jl)
     hanning, hamming, rect, bartlett, kaiser, nextfastfft              (src/windows.jl, src/util.jl)
+    lpc, arburg, levinson, LPCBurg, LPCLevinson                        (src/lpc.jl)
 
 All numerics run in hand-written CUDA kernels inside libdspb200.so; there is no CPU fallback.
 The directory is named `dsp.jl_b200` (not importable as written), so it is loaded under the module
@@ -24,7 +25,7 @@ name `dspb200` by the shim `dspb200.py` at the repository root.
 from . import _lib
 from ._lib import DSPB200Error, device_count, launch_count
 from .device import DeviceArray, sync, to_device, to_host
-from .errors import ArgumentError, DimensionMismatch, DomainError, InexactError
+from .errors import ArgumentError, BoundsError, DimensionMismatch, DomainError, InexactError
 from .util import fftabs2type, fftintype, fftouttype, nextfastfft, rfftfreq, fftfreq
 from .windows import bartlett, hamming, hann, hanning, kaiser, rect
 from .dspbase import SMALL_FILT_CUTOFF, conv, conv_, filt, filt_, optimalfftfiltlength, os_fft_complexity
@@ -39,6 +40,7 @@ from .multitaper import (Coherence, CrossPowerSpectra, MTCoherenceConfig, MTConf
                          MTSpectrogramStream, allocate_output, dpss, dpss_config, dpsseig, mt_coherence, mt_coherence_,
                          mt_cross_power_spectra, mt_cross_power_spectra_, mt_pgram, mt_spectrogram, mt_spectrogram_)
 from .clients import alignsignals, filtfilt, finddelay, hilbert, shiftsignal, xcorr
+from .lpc import LPC_P_MAX, LPCBurg, LPCLevinson, arburg, levinson, lpc
 from . import device, filters, sharding
 
 __version__ = "0.1.0"

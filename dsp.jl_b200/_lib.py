@@ -78,6 +78,10 @@ SIGNATURES = {
     "dspb200_shift_async": (_int, [_int, _vp, _i64, _i64, _i64, _vp, _int, _vp, _i64, _vp]),
     "dspb200_scale_div_async": (_int, [_int, _vp, _i64, _dbl, _vp]),
     "dspb200_conv_fft_columns": (_int, [_int, _vp, _i64, _i64, _vp, _i64, _i64, _vp, _vp]),
+    "dspb200_lpc_work_bytes": (_int, [_int, _i64, _i64, _i64, _int, _int, C.POINTER(_i64)]),
+    "dspb200_lpc_burg_async": (_int, [_int, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _int, _vp]),
+    "dspb200_lpc_levinson_async": (_int, [_int, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp, _vp]),
+    "dspb200_levinson_async": (_int, [_int, _vp, _i64, _i64, _i64, _vp, _vp, _vp, _vp]),
     "dspb200_spec_plan_create": (_int, [_pp, _int, _i64, _i64, _i64, _int, _vp]),
     "dspb200_spec_plan_info": (_int, [_vp, C.POINTER(_i64), C.POINTER(_int)]),
     "dspb200_spec_nsegments": (_i64, [_vp, _i64]),
@@ -555,3 +559,26 @@ def scale_div_async(dtype, x_ptr, n, divisor, stream=0):
 def conv_fft_columns(dtype, u_ptr, nu, ncols, v_ptr, nv, nfft, out_ptr, stream=0):
     check(lib.dspb200_conv_fft_columns(np_dtype_code(np.dtype(dtype)), u_ptr, int(nu), int(ncols), v_ptr, int(nv), int(nfft),
                                        out_ptr, stream))
+
+
+def lpc_work_bytes(dtype, n, ncols, p, method, pin=0):
+    """Bytes of the workspace of lpc_burg_async (method 0) or lpc_levinson_async (method 1)."""
+    b = _i64(0)
+    check(lib.dspb200_lpc_work_bytes(np_dtype_code(np.dtype(dtype)), int(n), int(ncols), int(p), int(method), int(pin),
+                                     C.byref(b)))
+    return b.value
+
+
+def lpc_burg_async(dtype, x_ptr, n, ncols, p, a_ptr, err_ptr, refl_ptr, work_ptr, pin=0, stream=0):
+    check(lib.dspb200_lpc_burg_async(np_dtype_code(np.dtype(dtype)), x_ptr, int(n), int(ncols), int(p), a_ptr, err_ptr, refl_ptr,
+                                     work_ptr, int(pin), stream))
+
+
+def lpc_levinson_async(dtype, x_ptr, n, ncols, p, a_ptr, err_ptr, refl_ptr, work_ptr, stream=0):
+    check(lib.dspb200_lpc_levinson_async(np_dtype_code(np.dtype(dtype)), x_ptr, int(n), int(ncols), int(p), a_ptr, err_ptr,
+                                         refl_ptr, work_ptr, stream))
+
+
+def levinson_async(dtype, r_ptr, nr, ncols, p, a_ptr, err_ptr, refl_ptr, stream=0):
+    check(lib.dspb200_levinson_async(np_dtype_code(np.dtype(dtype)), r_ptr, int(nr), int(ncols), int(p), a_ptr, err_ptr, refl_ptr,
+                                     stream))

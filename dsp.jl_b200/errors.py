@@ -15,3 +15,7 @@ class InexactError(ValueError):
 
 class DimensionMismatch(ValueError):
     """Julia DimensionMismatch (e.g. src/periodograms.jl:255, 735-737)."""
+
+
+class BoundsError(IndexError):
+    """Julia BoundsError (e.g. levinson(r, p) with p >= length(r), src/lpc.jl:122-146)."""

@@ -455,6 +455,67 @@ shiftsignal!(::Type{T}, out::Ptr{Cvoid}, x::Ptr{Cvoid}, n::Integer, ncols::Integ
                 (Cint, Ptr{Cvoid}, Int64, Int64, Int64, Ptr{Int64}, Cint, Ptr{Cvoid}, Int64, Ptr{Cvoid}),
                 dtype_code(T), x, n, ncols, shift, shifts, negate, out, n, stream))
 
+# ---- lpc / arburg / levinson, src/lpc.jl.  UNTESTED: no `julia` in the build image, so none of this has been run.
+# Device-pointer forms (column-major n x ncols, a CuArray binding would pass raw pointers and its stream): each enqueues its
+# launches on `stream` and returns.  a is (p + 1) x ncols for Burg (arburg's, with the leading 1), p x ncols otherwise.
+lpc_work_bytes(::Type{T}, n::Integer, ncols::Integer, p::Integer, method::Integer; pin::Integer=0) where {T<:GPUNumber} =
+    (b = Ref{Int64}(0); check(ccall((:dspb200_lpc_work_bytes, libdspb200), Cint, (Cint, Int64, Int64, Int64, Cint, Cint, Ref{Int64}),
+                                    dtype_code(T), n, ncols, p, method, pin, b)); b[])
+arburg!(::Type{T}, a::Ptr{Cvoid}, err::Ptr{Cvoid}, refl::Ptr{Cvoid}, x::Ptr{Cvoid}, n::Integer, ncols::Integer, p::Integer,
+        work::Ptr{Cvoid}; pin::Integer=0, stream::Ptr{Cvoid}=C_NULL) where {T<:GPUNumber} =
+    check(ccall((:dspb200_lpc_burg_async, libdspb200), Cint,
+                (Cint, Ptr{Cvoid}, Int64, Int64, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Cint, Ptr{Cvoid}),
+                dtype_code(T), x, n, ncols, p, a, err, refl, work, pin, stream))
+lpc_levinson!(::Type{T}, a::Ptr{Cvoid}, err::Ptr{Cvoid}, refl::Ptr{Cvoid}, x::Ptr{Cvoid}, n::Integer, ncols::Integer, p::Integer,
+              work::Ptr{Cvoid}; stream::Ptr{Cvoid}=C_NULL) where {T<:GPUNumber} =
+    check(ccall((:dspb200_lpc_levinson_async, libdspb200), Cint,
+                (Cint, Ptr{Cvoid}, Int64, Int64, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+                dtype_code(T), x, n, ncols, p, a, err, refl, work, stream))
+levinson!(::Type{T}, a::Ptr{Cvoid}, err::Ptr{Cvoid}, refl::Ptr{Cvoid}, r::Ptr{Cvoid}, nr::Integer, ncols::Integer, p::Integer;
+          stream::Ptr{Cvoid}=C_NULL) where {T<:GPUNumber} =
+    check(ccall((:dspb200_levinson_async, libdspb200), Cint,
+                (Cint, Ptr{Cvoid}, Int64, Int64, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+                dtype_code(T), r, nr, ncols, p, a, err, refl, stream))
+
+# Host vectors: staged through device buffers from dspb200_malloc, computed, copied back after one synchronisation.
+function _dev(bytes::Integer)
+    p = Ref{Ptr{Cvoid}}(C_NULL)
+    check(ccall((:dspb200_malloc, libdspb200), Cint, (Ref{Ptr{Cvoid}}, Csize_t), p, max(bytes, 16)))
+    p[]
+end
+_free(p::Ptr{Cvoid}) = ccall((:dspb200_free, libdspb200), Cint, (Ptr{Cvoid},), p)
+_h2d(d::Ptr{Cvoid}, h::Array) = GC.@preserve h check(ccall((:dspb200_memcpy_h2d, libdspb200), Cint,
+    (Ptr{Cvoid}, Ptr{Cvoid}, Csize_t, Ptr{Cvoid}), d, h, sizeof(h), C_NULL))
+_d2h(h::Array, d::Ptr{Cvoid}) = GC.@preserve h check(ccall((:dspb200_memcpy_d2h, libdspb200), Cint,
+    (Ptr{Cvoid}, Ptr{Cvoid}, Csize_t, Ptr{Cvoid}), h, d, sizeof(h), C_NULL))
+_sync() = check(ccall((:dspb200_stream_sync, libdspb200), Cint, (Ptr{Cvoid},), C_NULL))
+
+function _lpc_host(x::Vector{T}, p::Integer, method::Symbol) where {T<:GPUNumber}
+    n = length(x)
+    method === :burg ? (0 <= p <= n || throw(ArgumentError("arburg needs 0 <= p <= length(x)"))) :
+                       (1 <= p <= n - 1 || throw(BoundsError(x, p + 1)))
+    na = method === :burg ? p + 1 : p
+    a, err, refl = Vector{T}(undef, na), Vector{real(T)}(undef, 1), Vector{T}(undef, p)
+    wb = method === :levinson_r ? 0 : lpc_work_bytes(T, n, 1, p, method === :burg ? 0 : 1)
+    dx, da, de, dr, dw = _dev(sizeof(x)), _dev(sizeof(a)), _dev(sizeof(err)), _dev(sizeof(refl)), _dev(wb)
+    try
+        _h2d(dx, x)
+        method === :burg ? arburg!(T, da, de, dr, dx, n, 1, p, dw) :
+        method === :levinson ? lpc_levinson!(T, da, de, dr, dx, n, 1, p, dw) : levinson!(T, da, de, dr, dx, n, 1, p)
+        _d2h(a, da); _d2h(err, de); _d2h(refl, dr); _sync()
+    finally
+        foreach(_free, (dx, da, de, dr, dw))
+    end
+    return a, err[1], refl
+end
+arburg(x::Vector{T}, p::Integer) where {T<:GPUNumber} = _lpc_host(x, p, :burg)
+levinson(r::Vector{T}, p::Integer) where {T<:GPUNumber} = _lpc_host(r, p, :levinson_r)
+function lpc(x::Vector{T}, p::Integer, ::DSP.LPC.LPCBurg) where {T<:GPUNumber}
+    a, err, _ = _lpc_host(x, p, :burg)
+    return a[2:end], err
+end
+lpc(x::Vector{T}, p::Integer, ::DSP.LPC.LPCLevinson) where {T<:GPUNumber} = _lpc_host(x, p, :levinson)[1:2]
+
 # ---- mt_cross_power_spectra! / mt_coherence!, src/multitaper.jl:553-603, 722-790.  `plan` is a multitaper plan built
 # with dspb200_mt_plan_create from config.mt_config (tapers pre-scaled by 1/sqrt(r_t)); validation stays in DSP.jl.
 function mt_cross!(output::Array, signal::Matrix{T}, plan::Ptr{Cvoid}, demean::Bool, freq_inds::UnitRange{Int},
@@ -619,6 +680,10 @@ function install_overlay!()
             DSP.mt_pgram(s::Vector{$T}; kw...) = mt_pgram(s; kw...)
             DSP.mt_pgram(s::Matrix{$T}; kw...) = mt_pgram(s; kw...)
             DSP.mt_spectrogram(s::Matrix{$T}, n::Int, noverlap::Int; kw...) = mt_spectrogram(s, n, noverlap; kw...)
+            DSP.LPC.arburg(x::Vector{$T}, p::Integer) = arburg(x, p)
+            DSP.LPC.levinson(r::Vector{$T}, p::Integer) = levinson(r, p)
+            DSP.LPC.lpc(x::Vector{$T}, p::Integer, m::DSP.LPC.LPCBurg) = lpc(x, p, m)
+            DSP.LPC.lpc(x::Vector{$T}, p::Integer, m::DSP.LPC.LPCLevinson) = lpc(x, p, m)
         end
     end
     for T in (Float32, Float64)

@@ -230,6 +230,39 @@ DSPB200_API int dspb200_scale_div_async(int dtype, void* x, int64_t n, double di
 DSPB200_API int dspb200_conv_fft_columns(int dtype, const void* d_u, int64_t nu, int64_t ncols, const void* d_v, int64_t nv,
                                          int64_t nfft, void* d_out, void* stream);
 
+/* ------------------------------------------------------------------------------------------ linear prediction
+ * arburg / lpc / levinson (src/lpc.jl) of every column of an n x ncols column-major matrix.  The *_async conventions above:
+ * device pointers, every launch on `stream`, no synchronisation, capturable in a CUDA graph.  Outputs: a, err (ncols, in the
+ * real eltype: F32 for F32 and C32) and refl (NULL: not wanted), in dtype, one column per input column.
+ * Everything but the reductions follows src/lpc.jl operation by operation in dtype (muladd = one fma for reals, Base.muladd
+ * for complex; every other operation rounded).  The reductions dot(x, x), dot(eb, ef) and the autocorrelation lags run in
+ * one fixed order that depends only on their length: tiles of 1024 indices, in a tile 256 lanes (index i in lane i % 256)
+ * each a muladd chain in increasing index from +0, then lanes l + h into l for h = 16 .. 1 inside each warp and warps
+ * w + h into w for h = 4, 2, 1; tile sums added pairwise, adjacent first, an odd last one carried.  dot(x, x) is the real
+ * sum of |x_i|^2 (fma(re, re, .), then fma(im, im, .)).  The result does not depend on ncols, the column's position, the
+ * path or the stream.
+ * DSPB200_EINVALID, before any launch: a NULL required buffer, a negative size, p outside the call's range, an output
+ * overlapping an input, the workspace or another output, a size past DSPB200_INDEX_LIMIT.  p > 1024 (LPC_P_MAX):
+ * DSPB200_EUNSUPPORTED.  ncols == 0 launches nothing. */
+/* Bytes of `work` for dspb200_lpc_burg_async (method 0, with its pin) or dspb200_lpc_levinson_async (method 1). */
+DSPB200_API int dspb200_lpc_work_bytes(int dtype, int64_t n, int64_t ncols, int64_t p, int method, int pin, int64_t* bytes);
+/* arburg(x, p), 0 <= p <= n: a is (p + 1) x ncols with a[0] = 1, conjugated as arburg returns it; lpc(x, p, LPCBurg()) is
+ * rows 1 .. p.  One launch.  Path, from n alone: one CTA per column with the errors in shared memory when
+ * 4 n sizeof(dtype) <= 192 KiB, else a cluster of min(8, ceil(n / 65536)) CTAs per column with the errors in `work` (one
+ * HBM pass and one cluster barrier per order).  pin is a testing aid: 0 the rule above, -1 the shared-memory path
+ * (DSPB200_EUNSUPPORTED where it does not fit), 1 .. 8 the streamed path with that many CTAs per column. */
+DSPB200_API int dspb200_lpc_burg_async(int dtype, const void* x, int64_t n, int64_t ncols, int64_t p, void* a, void* err,
+                                       void* refl, void* work, int pin, void* stream);
+/* lpc(x, p, LPCLevinson()), 1 <= p <= n - 1: the biased autocorrelation at lags 0 .. p as a direct sum
+ * r[k] = sum_i x[i + k] conj(x[i]) (the order above) divided by n as dspb200_scale_div_async divides, then levinson.  a and
+ * refl are p x ncols.  Two launches. */
+DSPB200_API int dspb200_lpc_levinson_async(int dtype, const void* x, int64_t n, int64_t ncols, int64_t p, void* a, void* err,
+                                           void* refl, void* work, void* stream);
+/* levinson(r, p) of every column of r (nr x ncols), 1 <= p <= nr - 1; a and refl are p x ncols.  dotu is the in-order
+ * muladd chain; the first k of a complex r is Smith's division.  One launch. */
+DSPB200_API int dspb200_levinson_async(int dtype, const void* r, int64_t nr, int64_t ncols, int64_t p, void* a, void* err,
+                                       void* refl, void* stream);
+
 /* ------------------------------------------------------------------------------------------ Welch / STFT
  * One plan per (dtype, n, noverlap, nfft, onesided, window): the analogue of WelchConfig
  * (src/periodograms.jl:516-576) = ArraySplit segmenter (:32-73) + forward_plan (:511-514) + fft2pow! (:142-172)
